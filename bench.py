@@ -88,6 +88,15 @@ def cpu_arm_step(orc, q, c, k):
   return orc.brute_force_torch(q, c, k, chunk=512)
 
 
+def dump_topk(dirname, np, scores, indices):
+  """The [Q, k] result of the last timed step as a caller receives it: DIR/topk_scores.npy (float32) and
+  DIR/topk_indices.npy (float64, exact for indices < 2^53).  The inputs are seeded, so two builds run with the same
+  arguments can be compared output for output."""
+  os.makedirs(dirname, exist_ok=True)
+  np.save(os.path.join(dirname, "topk_scores.npy"), np.asarray(scores, dtype=np.float32))
+  np.save(os.path.join(dirname, "topk_indices.npy"), np.asarray(indices).astype(np.float64))
+
+
 def gen_corpus_block(torch, dev, b0, rows, d):
   """The synthetic corpus is defined block-wise (1M-row blocks, seed 1 + first row): every rank and the oracle leg
   regenerate exactly the same rows."""
@@ -144,9 +153,11 @@ def run_reference(args):
     cpu_arm_step(orc, qs, c, k)
   t0 = time.perf_counter()
   for _ in range(args.steps):
-    cpu_arm_step(orc, qs, c, k)
+    out = cpu_arm_step(orc, qs, c, k)
   dt = time.perf_counter() - t0
   value = sample_q * args.steps / dt
+  if args.dump_outputs:
+    dump_topk(args.dump_outputs, np, out[0], out[1])
   world = int(os.environ.get("WORLD_SIZE", "1"))
   line = {
       "impl": "reference", "metric": METRIC, "value": value, "unit": "queries/s", "n_gpus": args.gpus, "steps": args.steps,
@@ -178,6 +189,9 @@ def main():
   ap.add_argument("--no-secondary", action="store_true", help="skip the gather / Adagrad / training-step figures")
   ap.add_argument("--no-cpu-baseline", action="store_true")
   ap.add_argument("--no-tensor-cores", action="store_true", help="force the exact CUDA-core path (debug)")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="write what the last timed step returned (top-K scores, float32; indices, float64) as DIR/<name>.npy; "
+                       "with --impl reference, the CPU arm's result for its query sample")
   args = ap.parse_args()
   args.warmup = max(args.warmup, 3)
   if args.impl == "reference":
@@ -254,6 +268,8 @@ def main():
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
   ms_total = float(ms)
   value = Q * args.steps / (ms_total * 1e-3)
+  if args.dump_outputs and rank == 0:   # 4096 x 100 x 12 bytes at cfg2
+    dump_topk(args.dump_outputs, np, out[0].float().cpu().numpy(), out[1].cpu().numpy())
 
   # ---------------- end-to-end through the public API with host buffers (`e2e`) ----------------
   # Every step copies ITS queries from pinned host memory and brings ITS [Q,k] result back to pinned host memory.  The
@@ -343,17 +359,19 @@ def main():
       layer(query_batches[st % NQ])
     stage_ms, calls = ops.profile_read()
     ops.profile_enable(False)
-    peak = peaks.get("bf16_tflops", 1590.0)
-    which = "measured bf16_tflops (burst; the filter pass is timed alone)" if "bf16_tflops" in peaks else "fallback 1590"
+    peak = peaks.get("bf16_tflops", 989.0)
+    which = ("measured bf16_tflops (burst; the filter pass is timed alone)" if "bf16_tflops" in peaks else
+             "H100 SXM data sheet, dense FP16/BF16 at 700 W (not reached: a bound)")
     n_local = corpus_local.shape[0]
     flops = 2.0 * Q * n_local * d  # algorithmic: 2*Q*N*d per launch (SURVEY 8d: 128 MFLOP/query at N=1M,d=64)
     t_filter = stage_ms[2] / max(calls, 1) * 1e-3
     achieved = flops / t_filter / 1e12
     roofline = {"bound": "tensor", "kernel": "tc_scan_kernel<FILTER>", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                 "frac": achieved / peak, "peak_source": which,
-                # dram__bytes_read.sum + dram__bytes_write.sum of this kernel, per launch, from the committed ncu
-                # --set full capture (profiles/, see profiles/README.md); only for the cfg2 single-GPU shape
-                "traffic": TRAFFIC_CFG2_FILTER if (args.workload == "cfg2" and world == 1) else None, "traffic_unit": "bytes/launch",
+                # algorithmic bytes of one call: the filter pass streams the fp16 corpus image, the call reads the fp32
+                # queries and writes the [Q, k] (score, index) result; the survivor records the filter pass writes and
+                # the finalize step reads back are not counted
+                "traffic": n_local * d * 2 + Q * d * 4 + Q * k * 12, "traffic_unit": "bytes/launch (algorithmic)",
                 "whole_call_frac": (flops / (ms_total / args.steps * 1e-3) / 1e12) / peak,
                 "stage_ms_per_call": {"qprep": stage_ms[0] / calls, "sample_pass+threshold": stage_ms[1] / calls,
                                       "filter_pass": stage_ms[2] / calls, "rescore+finalize": stage_ms[3] / calls}}
@@ -402,11 +420,11 @@ def main():
     line = {
         "metric": METRIC, "value": value, "unit": "queries/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-        "dtype": "f32 (fp16 tcgen05 screening, fp32 accumulate + exact fp32 re-scoring)" if used_tc else "f32",
+        "dtype": "f32 (fp16 wgmma screening, fp32 accumulate + exact fp32 re-scoring)" if used_tc else "f32",
         "data": "synthetic",
         "config": {"workload": workload_string(args.workload, N, d, Q, k, world),
-                   "path": "tcgen05 screening + exact rescoring" if used_tc else "exact CUDA-core scan",
-                   "l2": "inputs (fp16 image 128 MB + fp32 corpus 256 MB per 1M rows) exceed the 126 MB L2 between steps; "
+                   "path": "wgmma screening + exact rescoring" if used_tc else "exact CUDA-core scan",
+                   "l2": "inputs (fp16 image 128 MB + fp32 corpus 256 MB per 1M rows) exceed the 50 MB L2 between steps; "
                          f"{NQ} query batches rotate",
                    "parallelism": f"corpus-shard x{world}",
                    "collective": (None if world == 1 else
@@ -434,11 +452,6 @@ def main():
   return 0
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of tc_scan_kernel<FILTER> at cfg2 on one GPU, per launch
-# (ncu --set full, profiles/r02_tc_scan_metrics.csv: 132.87 MB read + 31.38 MB written)
-TRAFFIC_CFG2_FILTER = 164.25e6
-
-
 def _time_ms(torch, fn, iters=20, warm=3):
   for _ in range(warm):
     fn()
@@ -455,7 +468,7 @@ def _time_ms(torch, fn, iters=20, warm=3):
 def secondary_figures(torch, tfrs, ops, dev, peaks):
   """HBM GB/s of the embedding gather (the second half of BASELINE.json's metric: cfg5 and cfg3 shapes, uniform and
   Zipf ids) and the sparse-Adagrad / in-batch-softmax times of a cfg3 training step.  Algorithmic bytes per SURVEY 8d."""
-  hbm = peaks.get("hbm_gbs", 6650.0)
+  hbm = peaks.get("hbm_gbs", 3350.0)
   out = {}
   g = torch.Generator(device=dev); g.manual_seed(7)
   # cfg5: 26 tables [1M, 32], B = 65536 -> [B, 845 (ld 848)]
@@ -479,7 +492,7 @@ def secondary_figures(torch, tfrs, ops, dev, peaks):
       fn()
     return _time_ms(torch, gr.replay)
 
-  out["gather"] = {"hbm_peak_gbs": hbm, "peak_source": "measured hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650",
+  out["gather"] = {"hbm_peak_gbs": hbm, "peak_source": "measured hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet 3350 GB/s",
                    "timing": "CUDA-graph replays of one tfrs_gather_f32 call (device time; 4 id sets rotate for the uniform case)"}
   id_sets = [[torch.randint(0, 1_000_000, (65536,), generator=g, device=dev, dtype=torch.int32) for _ in range(26)] for _ in range(4)]
   ms5 = sum(graph_ms(lambda ids=ids: ops.gather(tables, ids, out=act)) for ids in id_sets) / len(id_sets)

@@ -1,5 +1,5 @@
 /*
- * tfrs_b200.h -- C ABI of libtfrs_b200.so: the B200 (sm_100a) kernels behind the TensorFlow
+ * tfrs_b200.h -- C ABI of libtfrs_b200.so: the H100 (sm_90a) kernels behind the TensorFlow
  * Recommenders retrieval / ranking hot path.
  *
  * The reference (tensorflow/recommenders v0.7.7) has no native/FFI layer: its boundary with native
@@ -70,9 +70,9 @@ int tfrs_gather_f32(const float* const* tables, const int64_t* rows, const int32
  *
  * tfrs_topk_scan_f32      exact fp32 CUDA-core path (any N, d; used for small corpora/chunks).
  * tfrs_index_*            builds the tensor-core screening image of a corpus (fp16 after an exact
- *                         power-of-two rescale, UMMA SWIZZLE_128B K-major tiles + row-norm bound);
+ *                         power-of-two rescale, GMMA SWIZZLE_128B K-major tiles + row-norm bound);
  *                         done once at index() time (BruteForce.index, factorized_top_k.py:540-584).
- * tfrs_topk_tc_f32        tcgen05 screening GEMM (fp16 in / fp32 accumulate in TMEM) with a fused
+ * tfrs_topk_tc_f32        wgmma screening GEMM (fp16 in / fp32 accumulate in registers) with a fused
  *                         threshold filter, then exact fp32 rescoring of the survivors -- same
  *                         bit-exact result as tfrs_topk_scan_f32.  Needs d <= 128, k <= 256 and a
  *                         corpus of at least ~256*k rows (tfrs_topk_tc_workspace_bytes returns 0
@@ -235,7 +235,7 @@ int tfrs_inbatch_softmax_bwd(const float* q, const float* c, int64_t B, int64_t 
                              void* stream);
 
 /* K3 forward on the tensor cores (same contract and outputs as tfrs_inbatch_softmax_fwd; d <= 128):
- * hi/lo fp16 split of q and c (|err| <= 2^-21 |q||c| on a score), tcgen05 GEMM with fp32 TMEM accumulation and
+ * hi/lo fp16 split of q and c (|err| <= 2^-21 |q||c| on a score), wgmma GEMM with fp32 register accumulation and
  * an online log-sum-exp epilogue -- the [B,C] logits are never written.  `candidate_bias` (nullable, [C]) is added
  * to every logit of its column after the temperature: with bias_j = -log(clip(p_j, 1e-6, 1)) it is the
  * sampling-probability correction of tasks/retrieval.py:190-192 / layers/loss.py:150-158.  Returns TFRS_ERR_UNSUPPORTED
@@ -246,8 +246,8 @@ int tfrs_inbatch_softmax_tc_fwd(const float* q, const float* c, int64_t B, int64
                                 float* loss, float* lse, void* ws, size_t ws_bytes, void* stream);
 
 /* K3b on the tensor cores (same contract and outputs as tfrs_inbatch_softmax_bwd; d <= 64): two launches of one
- * flash-attention-backward-shaped kernel -- S = X.Y^T (tcgen05, split fp16 operands), G built from TMEM by the
- * epilogue warps and written back over S (tcgen05.st), dX += G.Y with G read from TMEM and the Y tile as an MN-major
+ * flash-attention-backward-shaped kernel -- S = X.Y^T (wgmma, split fp16 operands), G built on the register
+ * fragment of S, dX += G.Y with G as the register A operand of the next wgmma and the Y tile as an MN-major
  * operand; X = q gives dq, X = c gives dc.  Deterministic (no atomics).  workspace_bytes == 0 / TFRS_ERR_UNSUPPORTED
  * outside its range. */
 size_t tfrs_inbatch_softmax_tc_bwd_workspace_bytes(int64_t B, int64_t C, int d);
@@ -325,8 +325,8 @@ int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* W, const fl
                        int64_t B, int D, int64_t ld, float diag_scale, float* dx0, float* dx, float* dW,
                        float* dbias, void* ws, size_t ws_bytes, void* stream);
 
-/* K5 on the tensor cores (forward): the same cross formula as tfrs_cross_fwd_f32, computed as one tcgen05
- * GEMM on exactly-rescaled fp16 hi/lo splits of x and W (3 MMAs per K step, fp32 accumulation in TMEM;
+/* K5 on the tensor cores (forward): the same cross formula as tfrs_cross_fwd_f32, computed as one wgmma
+ * GEMM on exactly-rescaled fp16 hi/lo splits of x and W (3 MMAs per K step, fp32 accumulation in registers;
  * ~2^-21 relative error, inside the 1e-5 bar) with the formula fused in the epilogue.
  * tfrs_cross_tc_weight_build turns W [D,D] ([in,out]) into the K-major image of W^T; rebuild it whenever
  * W changes.  `ws` holds the per-call image of x. */
@@ -344,7 +344,7 @@ int tfrs_cross_tc_fwd_ex_f32(const float* x0, const float* x, const void* wbuf, 
                              unsigned int* out_amax_bits, void* ws, size_t ws_bytes, void* stream);
 
 /* K5b with both GEMMs on the tensor cores (same contract and outputs as tfrs_cross_bwd_f32): dx = gp.W^T + diag*gp + g
- * and dW = x^T.gp as split-fp16 tcgen05 GEMMs (dW accumulates the batch in chunks of 1024 rows, partials summed in
+ * and dW = x^T.gp as split-fp16 wgmma GEMMs (dW accumulates the batch in chunks of 1024 rows, partials summed in
  * fixed order); gp = g*x0, dx0 = g*prod and dbias = colsum(gp) as in the exact path.  Deterministic. */
 size_t tfrs_cross_tc_bwd_workspace_bytes(int64_t B, int D);
 int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const float* W, const float* prod, const float* dout,
@@ -362,7 +362,7 @@ int tfrs_gemm_tc_f32(int transA, int transB, int64_t M, int64_t N, int64_t K, co
 /* Low-rank DCN-v2 cross layer on the tensor cores (layers/feature_interaction/dcn.py:131-148,178-179 `projection_dim`;
  * the layer of MultiLayerDCN, multi_layer_dcn.py:146-148):
  *   t = x . U  [B,p] ;  out = x0 * (t . V + bias + diag_scale * x) + x       U [D,p], V [p,D] in Keras [in,out] layout
- * Two tcgen05 GEMMs; the cross formula is the epilogue of the second one (no [B,D] product round trip).  `t` (required)
+ * Two wgmma GEMMs; the cross formula is the epilogue of the second one (no [B,D] product round trip).  `t` (required)
  * and `prod` (nullable) are kept for the backward pass:
  *   gp = g*x0 ; dx0 = g*prod ; dt = gp.V^T ; dV = t^T.gp ; dU = x^T.dt ; dx = dt.U^T + diag_scale*gp + g ; dbias = colsum(gp)
  * -- four tensor-core GEMMs, deterministic.  D, p <= 1024.  dx0 / dx / dU / dV / dbias are nullable. */

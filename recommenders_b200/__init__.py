@@ -1,4 +1,4 @@
-"""recommenders_b200 -- a B200-native (sm_100a) implementation of the TensorFlow Recommenders retrieval /
+"""recommenders_b200 -- an H100-native (sm_90a) implementation of the TensorFlow Recommenders retrieval /
 ranking hot path behind the reference's own API surface:
 
     import recommenders_b200 as tfrs

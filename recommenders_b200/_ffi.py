@@ -109,7 +109,7 @@ def lib() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
       raise RuntimeError(
           f"libtfrs_b200.so not found at {LIB_PATH}. Build it with `python -m recommenders_b200.build` "
-          "(nvcc, sm_100a). There is no CPU fallback.")
+          "(nvcc, sm_90a). There is no CPU fallback.")
     l = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in _SIGNATURES.items():
       fn = getattr(l, name)  # AttributeError if the symbol is missing: fail loudly

@@ -17,11 +17,11 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int sm_count() {
   static int cached[64] = {};
   int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int& c = cached[dev & 63];
   if (!c) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) c = n;
-    else return 148;
+    else return 132;
   }
   return c;
 }

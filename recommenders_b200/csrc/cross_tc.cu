@@ -1,19 +1,19 @@
 // cross_tc.cu -- K5 on the tensor cores: DCN-v2 cross layer forward (layers/feature_interaction/dcn.py:176-186)
 //   out = x0 * (x . W + bias + diag_scale * x) + x        W [D,D] in Keras [in,out] layout
-// as ONE tcgen05 GEMM with the whole cross formula in the epilogue.
+// as ONE wgmma GEMM with the whole cross formula in the epilogue.
 //
 // fp32 parity on fp16 tensor cores: each operand is rescaled by an exact power of two and split into
 //   v = hi + lo,  hi = fp16(v), lo = fp16(v - hi)            (|v - hi - lo| <= 2^-22 |v|)
-// and the product is accumulated in fp32 (TMEM) as  hi_x*hi_w + lo_x*hi_w + hi_x*lo_w  (the dropped
+// and the product is accumulated in fp32 (registers) as  hi_x*hi_w + lo_x*hi_w + hi_x*lo_w  (the dropped
 // lo*lo term is 2^-22 relative), i.e. 3 MMAs per K step -- ~2^-21 relative error, inside the 1e-5 bar.
 //
-// Layout: x (per call) and W^T (once per weight version) are turned into UMMA SWIZZLE_128B K-major tile
+// Layout: x (per call) and W^T (once per weight version) are turned into GMMA SWIZZLE_128B K-major tile
 // images, 128 rows x 64 K-elements per 16 KB block, hi block then lo block per K slab (32 KB per slab).
-// Kernel: persistent CTAs (1/SM, 640 threads) over (256-row block, 128-column tile) pairs; per K slab a
-// bulk-TMA stage brings 2x(hi,lo) A blocks + (hi,lo) of W^T (96 KB); 24 MMAs (2 A blocks x 3 products x 4
-// K16 steps) accumulate into a 128-column TMEM buffer per A block (2 buffers -> next tile's MMAs overlap the
-// epilogue).  16 epilogue warps read 64 columns of one row each, fetch x0 / x / bias, apply the formula and
-// store fp32.
+// Kernel: persistent CTAs (1/SM, 544 threads) over (256-row block, 128-column tile) pairs; per K slab a
+// bulk-TMA stage brings 2x(hi,lo) A blocks + (hi,lo) of W^T (96 KB); each of 4 consumer warpgroups owns 64 rows
+// and issues 12 wgmma m64n128k16 (3 products x 4 K16 steps) per slab into its register accumulators, then applies
+// the formula on its fragment (fetch x0 / x / bias, store fp32).  The warpgroups run independently, so one's
+// MMAs overlap another's epilogue; a single producer warp (warp 16) drives the bulk-TMA ring.
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -22,7 +22,7 @@
 namespace tfrs {
 namespace tc {
 
-constexpr int CX_THREADS = 640;
+constexpr int CX_THREADS = 544;
 constexpr int CX_STAGES = 2;
 constexpr int CX_STAGE_BYTES = 6 * 16384;  // A: 2 blocks x (hi, lo); B: (hi, lo)
 struct CrossParams {
@@ -43,26 +43,18 @@ cross_tc_kernel(const CrossParams p) {
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CX_STAGES * CX_STAGE_BYTES);
   uint64_t* full = bars;                  // [CX_STAGES]
   uint64_t* empty = bars + CX_STAGES;     // [CX_STAGES]
-  uint64_t* t_full = empty + CX_STAGES;   // [2]
-  uint64_t* t_empty = t_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const long long n_tiles = (long long)p.n_mb * p.n_nt;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < CX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&t_full[b], 1); mbar_init(&t_empty[b], 16); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < CX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 16); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 4) {
+    if (threadIdx.x == 512) {
       int stage = 0; uint32_t phase = 0;
       for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const long long mb = t / p.n_nt; const int nt = (int)(t % p.n_nt);
@@ -77,136 +69,61 @@ cross_tc_kernel(const CrossParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-        const int buf = it & 1;
-        const uint32_t tphase = (it >> 1) & 1;
-        mbar_wait(&t_empty[buf], tphase ^ 1);
-        for (int ks = 0; ks < p.kb; ++ks) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sb = smem_u32(smem + stage * CX_STAGE_BYTES);
-          const uint64_t b_hi = make_smem_desc(sb + 65536), b_lo = make_smem_desc(sb + 65536 + 16384);
+    return;
+  }
+  // warpgroup c: rows [64 c, 64 c + 64) of the 256-row block = half (c & 1) of A block c / 2
+  const int c = wg;
+  const uint32_t a_off = (uint32_t)((c >> 1) * 32768 + (c & 1) * 8192);
+  const float unscale = ldexpf(1.0f, -(p.xst->exp + p.wst->exp));
+  float amax_out = 0.f;       // max |out| over this thread's elements (only used when p.out_amax is given)
+  int stage = 0; uint32_t phase = 0;
+  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const long long mb = t / p.n_nt; const int nt = (int)(t % p.n_nt);
+    float acc[64];
+    for (int ks = 0; ks < p.kb; ++ks) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sb = smem_u32(smem + stage * CX_STAGE_BYTES);
+      const uint64_t a_hi = make_smem_desc(sb + a_off), a_lo = make_smem_desc(sb + a_off + 16384);
+      const uint64_t b_hi = make_smem_desc(sb + 65536), b_lo = make_smem_desc(sb + 65536 + 16384);
+      wgmma_fence();
 #pragma unroll
-          for (int ab = 0; ab < 2; ++ab) {
-            const uint32_t d_tmem = tmem_base + (uint32_t)((ab * 2 + buf) * 128);
-            const uint64_t a_hi = make_smem_desc(sb + ab * 32768), a_lo = make_smem_desc(sb + ab * 32768 + 16384);
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              const uint64_t o = (uint64_t)(k4 * 2);
-              umma_f16(d_tmem, a_hi + o, b_hi + o, IDESC_F16_M128_N128, (uint32_t)((ks | k4) != 0));
-              umma_f16(d_tmem, a_lo + o, b_hi + o, IDESC_F16_M128_N128, 1u);
-              umma_f16(d_tmem, a_hi + o, b_lo + o, IDESC_F16_M128_N128, 1u);
-            }
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == CX_STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&t_full[buf]);
+      for (int k4 = 0; k4 < 4; ++k4) {
+        const uint64_t o = (uint64_t)(k4 * 2);
+        wgmma_m64n128_ss(acc, a_hi + o, b_hi + o, (uint32_t)((ks | k4) != 0));
+        wgmma_m64n128_ss(acc, a_lo + o, b_hi + o, 1u);
+        wgmma_m64n128_ss(acc, a_hi + o, b_lo + o, 1u);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);
+      if (++stage == CX_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int half = ew >> 3, ab = (ew >> 2) & 1, quad = ew & 3;
-    const float unscale = ldexpf(1.0f, -(p.xst->exp + p.wst->exp));
-    float amax_out = 0.f;       // max |out| over this thread's elements (only used when p.out_amax is given)
-    int it = 0;
-    for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t tphase = (it >> 1) & 1;
-      const long long mb = t / p.n_nt; const int nt = (int)(t % p.n_nt);
-      const int n0 = nt * 128 + half * 64;
-      mbar_wait(&t_full[buf], tphase);
-      tc_fence_after();
-      // The accumulators arrive one ROW per lane.  Global memory wants the other orientation, so each 32x32 block is
-      // transposed in registers (5 butterfly stages of shfl.xor): afterwards lane l holds COLUMN l of the 32 rows and every
-      // x / x0 / out access of the warp is one contiguous 128-byte segment of a row.  The 64 columns are taken from TMEM in
-      // two halves of 32 registers, which leaves room for 16 rows x 2 operands = 32 independent loads in flight per thread:
-      // the epilogue is a latency-bound stream (4 x [B,D] of HBM traffic), and with 4-row batches it, not the MMAs, paced
-      // the kernel (same time at K = 256 as at K = 845).
-      const long long row_base = mb * 256 + ab * 128 + quad * 32;
-#pragma unroll 1
-      for (int blk = 0; blk < 2; ++blk) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((ab * 2 + buf) * 128 + half * 64 + blk * 32), r);
-        tmem_ld_wait32(r);
-        if (blk == 1) {   // both halves are in registers: the MMA warp may reuse this TMEM buffer
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&t_empty[buf]);
-        }
+    // epilogue on the fragment: lane pairs of adjacent columns, rows r and r + 8 of the warp's 16
+    const long long row_base = mb * 256 + c * 64 + warp * 16;
+    const int n_base = nt * 128;
 #pragma unroll
-        for (int s = 16; s > 0; s >>= 1) {
-          const bool upper = (lane & s) != 0;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if ((i & s) == 0) {
-              const uint32_t lo_v = r[i], hi_v = r[i | s];
-              const uint32_t recv = __shfl_xor_sync(0xffffffffu, upper ? lo_v : hi_v, s);
-              r[i] = upper ? recv : lo_v;
-              r[i | s] = upper ? hi_v : recv;
-            }
-          }
-        }
-        // now r[j] = accumulator of row (row_base + j), column (n0 + blk*32 + lane)
-        const int col = n0 + blk * 32 + lane;
-        const long long base = row_base * p.ld + col;
-        const int ldi = (int)p.ld;
-        if (row_base + 32 <= p.B && n0 + blk * 32 + 32 <= p.D) {
-          // interior block (all but the ragged last column block / row block): no per-element predicates or branches and
-          // one 32-bit row offset shared by the four arrays -- the epilogue is INSTRUCTION-bound (ncu: issue slots, not
-          // DRAM or the LSU, limit it; the checked path below costs ~70 instructions per element)
-          const float* __restrict__ xp = p.x + base; const float* __restrict__ x0p = p.x0 + base;
-          float* __restrict__ op = p.out + base; float* __restrict__ pp = p.prod ? p.prod + base : nullptr;
-          const float bcol = p.bias ? __ldg(p.bias + col) : 0.f;
-          const float diag = p.diag;
-#pragma unroll
-          for (int j0 = 0; j0 < 32; j0 += 16) {
-            float xv[16], x0v[16];
-#pragma unroll
-            for (int u = 0; u < 16; ++u) { const int o = (j0 + u) * ldi; xv[u] = __ldg(xp + o); x0v[u] = __ldg(x0p + o); }
-#pragma unroll
-            for (int u = 0; u < 16; ++u) {
-              const int o = (j0 + u) * ldi;
-              float pv = fmaf(__uint_as_float(r[j0 + u]), unscale, bcol);
-              pv = fmaf(diag, xv[u], pv);
-              if (pp) pp[o] = pv;
-              const float ov = fmaf(x0v[u], pv, xv[u]);
-              op[o] = ov;
-              amax_out = fmaxf(amax_out, fabsf(ov));
-            }
-          }
-        } else if (col < p.D) {
-          const float bcol = p.bias ? __ldg(p.bias + col) : 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const long long rr = row_base + j;
-            if (rr < p.B) {
-              const long long o = rr * p.ld + col;
-              const float xv = __ldg(p.x + o), x0v = __ldg(p.x0 + o);
-              float pv = fmaf(__uint_as_float(r[j]), unscale, bcol);
-              pv = fmaf(p.diag, xv, pv);
-              if (p.prod) p.prod[o] = pv;
-              const float ov = fmaf(x0v, pv, xv);
-              p.out[o] = ov;
-              amax_out = fmaxf(amax_out, fabsf(ov));
-            }
-          }
-        }
+    for (int i = 0; i < 64; ++i) {
+      const long long rr = row_base + frag_row(i, lane);
+      const int col = n_base + frag_col(i, lane);
+      if (rr < p.B && col < p.D) {
+        const long long o = rr * p.ld + col;
+        const float xv = __ldg(p.x + o), x0v = __ldg(p.x0 + o);
+        float pv = fmaf(acc[i], unscale, p.bias ? __ldg(p.bias + col) : 0.f);
+        pv = fmaf(p.diag, xv, pv);
+        if (p.prod) p.prod[o] = pv;
+        const float ov = fmaf(x0v, pv, xv);
+        p.out[o] = ov;
+        amax_out = fmaxf(amax_out, fabsf(ov));
       }
-    }
-    if (p.out_amax) {   // same statistic, same bits, as a cx_amax_kernel pass over `out` (max is order-independent)
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) amax_out = fmaxf(amax_out, __shfl_xor_sync(0xffffffffu, amax_out, o));
-      if (lane == 0 && amax_out > 0.f) atomicMax(p.out_amax, __float_as_uint(amax_out));
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+  if (p.out_amax) {   // same statistic, same bits, as a cx_amax_kernel pass over `out` (max is order-independent)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax_out = fmaxf(amax_out, __shfl_xor_sync(0xffffffffu, amax_out, o));
+    if (lane == 0 && amax_out > 0.f) atomicMax(p.out_amax, __float_as_uint(amax_out));
+  }
 }
 
 }  // namespace tc
@@ -262,7 +179,7 @@ extern "C" int tfrs_cross_tc_fwd_ex_f32(const float* x0, const float* x, const v
   if (x_amax_bits) {   // max |x| is already known (the previous layer's epilogue produced it): no pass over x
     TFRS_CUDA(cudaMemcpyAsync(&xs->amax_bits, x_amax_bits, sizeof(unsigned int), cudaMemcpyDeviceToDevice, st));
   } else {
-    cx_amax_kernel<<<(unsigned)(148 * 8), 256, 0, st>>>(x, B, D, ld, xs);
+    cx_amax_kernel<<<(unsigned)(sm_count() * 8), 256, 0, st>>>(x, B, D, ld, xs);
     TFRS_LAUNCH_CHECK();
   }
   cx_exp_kernel<<<1, 1, 0, st>>>(xs);

@@ -3,13 +3,13 @@
 //     dx = gp . W^T + diag_scale * gp + g        [B,D] = [B,D] x [D,D]      (K = D)
 //     dW = x^T . gp                              [D,D] = [D,B] x [B,D]      (K = B, the batch)
 // Same fp32-parity scheme as the forward (cross_tc.cu): exact power-of-two rescale, fp16 hi/lo split of both
-// operands, hi*hi + lo*hi + hi*lo accumulated in fp32 in TMEM.  One kernel, two epilogues:
+// operands, hi*hi + lo*hi + hi*lo accumulated in fp32 in registers (wgmma).  One kernel, two epilogues:
 //   DX: A = image(gp), B = image(W) (rows = input feature, K = output feature: W as stored), formula in the epilogue.
 //   DW: A = image(x^T), B = image(gp^T) built by a tiled transpose; the batch is cut into chunks of 16 K-slabs
-//       (1024 rows) so an accumulation chain in TMEM is as short as the forward's (the tensor core's fp32 adder
+//       (1024 rows) so an accumulation chain is as short as the forward's (the tensor core's fp32 adder
 //       truncates; long chains drift), every chunk stores a partial [D,D] and a fixed-order fp32 reduction sums
 //       them -- deterministic, no atomics.
-// Work items (chunk, 256-row block, 128-column tile) are spread over persistent 640-thread CTAs; items of the
+// Work items (chunk, 256-row block, 128-column tile) are spread over persistent 544-thread CTAs (4 consumer warpgroups + 1 producer warp); items of the
 // same chunk run concurrently so their image slabs are read from HBM once and shared through L2.
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -20,7 +20,7 @@
 namespace tfrs {
 namespace tc {
 
-constexpr int SG_THREADS2 = 640;
+constexpr int SG_THREADS2 = 544;
 constexpr int SG_STAGES2 = 2;
 constexpr int SG_STAGE_BYTES = 6 * 16384;  // A: 2 blocks x (hi, lo); B: (hi, lo)
 constexpr int DW_CHUNK_SLABS = 16;         // 1024 batch rows per accumulation chain
@@ -47,27 +47,19 @@ split_gemm_kernel(const SgParams p) {
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SG_STAGES2 * SG_STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + SG_STAGES2;
-  uint64_t* t_full = empty + SG_STAGES2;   // [2]
-  uint64_t* t_empty = t_full + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const long long per_chunk = (long long)p.n_mb * p.n_nt;
   const long long n_items = per_chunk * p.n_kc;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < SG_STAGES2; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&t_full[b], 1); mbar_init(&t_empty[b], 16); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < SG_STAGES2; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 16); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 4) {
+    if (threadIdx.x == 512) {
       int stage = 0; uint32_t phase = 0;
       for (long long t = blockIdx.x; t < n_items; t += gridDim.x) {
         const int kc = (int)(t / per_chunk); const long long rem = t - kc * per_chunk;
@@ -84,158 +76,62 @@ split_gemm_kernel(const SgParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (long long t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
-        const int kc = (int)(t / per_chunk);
-        const int k0 = kc * p.kb_chunk, k1 = min(p.kb_total, k0 + p.kb_chunk);
-        const int buf = it & 1;
-        const uint32_t tphase = (it >> 1) & 1;
-        mbar_wait(&t_empty[buf], tphase ^ 1);
-        for (int ks = k0; ks < k1; ++ks) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sb = smem_u32(smem + stage * SG_STAGE_BYTES);
-          const uint64_t b_hi = make_smem_desc(sb + 65536), b_lo = make_smem_desc(sb + 65536 + 16384);
+    return;
+  }
+  // warpgroup c: rows [64 c, 64 c + 64) of the 256-row block = half (c & 1) of A block c / 2
+  const int c = wg;
+  const uint32_t a_off = (uint32_t)((c >> 1) * 32768 + (c & 1) * 8192);
+  const float unscale = ldexpf(1.0f, -(p.ast->exp + p.bst->exp));
+  int stage = 0; uint32_t phase = 0;
+  for (long long t = blockIdx.x; t < n_items; t += gridDim.x) {
+    const int kc = (int)(t / per_chunk); const long long rem = t - kc * per_chunk;
+    const long long mb = rem / p.n_nt; const int nt = (int)(rem % p.n_nt);
+    const int k0 = kc * p.kb_chunk, k1 = min(p.kb_total, k0 + p.kb_chunk);
+    float acc[64];
+    for (int ks = k0; ks < k1; ++ks) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sb = smem_u32(smem + stage * SG_STAGE_BYTES);
+      const uint64_t a_hi = make_smem_desc(sb + a_off), a_lo = make_smem_desc(sb + a_off + 16384);
+      const uint64_t b_hi = make_smem_desc(sb + 65536), b_lo = make_smem_desc(sb + 65536 + 16384);
+      wgmma_fence();
 #pragma unroll
-          for (int ab = 0; ab < 2; ++ab) {
-            const uint32_t d_tmem = tmem_base + (uint32_t)((ab * 2 + buf) * 128);
-            const uint64_t a_hi = make_smem_desc(sb + ab * 32768), a_lo = make_smem_desc(sb + ab * 32768 + 16384);
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              const uint64_t o = (uint64_t)(k4 * 2);
-              umma_f16(d_tmem, a_hi + o, b_hi + o, IDESC_F16_M128_N128, (uint32_t)((ks != k0) | (k4 != 0)));
-              umma_f16(d_tmem, a_lo + o, b_hi + o, IDESC_F16_M128_N128, 1u);
-              umma_f16(d_tmem, a_hi + o, b_lo + o, IDESC_F16_M128_N128, 1u);
-            }
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == SG_STAGES2) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&t_full[buf]);
+      for (int k4 = 0; k4 < 4; ++k4) {
+        const uint64_t o = (uint64_t)(k4 * 2);
+        wgmma_m64n128_ss(acc, a_hi + o, b_hi + o, (uint32_t)((ks != k0) | (k4 != 0)));
+        wgmma_m64n128_ss(acc, a_lo + o, b_hi + o, 1u);
+        wgmma_m64n128_ss(acc, a_hi + o, b_lo + o, 1u);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);
+      if (++stage == SG_STAGES2) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int half = ew >> 3, ab = (ew >> 2) & 1, quad = ew & 3;
-    const float unscale = ldexpf(1.0f, -(p.ast->exp + p.bst->exp));
-    int it = 0;
-    for (long long t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
-      const int kc = (int)(t / per_chunk); const long long rem = t - kc * per_chunk;
-      const long long mb = rem / p.n_nt; const int nt = (int)(rem % p.n_nt);
-      const int buf = it & 1;
-      const uint32_t tphase = (it >> 1) & 1;
-      const int n0 = nt * 128 + half * 64;
-      mbar_wait(&t_full[buf], tphase);
-      tc_fence_after();
-      // one accumulator ROW per lane -> each 32x32 block is transposed in registers so that lane l holds COLUMN l of the 32
-      // rows and every global access of the warp is one contiguous 128-byte row segment.  TMEM is read in two 32-column
-      // halves: 32 accumulator registers leave room for 16-row batches of epilogue loads (see cross_tc.cu).
-      const long long row_base = mb * 256 + ab * 128 + quad * 32;
-#pragma unroll 1
-      for (int blk = 0; blk < 2; ++blk) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((ab * 2 + buf) * 128 + half * 64 + blk * 32), r);
-        tmem_ld_wait32(r);
-        if (blk == 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&t_empty[buf]);
-        }
+    const long long row_base = mb * 256 + c * 64 + warp * 16;
+    const int n_base = nt * 128;
 #pragma unroll
-        for (int s = 16; s > 0; s >>= 1) {
-          const bool upper = (lane & s) != 0;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if ((i & s) == 0) {
-              const uint32_t lo_v = r[i], hi_v = r[i | s];
-              const uint32_t recv = __shfl_xor_sync(0xffffffffu, upper ? lo_v : hi_v, s);
-              r[i] = upper ? recv : lo_v;
-              r[i | s] = upper ? hi_v : recv;
-            }
-          }
-        }
-        const int col = n0 + blk * 32 + lane;
-        const bool interior = row_base + 32 <= p.M && n0 + blk * 32 + 32 <= p.N;   // warp-uniform
-        if (MODE == SG_DW || MODE == SG_PLAIN) {
-          float* dst = MODE == SG_DW ? p.out + (long long)kc * p.M * p.N + row_base * p.N + col : p.out + row_base * p.ld_out + col;
-          const int ldo = MODE == SG_DW ? (int)p.N : (int)p.ld_out;
-          if (interior) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) dst[j * ldo] = __uint_as_float(r[j]) * unscale;
-          } else if (col < p.N) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (row_base + j < p.M) dst[(long long)j * ldo] = __uint_as_float(r[j]) * unscale;
-          }
-        } else if (MODE == SG_CROSS) {   // out = x0 * (acc + bias + diag * x) + x   (dcn.py:176-186)
-          if (interior) {   // no per-element predicates; one 32-bit row offset per array (instruction-bound epilogue, see cross_tc.cu)
-            const float* __restrict__ x0p = p.e0 + row_base * p.ld0 + col; const float* __restrict__ xp = p.e1 + row_base * p.ld1 + col;
-            float* __restrict__ op = p.out + row_base * p.ld_out + col; float* __restrict__ pp = p.prod ? p.prod + row_base * p.ld_out + col : nullptr;
-            const int l0 = (int)p.ld0, l1 = (int)p.ld1, lo = (int)p.ld_out;
-            const float bcol = p.bias ? __ldg(p.bias + col) : 0.f;
-            const float diag = p.diag;
-#pragma unroll
-            for (int j0 = 0; j0 < 32; j0 += 16) {
-              float xv[16], x0v[16];
-#pragma unroll
-              for (int u = 0; u < 16; ++u) { x0v[u] = __ldg(x0p + (j0 + u) * l0); xv[u] = __ldg(xp + (j0 + u) * l1); }
-#pragma unroll
-              for (int u = 0; u < 16; ++u) {
-                float pv = fmaf(__uint_as_float(r[j0 + u]), unscale, bcol);
-                pv = fmaf(diag, xv[u], pv);
-                if (pp) pp[(j0 + u) * lo] = pv;
-                op[(j0 + u) * lo] = fmaf(x0v[u], pv, xv[u]);
-              }
-            }
-          } else if (col < p.N) {
-            const float bcol = p.bias ? __ldg(p.bias + col) : 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const long long rr = row_base + j;
-              if (rr < p.M) {
-                const float x0v = __ldg(p.e0 + rr * p.ld0 + col), xv = __ldg(p.e1 + rr * p.ld1 + col);
-                float pv = fmaf(__uint_as_float(r[j]), unscale, bcol);
-                pv = fmaf(p.diag, xv, pv);
-                if (p.prod) p.prod[rr * p.ld_out + col] = pv;
-                p.out[rr * p.ld_out + col] = fmaf(x0v, pv, xv);
-              }
-            }
-          }
-        } else {                          // DX: dx = acc + diag * gp + g
-          if (interior) {
-            const float* __restrict__ gpp = p.e0 + row_base * p.ld0 + col; const float* __restrict__ gp_ = p.e1 + row_base * p.ld1 + col;
-            float* __restrict__ op = p.out + row_base * p.ld_out + col;
-            const int l0 = (int)p.ld0, l1 = (int)p.ld1, lo = (int)p.ld_out;
-            const float diag = p.diag;
-#pragma unroll
-            for (int j0 = 0; j0 < 32; j0 += 16) {
-              float gv[16], gpv[16];
-#pragma unroll
-              for (int u = 0; u < 16; ++u) { gv[u] = __ldg(gp_ + (j0 + u) * l1); gpv[u] = diag != 0.f ? __ldg(gpp + (j0 + u) * l0) : 0.f; }
-#pragma unroll
-              for (int u = 0; u < 16; ++u) op[(j0 + u) * lo] = fmaf(diag, gpv[u], fmaf(__uint_as_float(r[j0 + u]), unscale, gv[u]));
-            }
-          } else if (col < p.N) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const long long rr = row_base + j;
-              if (rr < p.M) {
-                float v = fmaf(__uint_as_float(r[j]), unscale, __ldg(p.e1 + rr * p.ld1 + col));
-                if (p.diag != 0.f) v = fmaf(p.diag, __ldg(p.e0 + rr * p.ld0 + col), v);
-                p.out[rr * p.ld_out + col] = v;
-              }
-            }
-          }
-        }
+    for (int i = 0; i < 64; ++i) {
+      const long long rr = row_base + frag_row(i, lane);
+      const long long col = n_base + frag_col(i, lane);
+      if (rr >= p.M || col >= p.N) continue;
+      if (MODE == SG_DW) {
+        p.out[(long long)kc * p.M * p.N + rr * p.N + col] = acc[i] * unscale;
+      } else if (MODE == SG_PLAIN) {
+        p.out[rr * p.ld_out + col] = acc[i] * unscale;
+      } else if (MODE == SG_CROSS) {   // out = x0 * (acc + bias + diag * x) + x   (dcn.py:176-186)
+        const float x0v = __ldg(p.e0 + rr * p.ld0 + col), xv = __ldg(p.e1 + rr * p.ld1 + col);
+        float pv = fmaf(acc[i], unscale, p.bias ? __ldg(p.bias + col) : 0.f);
+        pv = fmaf(p.diag, xv, pv);
+        if (p.prod) p.prod[rr * p.ld_out + col] = pv;
+        p.out[rr * p.ld_out + col] = fmaf(x0v, pv, xv);
+      } else {                          // DX: dx = acc + diag * gp + g
+        float v = fmaf(acc[i], unscale, __ldg(p.e1 + rr * p.ld1 + col));
+        if (p.diag != 0.f) v = fmaf(p.diag, __ldg(p.e0 + rr * p.ld0 + col), v);
+        p.out[rr * p.ld_out + col] = v;
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // fp32 src [K, M] (row stride ld)  ->  hi/lo fp16 image of src^T: image rows = columns m of src, reduction index = rows

@@ -1,13 +1,13 @@
 // softmax_tc.cu -- K3 forward on the tensor cores: in-batch sampled-softmax loss of tfrs.tasks.Retrieval
 //   tasks/retrieval.py:178-180 (scores = q . c^T), :185 (labels = eye), :187-188 (/temperature), :210 + :86-87
 //   loss = sum_i w_i * (logsumexp_j (q_i . c_j / T)  -  q_i . c_i / T)
-// as ONE tcgen05 GEMM whose epilogue keeps an online (max, sum-exp) per query row and picks the diagonal --
+// as ONE wgmma GEMM whose epilogue keeps an online (max, sum-exp) per query row and picks the diagonal --
 // the [B,C] logits and the eye() labels never exist.  fp32 parity: hi/lo fp16 split of both operands (tc_split.cuh),
-// 3 MMAs per K step, fp32 accumulation in TMEM (~2^-21 relative on a score).
+// 3 MMAs per K step, fp32 accumulation in registers (~2^-21 relative on a score).
 //
 // CTA shape = the top-K scan's: 256 query rows (two 128-row A blocks, hi+lo, resident), candidate tiles of
-// 128 rows streamed through a bulk-TMA ring, 2x2 TMEM accumulator buffers, 16 epilogue warps (one row x 64
-// columns per thread).  Grid = query blocks x candidate parts; every (row, part, column-half) leaves a partial
+// 128 rows streamed through a bulk-TMA ring by one producer warp, 4 consumer warpgroups (64 query rows each,
+// wgmma m64n128k16, the epilogue on the register fragment).  Grid = query blocks x candidate parts; every (row, part, column-half) leaves a partial
 // (max, sum-exp) pair that `smtc_combine_kernel` folds into lse_i and the weighted row loss; the scalar loss is
 // reduced in fixed order in fp64 (deterministic).  The backward pass (softmax.cu) consumes the same `lse`.
 #include <cuda_fp16.h>
@@ -19,7 +19,7 @@
 namespace tfrs {
 namespace tc {
 
-constexpr int SX_THREADS = 640;
+constexpr int SX_THREADS = 544;
 // candidate-tile ring depth: 4 x 32 KB at d <= 64, 1 x 64 KB at d <= 128 (A = 128 KB there)
 __host__ __device__ constexpr int sx_stages(int kb) { return kb == 1 ? 4 : 1; }
 constexpr float SX_LOG2E = 1.4426950408889634f;
@@ -46,6 +46,14 @@ constexpr float SX_MIN2 = -3.4028235e36f * SX_LOG2E;
 // MODE 0: plain; 1: + per-candidate bias (sampling-probability correction); 2: + accidental-hit removal (candidate ids,
 // tasks/retrieval.py:194-200, layers/loss.py:114-147: logits + dup * MIN_FLOAT == MIN_FLOAT in fp32) and score_mask
 // (retrieval.py:202-203: where(mask, s, MIN_FLOAT)) applied to the accumulators in registers.
+// (m, l) pairs in log2 units: merge b into a (an empty pair is m = -inf, l = 0)
+__device__ __forceinline__ void lse_merge(float& m, float& l, float mb, float lb) {
+  const float M = fmaxf(m, mb);
+  if (M == -INFINITY) return;
+  l = l * ex2_approx(m - M) + lb * ex2_approx(mb - M);
+  m = M;
+}
+
 template <int KB, int MODE>
 __global__ void __launch_bounds__(SX_THREADS, 1)
 softmax_tc_kernel(const SoftmaxTcParams p) {
@@ -62,30 +70,22 @@ softmax_tc_kernel(const SoftmaxTcParams p) {
   uint64_t* full = bars;
   uint64_t* empty = bars + SX_STAGES;
   uint64_t* a_full = bars + 2 * SX_STAGES;
-  uint64_t* t_full = a_full + 1;     // [ab][buf]: the two 128-row halves signal separately, so one half's epilogue warps
-  uint64_t* t_empty = t_full + 4;    //            pull from TMEM while the other half's are busy on the MUFU pipe
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 4);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
   const long long t_begin = (long long)part * p.n_ctiles / p.parts;
   const long long t_end = (long long)(part + 1) * p.n_ctiles / p.parts;
   const int n_iter = (int)(t_end - t_begin);
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < SX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < SX_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 16); }
     mbar_init(a_full, 1);
-    for (int b = 0; b < 4; ++b) { mbar_init(&t_full[b], 1); mbar_init(&t_empty[b], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 4) {
+    if (threadIdx.x == 512) {
       mbar_expect_tx(a_full, A_BYTES);
       bulk_g2s(sA, p.qimg + (long long)qb * A_BYTES, A_BYTES, a_full);
       int stage = 0; uint32_t phase = 0;
@@ -96,151 +96,125 @@ softmax_tc_kernel(const SoftmaxTcParams p) {
         if (++stage == SX_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(a_full, 0);
-      tc_fence_after();
-      int stage = 0; uint32_t phase = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        const int buf = it & 1;
-        const uint32_t tphase = (it >> 1) & 1;
-        mbar_wait(&full[stage], phase);
+    return;
+  }
+  // warpgroup c: query rows [64 c, 64 c + 64) of the CTA's 256 (half c & 1 of A block c / 2); a thread holds rows r, r + 8
+  // x 32 columns of every tile and keeps an online (max, sum-exp) per (row, column half), merged over the quad at the end
+  const int c = wg;
+  const long long row_a = (long long)qb * 256 + c * 64 + warp * 16 + (lane >> 2);
+  // logits in log2 units: s2 = acc * 2^-(eq+ec) * invT * log2(e)
+  const float scale2 = ldexpf(p.inv_t * SX_LOG2E, -(p.qst->exp + p.cst->exp));
+  float m2[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, l[4] = {0.f, 0.f, 0.f, 0.f};   // s = 2 rr + half
+  float pos2[2] = {0.f, 0.f};
+  bool has_pos[2] = {false, false};
+  int rid_lo[2] = {0, 0}, rid_hi[2] = {0, 0};   // id of each row's positive candidate (candidate `row`); arrays padded past Bp
+  if (EXT && p.id_lo) {
 #pragma unroll
-        for (int ab = 0; ab < 2; ++ab) {
-          mbar_wait(&t_empty[ab * 2 + buf], tphase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)((ab * 2 + buf) * 128);
+    for (int rr = 0; rr < 2; ++rr) { rid_lo[rr] = p.id_lo[row_a + 8 * rr]; rid_hi[rr] = p.id_hi[row_a + 8 * rr]; }
+  }
+  mbar_wait(a_full, 0);
+  const uint32_t a0 = smem_u32(sA + (c >> 1) * KB * 32768 + (c & 1) * 8192);
+  int stage = 0; uint32_t phase = 0;
+  for (int it = 0; it < n_iter; ++it) {
+    const long long col0 = (t_begin + it) * 128;
+    mbar_wait(&full[stage], phase);
+    float acc[64];
+    wgmma_fence();
 #pragma unroll
-          for (int kb = 0; kb < KB; ++kb) {
-            const uint32_t a0 = smem_u32(sA + (ab * KB + kb) * 32768), b0 = smem_u32(sB + stage * B_BYTES + kb * 32768);
-            const uint64_t a_hi = make_smem_desc(a0), a_lo = make_smem_desc(a0 + 16384);
-            const uint64_t b_hi = make_smem_desc(b0), b_lo = make_smem_desc(b0 + 16384);
+    for (int kb = 0; kb < KB; ++kb) {
+      const uint32_t b0 = smem_u32(sB + stage * B_BYTES + kb * 32768);
+      const uint64_t a_hi = make_smem_desc(a0 + kb * 32768), a_lo = make_smem_desc(a0 + kb * 32768 + 16384);
+      const uint64_t b_hi = make_smem_desc(b0), b_lo = make_smem_desc(b0 + 16384);
 #pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              const uint64_t o = (uint64_t)(k4 * 2);
-              umma_f16(d_tmem, a_hi + o, b_hi + o, IDESC_F16_M128_N128, (uint32_t)((kb | k4) != 0));
-              umma_f16(d_tmem, a_lo + o, b_hi + o, IDESC_F16_M128_N128, 1u);
-              umma_f16(d_tmem, a_hi + o, b_lo + o, IDESC_F16_M128_N128, 1u);
-            }
-          }
-          umma_commit(&t_full[ab * 2 + buf]);
-        }
-        umma_commit(&empty[stage]);
-        if (++stage == SX_STAGES) { stage = 0; phase ^= 1; }
+      for (int k4 = 0; k4 < 4; ++k4) {
+        const uint64_t o = (uint64_t)(k4 * 2);
+        wgmma_m64n128_ss(acc, a_hi + o, b_hi + o, (uint32_t)((kb | k4) != 0));
+        wgmma_m64n128_ss(acc, a_lo + o, b_hi + o, 1u);
+        wgmma_m64n128_ss(acc, a_hi + o, b_lo + o, 1u);
       }
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int half = ew >> 3, ab = (ew >> 2) & 1, quad = ew & 3;
-    const long long row = (long long)qb * 256 + ab * 128 + quad * 32 + lane;
-    // logits in log2 units: s2 = acc * 2^-(eq+ec) * invT * log2(e)
-    const float scale2 = ldexpf(p.inv_t * SX_LOG2E, -(p.qst->exp + p.cst->exp));
-    float m2 = -INFINITY, l = 0.f, pos2 = 0.f;
-    int rid_lo = 0, rid_hi = 0;   // id of this row's positive candidate (candidate `row`); the arrays are padded past Bp
-    if (EXT && p.id_lo) { rid_lo = p.id_lo[row]; rid_hi = p.id_hi[row]; }
-    for (int it = 0; it < n_iter; ++it) {
-      const int buf = it & 1;
-      const uint32_t tphase = (it >> 1) & 1;
-      const long long col0 = (t_begin + it) * 128 + half * 64;
-      mbar_wait(&t_full[ab * 2 + buf], tphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((ab * 2 + buf) * 128 + half * 64);
-      uint32_t r[64];
-      tmem_ld64(taddr, r);
-      tmem_ld_wait64(r);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_empty[ab * 2 + buf]);
-      const int n_valid = (int)min(64ll, p.C - col0);  // columns beyond C are zero-padded rows of the image
-      if (n_valid <= 0) continue;
-      // BIAS (sampling-probability correction, retrieval.py:190-192): logits s/T + b_j.  The scores are turned into
-      // log2-unit logits in place (one FFMA with the per-candidate bias, read through L2), the rest runs with scale 1.
-      if (BIAS) {
-        const float4* b4 = reinterpret_cast<const float4*>(p.cbias2 + col0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);
+    if (++stage == SX_STAGES) { stage = 0; phase ^= 1; }
+
+    // BIAS (sampling-probability correction, retrieval.py:190-192): logits s/T + b_j -> turned into log2-unit logits in
+    // place (one FFMA with the per-candidate bias), the rest runs with scale 1.  EXT masks set MIN_FLOAT.
+    if (BIAS || EXT) {
 #pragma unroll
-        for (int j4 = 0; j4 < 16; ++j4) {
-          const float4 bb = __ldg(b4 + j4);
-          r[4 * j4 + 0] = __float_as_uint(fmaf(__uint_as_float(r[4 * j4 + 0]), scale2, bb.x));
-          r[4 * j4 + 1] = __float_as_uint(fmaf(__uint_as_float(r[4 * j4 + 1]), scale2, bb.y));
-          r[4 * j4 + 2] = __float_as_uint(fmaf(__uint_as_float(r[4 * j4 + 2]), scale2, bb.z));
-          r[4 * j4 + 3] = __float_as_uint(fmaf(__uint_as_float(r[4 * j4 + 3]), scale2, bb.w));
-        }
-      }
-      if (EXT) {
-        if (p.id_lo) {   // accidental hits: another candidate with the id of this row's positive -> MIN_FLOAT
-          const int4* il = reinterpret_cast<const int4*>(p.id_lo + col0);
-#pragma unroll
-          for (int j4 = 0; j4 < 16; ++j4) {
-            const int4 v = __ldg(il + j4);
-            if ((v.x == rid_lo) | (v.y == rid_lo) | (v.z == rid_lo) | (v.w == rid_lo)) {   // rare
-              const int* ih = p.id_hi + col0 + 4 * j4;
-              const long long c = col0 + 4 * j4;
-              if (v.x == rid_lo && __ldg(ih + 0) == rid_hi && c + 0 != row) r[4 * j4 + 0] = __float_as_uint(SX_MIN2);
-              if (v.y == rid_lo && __ldg(ih + 1) == rid_hi && c + 1 != row) r[4 * j4 + 1] = __float_as_uint(SX_MIN2);
-              if (v.z == rid_lo && __ldg(ih + 2) == rid_hi && c + 2 != row) r[4 * j4 + 2] = __float_as_uint(SX_MIN2);
-              if (v.w == rid_lo && __ldg(ih + 3) == rid_hi && c + 3 != row) r[4 * j4 + 3] = __float_as_uint(SX_MIN2);
-            }
+      for (int i = 0; i < 64; ++i) {
+        const long long col = col0 + frag_col(i, lane);
+        const int rr = (i >> 1) & 1;
+        float v = acc[i];
+        if (BIAS) v = fmaf(v, scale2, __ldg(p.cbias2 + col));
+        if (EXT) {
+          const long long row = row_a + 8 * rr;
+          if (p.id_lo && __ldg(p.id_lo + col) == rid_lo[rr] && __ldg(p.id_hi + col) == rid_hi[rr] && col != row) v = SX_MIN2;
+          if (p.mbits) {
+            const int cl = frag_col(i, lane);
+            const uint32_t mw = __ldg(p.mbits + row * p.mwords + (t_begin + it) * 4 + (cl >> 5));
+            if (!((mw >> (cl & 31)) & 1u)) v = SX_MIN2;
           }
         }
-        if (p.mbits) {   // score_mask: bit = keep
-          const uint2 mw = __ldg(reinterpret_cast<const uint2*>(p.mbits + row * p.mwords + (t_begin + it) * 4 + half * 2));
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (!((mw.x >> j) & 1u)) r[j] = __float_as_uint(SX_MIN2);
-            if (!((mw.y >> j) & 1u)) r[32 + j] = __float_as_uint(SX_MIN2);
-          }
-        }
+        acc[i] = v;
       }
-      const float sc = BIAS ? 1.0f : scale2;
-      const long long blk0 = (long long)qb * 256 + ab * 128;
-      const bool edge = n_valid < 64 || (blk0 < col0 + 64 && col0 < blk0 + 128);  // ragged tail, or the tile with the positives
-      float m_new, acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;
-      if (!edge) {
-        // scale2 > 0: the row maximum can be taken on the raw accumulators (FMNMX3 tree), one FFMA + one MUFU per score
-        float t[8];
+    }
+    const float sc = BIAS ? 1.0f : scale2;
+    const int n_valid = (int)min(128ll, p.C - col0);  // columns beyond C are zero-padded rows of the image
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const float a0 = max3(__uint_as_float(r[8 * g]), __uint_as_float(r[8 * g + 1]), __uint_as_float(r[8 * g + 2]));
-          const float a1 = max3(__uint_as_float(r[8 * g + 3]), __uint_as_float(r[8 * g + 4]), __uint_as_float(r[8 * g + 5]));
-          t[g] = max3(a0, a1, fmaxf(__uint_as_float(r[8 * g + 6]), __uint_as_float(r[8 * g + 7])));
-        }
-        const float tmax = max3(max3(t[0], t[1], t[2]), max3(t[3], t[4], t[5]), fmaxf(t[6], t[7]));
-        m_new = fmaxf(m2, tmax * sc);
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long row = row_a + 8 * rr;
+      if (row >= col0 && row < col0 + 128) {   // the positive of query i is candidate i (retrieval.py:185)
 #pragma unroll
-        for (int j = 0; j < 64; j += 4) {
-          acc0 += ex2_approx(fmaf(__uint_as_float(r[j]), sc, -m_new));
-          acc1 += ex2_approx(fmaf(__uint_as_float(r[j + 1]), sc, -m_new));
-          acc2 += ex2_approx(fmaf(__uint_as_float(r[j + 2]), sc, -m_new));
-          acc3 += ex2_approx(fmaf(__uint_as_float(r[j + 3]), sc, -m_new));
-        }
-      } else {
+        for (int i = 0; i < 64; ++i)
+          if (((i >> 1) & 1) == rr && col0 + frag_col(i, lane) == row) { pos2[rr] = acc[i] * sc; has_pos[rr] = true; }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
         float tmax = -INFINITY;
 #pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (j < n_valid) tmax = fmaxf(tmax, __uint_as_float(r[j]));
-        m_new = fmaxf(m2, tmax * sc);
-        if (row >= col0 && row < col0 + 64) {   // the positive of query i is candidate i (retrieval.py:185)
-          const int jd = (int)(row - col0);
-#pragma unroll
-          for (int j = 0; j < 64; ++j) if (j == jd) pos2 = __uint_as_float(r[j]) * sc;
+        for (int jj = 0; jj < 8; ++jj) {
+          const int i = 4 * (8 * h + jj) + 2 * rr;
+          if (frag_col(i, lane) < n_valid) tmax = fmaxf(tmax, acc[i]);
+          if (frag_col(i + 1, lane) < n_valid) tmax = fmaxf(tmax, acc[i + 1]);
         }
+        if (tmax == -INFINITY) continue;
+        const int s = 2 * rr + h;
+        const float m_new = fmaxf(m2[s], tmax * sc);
+        float a0s = 0.f, a1s = 0.f;
 #pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (j < n_valid) acc0 += ex2_approx(fmaf(__uint_as_float(r[j]), sc, -m_new));
+        for (int jj = 0; jj < 8; ++jj) {
+          const int i = 4 * (8 * h + jj) + 2 * rr;
+          if (frag_col(i, lane) < n_valid) a0s += ex2_approx(fmaf(acc[i], sc, -m_new));
+          if (frag_col(i + 1, lane) < n_valid) a1s += ex2_approx(fmaf(acc[i + 1], sc, -m_new));
+        }
+        l[s] = l[s] * ex2_approx(m2[s] - m_new) + (a0s + a1s);
+        m2[s] = m_new;
       }
-      l = l * ex2_approx(m2 - m_new) + ((acc0 + acc1) + (acc2 + acc3));
-      m2 = m_new;
-    }
-    if (row < p.B) {
-      p.partial[(row * p.parts + part) * 2 + half] = make_float2(m2, l);
-      // exactly one (part, half) thread of the row saw the diagonal column
-      const long long dt = row / 128;
-      if (dt >= t_begin && dt < t_end && ((row % 128) / 64) == half) p.pos[row] = pos2;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+  // merge the quad's partial (max, sum-exp) pairs; the quad leader writes them
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      const float mo = __shfl_xor_sync(0xffffffffu, m2[s], o), lo_ = __shfl_xor_sync(0xffffffffu, l[s], o);
+      lse_merge(m2[s], l[s], mo, lo_);
+    }
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const long long row = row_a + 8 * rr;
+    if (row < p.B) {
+      if ((lane & 3) == 0) {
+        p.partial[(row * p.parts + part) * 2 + 0] = make_float2(m2[2 * rr], l[2 * rr]);
+        p.partial[(row * p.parts + part) * 2 + 1] = make_float2(m2[2 * rr + 1], l[2 * rr + 1]);
+      }
+      if (has_pos[rr]) p.pos[row] = pos2[rr];   // exactly one thread of one part saw the diagonal column
+    }
+  }
 }
 
 // lse_i = ln2 * (M + log2(sum_p l_p 2^(m_p - M)));  rowloss_i = w_i (lse_i - pos_i), formed as ln2 * ((M - pos2_i) + log2 L)

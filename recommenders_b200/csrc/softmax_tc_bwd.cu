@@ -2,11 +2,12 @@
 //   (tape.gradient at models/base.py:77 through tasks/retrieval.py:178-210)
 //   G_ij = (softmax(s)_ij - [i == j]) * w_i * grad_loss / T ;   dq = G . c  [B,d] ;   dc = G^T . q  [C,d]
 // as two launches of ONE kernel (flash-attention-backward shape, deterministic -- no atomics):
-//   stationary operand X (128 rows = TMEM lanes, resident in smem), streaming operand Y (128-row tiles, bulk-TMA ring)
-//     S   = X . Y^T          tcgen05 SS-mode, hi/lo fp16 split operands (3 MMAs per K16), fp32 in TMEM
-//     A   = (exp(S/T - lse_q) - diag) * w_q     computed by the epilogue warps from TMEM, split into fp16 hi/lo and
-//                                               written back IN PLACE over S with tcgen05.st (128 fp32 cols -> 64+64)
-//     dX += A . Y            tcgen05 TS-mode: A from TMEM, Y straight from the same smem tile as an MN-major operand
+//   stationary operand X (128 rows, resident in smem), streaming operand Y (128-row tiles, bulk-TMA ring); two consumer
+//   warpgroups own 64 rows of X each:
+//     S   = X . Y^T          wgmma SS-mode, hi/lo fp16 split operands (3 MMAs per K16), fp32 in registers
+//     G   = (exp(S/T - lse_q) - diag) * w_q     computed on the register fragment and split into fp16 hi/lo, which is
+//                                               exactly the register layout of a wgmma A operand
+//     dX += G . Y            wgmma RS-mode: G from registers, Y straight from the same smem tile as an MN-major operand
 //   launch 1: X = q, Y = c  -> dq ;  launch 2: X = c, Y = q (lse/w become per-column vectors staged with the tile) -> dc.
 // The [B,C] logits / probabilities never touch HBM; the scores are the same split products as the forward pass
 // (softmax_tc.cu), so exp(s - lse) is consistent with the saved lse.  d <= 64.
@@ -19,14 +20,12 @@
 namespace tfrs {
 namespace tc {
 
-constexpr int SB_THREADS = 640;                // warp 0 producer, 1 MMA, 2 TMEM alloc, 4-19 epilogue (TMEM lane quad = warp & 3)
-constexpr int SB_W_PROD = 0, SB_W_MMA = 1, SB_W_ALLOC = 2;
+constexpr int SB_THREADS = 288;                // warpgroups 0-1: MMA + transform, warp 8: bulk-TMA producer
 constexpr int SB_STAGES = 4;
-// the tensor core's fp32 adder truncates: a chain of thousands of accumulations into the same TMEM tile drifts (5e-5 of
-// the gradient scale at C = 16384), so the dX tile is drained into fp32 registers (round-to-nearest adds) every
-// SB_DRAIN streamed tiles = 192 accumulation steps, the length of the forward Cross chain
+// the tensor core's fp32 adder truncates: a chain of thousands of accumulations into the same accumulator drifts (5e-5
+// of the gradient scale at C = 16384), so each chain restarts every SB_DRAIN streamed tiles = 192 accumulation steps
+// (the length of the forward Cross chain) and is added into an fp32 register sum (round-to-nearest adds)
 constexpr int SB_DRAIN = 8;
-constexpr int SB_BUFS = 3;                     // S/G accumulator buffers in TMEM (3 x 128 columns) + dX (64 columns)
 constexpr int SB_Y_BYTES = 32768;              // one 128-row tile: hi 16 KB | lo 16 KB
 constexpr int SB_STAGE_BYTES = SB_Y_BYTES + 1024;  // + lse[128] | w[128] of the tile (transposed launch)
 constexpr float SB_LOG2E = 1.4426950408889634f;
@@ -46,54 +45,9 @@ struct SoftmaxBwdParams {
   const uint32_t* mbits; int mwords;    // keep-bits [stationary row][streamed column]: the (B,C) matrix for dq, its transpose for dc
 };
 
-// One thread's 64 accumulator columns -> A, split into fp16 hi (written in place over r[0..31]: output slot 2*j4+e
-// is only written after inputs 4*j4.. are consumed) and lo[32].
-//   non-transposed: A = (exp(s/T - lse_i) - diag) * 2^14 -- lse_r already carries the -14 ln2, the weight of row i is
-//                   applied once to the dX block;   transposed: A = (exp(s/T - lse_j) - diag) * w^_j (per-column vectors).
-// EDGE = the tile holds the diagonal or columns beyond the valid range (rare): masks compiled in only there.
-// BIAS: logits carry a per-candidate bias b_c: the exponent is s/T + b_c - lse_q.  Non-transposed: candidates are the
-// columns (cb4 = this thread's 64 biases, read through L2); transposed: the candidate is the row (bias_r).
-// EXT: kill0 / kill1 = bit j set -> entry j (columns 0..31 / 32..63) is masked: A = 0 (where() blocks the gradient of a
-// masked score, and exp(MIN_FLOAT - lse) = 0 for an accidental hit).
-template <bool TRANSPOSED, bool EDGE, bool BIAS, bool EXT>
-__device__ __forceinline__ void sb_transform(uint32_t (&r)[64], uint32_t (&lo)[32], float scale, float lse_r,
-                                             const float4* __restrict__ aux4, int n_valid, int jd,
-                                             const float4* __restrict__ cb4, float bias_r, uint32_t kill0, uint32_t kill1) {
-#pragma unroll
-  for (int j4 = 0; j4 < 16; ++j4) {
-    float lq[4] = {lse_r, lse_r, lse_r, lse_r}, wq[4] = {16384.f, 16384.f, 16384.f, 16384.f};
-    if (TRANSPOSED) {
-      const float4 l4 = aux4[j4], w4 = aux4[32 + j4];
-      lq[0] = l4.x; lq[1] = l4.y; lq[2] = l4.z; lq[3] = l4.w;
-      wq[0] = w4.x; wq[1] = w4.y; wq[2] = w4.z; wq[3] = w4.w;
-      if (BIAS) { lq[0] -= bias_r; lq[1] -= bias_r; lq[2] -= bias_r; lq[3] -= bias_r; }
-    } else if (BIAS) {
-      const float4 bb = __ldg(cb4 + j4);
-      lq[0] -= bb.x; lq[1] -= bb.y; lq[2] -= bb.z; lq[3] -= bb.w;
-    }
-    float a[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int j = 4 * j4 + e;
-      float pr = ex2_approx(fmaf(__uint_as_float(r[j]), scale, -lq[e]) * SB_LOG2E);
-      if (TRANSPOSED) {
-        if (EDGE && j == jd) pr -= 1.0f;
-        pr *= wq[e];
-      } else {
-        if (EDGE && j == jd) pr -= 16384.f;
-      }
-      a[e] = (!EDGE || j < n_valid) ? pr : 0.f;
-      if (EXT && (((j < 32 ? kill0 : kill1) >> (j & 31)) & 1u)) a[e] = 0.f;
-    }
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const __half2 h = __floats2half2_rn(a[2 * e], a[2 * e + 1]);
-      const float2 hf = __half22float2(h);
-      const __half2 l = __floats2half2_rn(a[2 * e] - hf.x, a[2 * e + 1] - hf.y);
-      r[2 * j4 + e] = *reinterpret_cast<const uint32_t*>(&h);
-      lo[2 * j4 + e] = *reinterpret_cast<const uint32_t*>(&l);
-    }
-  }
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 template <bool TRANSPOSED, int MODE>
@@ -109,35 +63,22 @@ softmax_tc_bwd_kernel(const SoftmaxBwdParams p) {
   uint64_t* y_full = bars;
   uint64_t* y_empty = bars + SB_STAGES;
   uint64_t* x_full = bars + 2 * SB_STAGES;
-  uint64_t* s_full = x_full + 1;     // [SB_BUFS]
-  uint64_t* g_ready = s_full + SB_BUFS;
-  uint64_t* dx_full = g_ready + SB_BUFS;
-  uint64_t* dx_drained = dx_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dx_drained + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int xb = blockIdx.x % p.n_xb, part = blockIdx.x / p.n_xb;
   const long long t_begin = (long long)part * p.n_ytiles / p.parts;
   const long long t_end = (long long)(part + 1) * p.n_ytiles / p.parts;
   const int n_iter = (int)(t_end - t_begin);
 
-  if (warp == SB_W_MMA && lane == 0) {
-    for (int s = 0; s < SB_STAGES; ++s) { mbar_init(&y_full[s], 1); mbar_init(&y_empty[s], 1); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < SB_STAGES; ++s) { mbar_init(&y_full[s], 1); mbar_init(&y_empty[s], 8); }
     mbar_init(x_full, 1);
-    for (int b = 0; b < SB_BUFS; ++b) { mbar_init(&s_full[b], 1); mbar_init(&g_ready[b], 8); }
-    mbar_init(dx_full, 1);
-    mbar_init(dx_drained, 16);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == SB_W_ALLOC) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_dx = tmem_base + SB_BUFS * 128;
 
-  if (warp == SB_W_PROD) {
-    if (lane == 0) {
+  if (wg == 2) {
+    if (threadIdx.x == 256) {
       mbar_expect_tx(x_full, 32768);
       bulk_g2s(sX, p.ximg + (long long)xb * 32768, 32768, x_full);
       int stage = 0; uint32_t phase = 0;
@@ -154,168 +95,130 @@ softmax_tc_bwd_kernel(const SoftmaxBwdParams p) {
         if (++stage == SB_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == SB_W_MMA) {
-    if (lane == 0) {
-      mbar_wait(x_full, 0);
-      tc_fence_after();
-      const uint32_t x0 = smem_u32(sX);
-      const uint64_t x_hi = make_smem_desc(x0), x_lo = make_smem_desc(x0 + 16384);
-      // dX(u) += A(u) . Y(u):  A from TMEM buffer u&1 (hi | lo per 64-column half), Y tile as MN-major B (K = its rows)
-      auto issue_dx = [&](int u) {
-        const int buf = u % SB_BUFS, stage = u % SB_STAGES;
-        const int chunk = u / SB_DRAIN, first = (u % SB_DRAIN) == 0;
-        if (first && chunk > 0) mbar_wait(dx_drained, (uint32_t)((chunk - 1) & 1));  // epilogue took the previous chunk's sum
-        mbar_wait(&g_ready[buf], (uint32_t)((u / SB_BUFS) & 1));
-        tc_fence_after();
-        const uint32_t y0 = smem_u32(sY + stage * SB_STAGE_BYTES);
+    return;
+  }
+  // warpgroup c: stationary rows [64 c, 64 c + 64) of the 128-row block; a thread holds rows r, r + 8 of the warp's 16
+  const int c = wg;
+  const long long row_a = (long long)xb * 128 + c * 64 + warp * 16 + (lane >> 2);
+  const float scale = ldexpf(p.inv_t, -(p.xst->exp + p.yst->exp));  // accumulator -> logit (natural units)
+  float lse_r[2] = {0.f, 0.f}, w_r[2] = {1.f, 1.f}, bias_r[2] = {0.f, 0.f};
+  int rid_lo[2] = {0, 0}, rid_hi[2] = {0, 0};   // id of the stationary row: the positive's id of query `row` (dq) / candidate `row` (dc)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t a_hi = tmem_base + (uint32_t)(buf * 128 + 64 * (j >> 2) + 8 * (j & 3));
-          const uint32_t a_lo = a_hi + 32;
-          const uint64_t b_hi = make_smem_desc(y0 + j * 2048), b_lo = make_smem_desc(y0 + 16384 + j * 2048);
-          umma_f16_ts(tmem_dx, a_hi, b_hi, IDESC_F16_M128_N64_BMN, (uint32_t)(!first || j != 0));
-          umma_f16_ts(tmem_dx, a_lo, b_hi, IDESC_F16_M128_N64_BMN, 1u);
-          umma_f16_ts(tmem_dx, a_hi, b_lo, IDESC_F16_M128_N64_BMN, 1u);
-        }
-        umma_commit(&y_empty[stage]);
-        if ((u % SB_DRAIN) == SB_DRAIN - 1 || u == n_iter - 1) umma_commit(dx_full);  // chunk complete
-      };
-      for (int it = 0; it < n_iter; ++it) {
-        const int buf = it % SB_BUFS, stage = it % SB_STAGES;
-        mbar_wait(&y_full[stage], (uint32_t)((it / SB_STAGES) & 1));
-        tc_fence_after();
-        const uint32_t y0 = smem_u32(sY + stage * SB_STAGE_BYTES);
-        const uint64_t y_hi = make_smem_desc(y0), y_lo = make_smem_desc(y0 + 16384);
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * 128);
-#pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4) {
-          const uint64_t o = (uint64_t)(k4 * 2);
-          // same three products, in the same order, as the forward pass (q_hi c_hi, q_lo c_hi, q_hi c_lo)
-          umma_f16(d_tmem, x_hi + o, y_hi + o, IDESC_F16_M128_N128, (uint32_t)(k4 != 0));
-          if (TRANSPOSED) {
-            umma_f16(d_tmem, x_hi + o, y_lo + o, IDESC_F16_M128_N128, 1u);
-            umma_f16(d_tmem, x_lo + o, y_hi + o, IDESC_F16_M128_N128, 1u);
-          } else {
-            umma_f16(d_tmem, x_lo + o, y_hi + o, IDESC_F16_M128_N128, 1u);
-            umma_f16(d_tmem, x_hi + o, y_lo + o, IDESC_F16_M128_N128, 1u);
-          }
-        }
-        umma_commit(&s_full[buf]);
-        if (it >= 2) issue_dx(it - 2);   // two tiles behind: the epilogue of tile it-2 has had two S-MMA times to finish
-      }
-      if (n_iter >= 2) issue_dx(n_iter - 2);
-      issue_dx(n_iter - 1);
+  for (int rr = 0; rr < 2; ++rr) {
+    const long long row = row_a + 8 * rr;   // padded arrays: in range for every row of the block
+    if (BIAS && TRANSPOSED) bias_r[rr] = p.cbias_pad[row];
+    if (!TRANSPOSED) {
+      lse_r[rr] = p.lse_pad[row] - 14.0f * 0.6931471805599453f;  // folds the 2^14 fp16 range scale into the exponent
+      w_r[rr] = p.w_pad[row];                                     // w_i * 2^wst.exp, applied to the dX row at the end
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int grp = ew >> 3, half = (ew >> 2) & 1, quad = ew & 3;
-    const int r_local = quad * 32 + lane;
-    const long long row = (long long)xb * 128 + r_local;
-    const float scale = ldexpf(p.inv_t, -(p.xst->exp + p.yst->exp));  // accumulator -> logit (natural units)
-    float lse_r = 0.f, w_r = 1.f;
-    const float bias_r = (BIAS && TRANSPOSED) ? p.cbias_pad[row] : 0.f;  // padded: in range for every row of the block
-    if (!TRANSPOSED) {  // padded arrays: in range for every row of the block
-      lse_r = p.lse_pad[row] - 14.0f * 0.6931471805599453f;  // folds the 2^14 fp16 range scale into the exponent
-      w_r = p.w_pad[row];                                     // w_i * 2^wst.exp, applied to the dX row at the end
-    }
-    // dX block: 128 rows x 64 columns of fp32 in TMEM; thread = (row, 16 columns).  Chunk k (tiles [8k, 8k+8)) is added
-    // into dacc once its last dX MMA has retired; a warp does that before it waits for a tile >= 3 past the chunk end
-    // (everything that chunk needs was issued before the MMA thread can block on dx_drained: no circular wait).
-    const int c0 = grp * 32 + half * 16;
-    const uint32_t dx_addr = tmem_dx + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0;
-    // running fp32 sum of the drained chunks: 16 values per thread, kept in SHARED memory ([i][epilogue thread]: conflict-free)
-    // -- in registers they pushed the transform loop (64 accumulators + 32 lo words live) past the 96-register budget
-    float* dacc = reinterpret_cast<float*>(smem + 32768 + SB_STAGES * SB_STAGE_BYTES + 1024) + (ew * 32 + lane);
+    if (EXT && p.id_lo) { rid_lo[rr] = p.id_lo[row]; rid_hi[rr] = p.id_hi[row]; }
+  }
+  float dacc[32];   // fp32 sum of the drained chunks (round-to-nearest adds between tensor-core chains)
 #pragma unroll
-    for (int i = 0; i < 16; ++i) dacc[i * 512] = 0.f;
-    int rid_lo = 0, rid_hi = 0;   // id of the stationary row: the positive's id of query `row` (dq) / of candidate `row` (dc)
-    if (EXT && p.id_lo) { rid_lo = p.id_lo[row]; rid_hi = p.id_hi[row]; }
-    const int n_chunks = (n_iter + SB_DRAIN - 1) / SB_DRAIN;
-    int next_chunk = 0;
-    auto drain_until = [&](int t_next) {  // drain every chunk whose last tile is <= t_next - 3
-      while (next_chunk < n_chunks && min(next_chunk * SB_DRAIN + SB_DRAIN - 1, n_iter - 1) + 3 <= t_next) {
-        mbar_wait(dx_full, (uint32_t)(next_chunk & 1));
-        tc_fence_after();
-        uint32_t acc[16];
-        tmem_ld16(dx_addr, acc);
-        tmem_ld_wait16(acc);
+  for (int i = 0; i < 32; ++i) dacc[i] = 0.f;
+  float dx[32];
+
+  mbar_wait(x_full, 0);
+  const uint32_t xa = smem_u32(sX) + c * 8192;
+  const uint64_t x_hi = make_smem_desc(xa), x_lo = make_smem_desc(xa + 16384);
+  for (int it = 0; it < n_iter; ++it) {
+    const int stage = it % SB_STAGES;
+    mbar_wait(&y_full[stage], (uint32_t)((it / SB_STAGES) & 1));
+    const uint32_t y0 = smem_u32(sY + stage * SB_STAGE_BYTES);
+    const uint64_t y_hi = make_smem_desc(y0), y_lo = make_smem_desc(y0 + 16384);
+    // S = X . Y^T: the same three products, in the same order, as the forward pass (q_hi c_hi, q_lo c_hi, q_hi c_lo)
+    float acc[64];
+    wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) dacc[i * 512] += __uint_as_float(acc[i]);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dx_drained);
-        ++next_chunk;
-      }
-    };
-    for (int it = grp; it < n_iter; it += 2) {
-      drain_until(it);
-      const int stage = it % SB_STAGES, buf = it % SB_BUFS;
-      const long long col0 = (t_begin + it) * 128 + half * 64;
-      mbar_wait(&s_full[buf], (uint32_t)((it / SB_BUFS) & 1));
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * 128 + half * 64);
-      uint32_t r[64];
-      tmem_ld64(taddr, r);
-      tmem_ld_wait64(r);
-      if (TRANSPOSED) mbar_wait(&y_full[stage], (uint32_t)((it / SB_STAGES) & 1));  // the tile's lse | w vectors (bulk-copied)
-      const float4* aux4 = reinterpret_cast<const float4*>(sY + stage * SB_STAGE_BYTES + SB_Y_BYTES) + half * 16;
-      const int n_valid = (int)max(0ll, min(64ll, p.n_y_valid - col0));
-      // the positive (query i <-> candidate i) can only sit in the tile whose columns cover this block's rows
-      const bool edge = n_valid < 64 || ((long long)xb * 128 < col0 + 64 && col0 < (long long)xb * 128 + 128);
-      uint32_t lo[32];
-      const float4* cb4 = (BIAS && !TRANSPOSED) ? reinterpret_cast<const float4*>(p.cbias_pad + col0) : nullptr;
-      uint32_t kill0 = 0, kill1 = 0;
-      if (EXT) {
-        if (p.mbits) {
-          const uint2 mw = __ldg(reinterpret_cast<const uint2*>(p.mbits + row * p.mwords + (t_begin + it) * 4 + half * 2));
-          kill0 = ~mw.x; kill1 = ~mw.y;
-        }
-        if (p.id_lo) {
-          const int4* il = reinterpret_cast<const int4*>(p.id_lo + col0);
-#pragma unroll
-          for (int j4 = 0; j4 < 16; ++j4) {
-            const int4 v = __ldg(il + j4);
-            if ((v.x == rid_lo) | (v.y == rid_lo) | (v.z == rid_lo) | (v.w == rid_lo)) {   // rare
-              const int* ih = p.id_hi + col0 + 4 * j4;
-              const long long c = col0 + 4 * j4;
-              uint32_t hit = 0;
-              if (v.x == rid_lo && __ldg(ih + 0) == rid_hi && c + 0 != row) hit |= 1u;
-              if (v.y == rid_lo && __ldg(ih + 1) == rid_hi && c + 1 != row) hit |= 2u;
-              if (v.z == rid_lo && __ldg(ih + 2) == rid_hi && c + 2 != row) hit |= 4u;
-              if (v.w == rid_lo && __ldg(ih + 3) == rid_hi && c + 3 != row) hit |= 8u;
-              if (j4 < 8) kill0 |= hit << (4 * j4); else kill1 |= hit << (4 * (j4 - 8));
-            }
-          }
-        }
-      }
-      if (edge) {
-        const int jd = (row >= col0 && row < col0 + 64) ? (int)(row - col0) : -1;
-        sb_transform<TRANSPOSED, true, BIAS, EXT>(r, lo, scale, lse_r, aux4, n_valid, jd, cb4, bias_r, kill0, kill1);
+    for (int k4 = 0; k4 < 4; ++k4) {
+      const uint64_t o = (uint64_t)(k4 * 2);
+      wgmma_m64n128_ss(acc, x_hi + o, y_hi + o, (uint32_t)(k4 != 0));
+      if (TRANSPOSED) {
+        wgmma_m64n128_ss(acc, x_hi + o, y_lo + o, 1u);
+        wgmma_m64n128_ss(acc, x_lo + o, y_hi + o, 1u);
       } else {
-        sb_transform<TRANSPOSED, false, BIAS, EXT>(r, lo, scale, lse_r, aux4, 64, -1, cb4, bias_r, kill0, kill1);
+        wgmma_m64n128_ss(acc, x_lo + o, y_hi + o, 1u);
+        wgmma_m64n128_ss(acc, x_hi + o, y_lo + o, 1u);
       }
-      tmem_st32(taddr, r);        // hi: columns [0, 32) of this 64-column half
-      tmem_st32(taddr + 32, lo);  // lo: columns [32, 64)
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&g_ready[buf]);
     }
-    drain_until(n_iter + 3 + SB_DRAIN);  // the remaining chunks
-    if (row < p.n_x_rows) {
-      const float gl = p.grad_loss ? p.grad_loss[0] : 1.0f;
-      // transposed: A carried w^ = w 2^wexp per column; otherwise A carried 2^14 and the row weight is applied here
-      const float fs = TRANSPOSED ? ldexpf(gl * p.inv_t, -(p.wst->exp + p.yst->exp))
-                                  : ldexpf(gl * p.inv_t * w_r, -(p.wst->exp + 14 + p.yst->exp));
-      float* dst = p.out + (long long)part * p.part_stride + row * p.d;
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
+
+    // G = (exp(s/T - lse) - diag) * weight, masked entries 0 (see the header); then hi/lo fp16 as wgmma A fragments
+    const long long col0 = (t_begin + it) * 128;
+    const float* lse_s = reinterpret_cast<const float*>(sY + stage * SB_STAGE_BYTES + SB_Y_BYTES);   // TRANSPOSED
+    const float* w_s = lse_s + 128;
+    uint32_t ghi[32], glo[32];
 #pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (c0 + i < p.d) dst[c0 + i] = dacc[i * 512] * fs;
+    for (int i = 0; i < 64; i += 2) {
+      const int rr = (i >> 1) & 1;
+      const long long row = row_a + 8 * rr;
+      float a[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int cl = frag_col(i + e, lane);
+        const long long col = col0 + cl;
+        float lq = lse_r[rr], wq = 16384.f;
+        if (TRANSPOSED) { lq = lse_s[cl]; wq = w_s[cl]; if (BIAS) lq -= bias_r[rr]; }
+        else if (BIAS) lq -= __ldg(p.cbias_pad + col);
+        float pr = ex2_approx(fmaf(acc[i + e], scale, -lq) * SB_LOG2E);
+        if (TRANSPOSED) {
+          if (col == row) pr -= 1.0f;
+          pr *= wq;
+        } else {
+          if (col == row) pr -= 16384.f;
+        }
+        bool keep = col < p.n_y_valid;
+        if (EXT) {
+          if (p.mbits) keep &= ((__ldg(p.mbits + row * p.mwords + (t_begin + it) * 4 + (cl >> 5)) >> (cl & 31)) & 1u) != 0u;
+          if (p.id_lo && __ldg(p.id_lo + col) == rid_lo[rr] && __ldg(p.id_hi + col) == rid_hi[rr] && col != row) keep = false;
+        }
+        a[e] = keep ? pr : 0.f;
+      }
+      const __half2 h = __floats2half2_rn(a[0], a[1]);
+      const float2 hf = __half22float2(h);
+      ghi[i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
+      glo[i >> 1] = pack_half2(a[0] - hf.x, a[1] - hf.y);
+    }
+    // dX += G . Y: K = the tile's 128 rows in 8 steps of 16; the Y tile is the MN-major B operand (d contiguous)
+    const bool first = (it % SB_DRAIN) == 0;
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+      const uint32_t ah[4] = {ghi[4 * kc], ghi[4 * kc + 1], ghi[4 * kc + 2], ghi[4 * kc + 3]};
+      const uint32_t al[4] = {glo[4 * kc], glo[4 * kc + 1], glo[4 * kc + 2], glo[4 * kc + 3]};
+      const uint64_t b_hi = make_smem_desc(y0 + kc * 2048), b_lo = make_smem_desc(y0 + 16384 + kc * 2048);
+      wgmma_m64n64_rs_bmn(dx, ah, b_hi, (uint32_t)(!first || kc != 0));
+      wgmma_m64n64_rs_bmn(dx, al, b_hi, 1u);
+      wgmma_m64n64_rs_bmn(dx, ah, b_lo, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(dx);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&y_empty[stage]);
+    if ((it % SB_DRAIN) == SB_DRAIN - 1 || it == n_iter - 1) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dacc[i] += dx[i];
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == SB_W_ALLOC) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+  const float gl = p.grad_loss ? p.grad_loss[0] : 1.0f;
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const long long row = row_a + 8 * rr;
+    if (row >= p.n_x_rows) continue;
+    // transposed: G carried w^ = w 2^wexp per column; otherwise G carried 2^14 and the row weight is applied here
+    const float fs = TRANSPOSED ? ldexpf(gl * p.inv_t, -(p.wst->exp + p.yst->exp))
+                                : ldexpf(gl * p.inv_t * w_r[rr], -(p.wst->exp + 14 + p.yst->exp));
+    float* dst = p.out + (long long)part * p.part_stride + row * p.d;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if (((i >> 1) & 1) != rr) continue;
+      const int col = frag_col(i, lane);
+      if (col < p.d) dst[col] = dacc[i] * fs;
+    }
+  }
 }
 
 // max |w| (1 when w == NULL) -> the exact power-of-two scale that puts it in [2^13, 2^14)
@@ -446,7 +349,7 @@ extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, in
   TFRS_LAUNCH_CHECK();
   sb_prep_kernel<<<(unsigned)ceil_div(pl.q_tiles * 128, 256), 256, 0, st>>>(lse, sample_weight, B, pl.q_tiles * 128, wst, lse_pad, w_pad);
   TFRS_LAUNCH_CHECK();
-  const size_t smem = 32768 + (size_t)SB_STAGES * SB_STAGE_BYTES + 1024 + 32768 + 256;  // X | Y ring | barriers | dX sums | align slack
+  const size_t smem = 32768 + (size_t)SB_STAGES * SB_STAGE_BYTES + 1024 + 256;  // X | Y ring | align slack | barriers
   TFRS_DYN_SMEM((softmax_tc_bwd_kernel<false, 0>), (int)smem);
   TFRS_DYN_SMEM((softmax_tc_bwd_kernel<true, 0>), (int)smem);
   TFRS_DYN_SMEM((softmax_tc_bwd_kernel<false, 1>), (int)smem);

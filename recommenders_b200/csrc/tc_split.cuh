@@ -1,8 +1,8 @@
-// tc_split.cuh -- exact power-of-two rescale + fp16 hi/lo split images for fp32-parity GEMMs on tcgen05.
+// tc_split.cuh -- exact power-of-two rescale + fp16 hi/lo split images for fp32-parity GEMMs on wgmma.
 //   v = hi + lo,  hi = fp16(v), lo = fp16(v - hi)   (|v - hi - lo| <= 2^-22 |v|);  products are accumulated as
 //   hi*hi + lo*hi + hi*lo in fp32 (the dropped lo*lo term is 2^-22 relative).
 // Image layout: 128-row tiles x 64-wide K slabs, per slab a hi block then a lo block, each 128 rows x 128 B in
-// UMMA SWIZZLE_128B K-major order (16-byte chunk j of row r at chunk j ^ (r & 7)).
+// GMMA SWIZZLE_128B K-major order (16-byte chunk j of row r at chunk j ^ (r & 7)).
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"

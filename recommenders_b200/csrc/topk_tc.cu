@@ -1,4 +1,4 @@
-// topk_tc.cu -- K2: brute-force top-K on the 5th-gen tensor cores (tcgen05 + TMEM + bulk-TMA), sm_100a.
+// topk_tc.cu -- K2: brute-force top-K on the Hopper tensor cores (wgmma + bulk-TMA + mbarrier), sm_90a.
 //
 // Replaces  scores = matmul(q, c^T); top_k(scores, k)  (layers/factorized_top_k.py:603-605) for large
 // corpora.  The [Q,N] score matrix never exists in HBM:
@@ -12,7 +12,7 @@
 //                    registers) takes the K-th largest bin maximum L_q: K distinct bins hold K distinct candidates
 //                    >= L_q, so L_q is a valid lower bound of the K-th best screening score
 //                (2) tc_scan<FILTER> : screening GEMM over the whole corpus; epilogue compares the fp32
-//                    accumulators (read from TMEM) with T_q = L_q - margin_q and appends the rare
+//                    accumulators (in registers) with T_q = L_q - margin_q and appends the rare
 //                    survivors (octet records) to per-(query, part, half) lists -- nothing else leaves the SM
 //                (3) tc_finalize (a warp per query, no block barriers): tau = K-th best screening score; survivors
 //                    within the error band of tau are re-scored EXACTLY (sequential fp32 fmaf chain on the fp32
@@ -27,13 +27,11 @@
 // of the exact top-K has screening score >= tau - 2*eps_q >= L_q - 2*eps_q, so it is in the list and in
 // the re-scored band.
 //
-// Scan kernel shape (per CTA, 1 CTA / SM, 640 threads): 256 queries (two 128-row A blocks, resident in smem)
-// x a contiguous range of 128-row corpus tiles streamed through a 4-6 stage bulk-TMA ring; warp 0 = TMA
-// producer, warp 1 = MMA issuer (one thread, tcgen05.mma M=128 N=128 K=16, fp16 -> fp32 in TMEM),
-// warp 2 = TMEM allocator, warps 4-19 = epilogue (one query row x 64 columns per thread, tcgen05.ld 32x32b.x64).
-// TMEM holds 2 A-blocks x 2 buffers x 128 columns = all 512 columns, so tile t+1's MMAs overlap tile
-// t's epilogue.  Each B tile feeds two MMAs (both A blocks): 16 KB of L2->smem traffic per 512
-// tensor-core cycles keeps the chip under the ~6.3 KB/clk L2 fabric limit.
+// Scan kernel shape (per CTA, 1 CTA / SM, 544 threads): 256 queries (two 128-row A blocks, resident in smem)
+// x a contiguous range of 128-row corpus tiles streamed through a 4-6 stage bulk-TMA ring; warp 16 = TMA
+// producer (one thread), warpgroups 0-3 = one 64-query slice each: wgmma m64n128k16 (fp16 -> fp32 in registers),
+// then the epilogue on the register fragment.  The four consumer warpgroups run independently, so one's MMAs
+// overlap another's epilogue; each B tile in smem feeds all four (256 query rows per 16 KB of L2->smem traffic).
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
@@ -49,16 +47,15 @@ constexpr int QBLK = 256;            // queries per CTA (2 A blocks)
 constexpr int KSLAB = 64;            // fp16 elements per 128-byte swizzle row
 constexpr int SLAB_BYTES = TILE_N * 128;  // 16 KB: 128 rows x 128 B
 constexpr int HEADER_BYTES = 1024;
-constexpr int THREADS = 640;      // 4 control warps + 16 epilogue warps (4 per SM sub-partition)
-constexpr int EPI_WARPS = 16;
-constexpr int EPI_WARP0 = 4;
+constexpr int THREADS = 544;         // 4 consumer warpgroups + 1 producer warp
+constexpr int CONSUMER_WARPS = 16;
 constexpr int CAND_CAP = 2048;       // octet records kept per query across all segments (sizing of cap_part)
 constexpr int MAX_SAMPLE_STRIDE = 4;
-constexpr int FIN_MAX_PARTS = 2 * 148;  // survivor-list segments per query: (corpus part, column half)
+constexpr int FIN_MAX_PARTS = 2 * 132;  // survivor-list segments per query: (corpus part, column half); parts <= SMs
 constexpr int MAX_BINS = 1024;       // bin maxima per query (32 per lane of the threshold warp)
 constexpr int FP16_TARGET = 15;      // largest operand magnitude lands in [2^14, 2^15)
 // Screening error model (operands: fp16 after an exact power-of-two rescale -- one exponent for the whole corpus,
-// one per query row -- so that the largest magnitude lands in [2^14, 2^15); accumulate: fp32 in TMEM):
+// one per query row -- so that the largest magnitude lands in [2^14, 2^15); accumulate: fp32 in registers):
 //   |x^ - x| <= 2^-11 |x| (+2^-25 absolute below the fp16 normal range, negligible after the rescale)
 //   => |screen - exact| <= (2^-10 + 2^-22) sum|q_k c_k|  + accumulation slack (budget 2^-14) + fmaf-chain 2^-16
 //   <= E_REL * |q| * |c|   (Cauchy-Schwarz), E_REL = 0.00108 including the 0.1 % norm inflation.
@@ -213,7 +210,6 @@ struct ScanParams {
   float* cand_s;                  // [Qp, parts, 2, cap_part, 8] screening scores of the octet
   unsigned int* cand_i;           // [Qp, parts, 2, cap_part]    local index of the octet's first column
   int cap_part;                   // records per segment
-  uint32_t idesc;
 };
 
 template <int KB, int STAGES, int MODE>
@@ -228,31 +224,23 @@ tc_scan_kernel(const ScanParams p) {
   uint64_t* full = bars;                 // [STAGES]
   uint64_t* empty = bars + STAGES;       // [STAGES]
   uint64_t* a_full = bars + 2 * STAGES;  // [1]
-  uint64_t* t_full = a_full + 1;         // [2]
-  uint64_t* t_empty = t_full + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
   const int u_begin = (int)((long long)part * p.n_seq / p.parts);
   const int u_end = (int)((long long)(part + 1) * p.n_seq / p.parts);
   const int n_iter = u_end - u_begin;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
     mbar_init(a_full, 1);
-    for (int b = 0; b < 2; ++b) { mbar_init(&t_full[b], 1); mbar_init(&t_empty[b], EPI_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 4) {
     // ===== bulk-TMA producer =====
-    if (lane == 0) {
+    if (threadIdx.x == 512) {
       mbar_expect_tx(a_full, 2 * KB * SLAB_BYTES);
       bulk_g2s(sA, p.qimg + (long long)qb * 2 * KB * SLAB_BYTES, 2 * KB * SLAB_BYTES, a_full);
       int stage = 0; uint32_t phase = 0;
@@ -268,133 +256,117 @@ tc_scan_kernel(const ScanParams p) {
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (single thread) =====
-    if (lane == 0) {
-      mbar_wait(a_full, 0);
-      tc_fence_after();
-      int stage = 0; uint32_t phase = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        const int buf = it & 1;
-        const uint32_t tphase = (it >> 1) & 1;
-        mbar_wait(&t_empty[buf], tphase ^ 1);   // epilogue drained this accumulator buffer
-        mbar_wait(&full[stage], phase);         // B tile landed
-        tc_fence_after();
+    return;
+  }
+
+  // ===== consumers: warpgroup c computes the 64 query rows [64 c, 64 c + 64) of the CTA's 256 against each tile and runs
+  // the epilogue on its register fragment: a thread holds rows r and r + 8 x 32 columns (pairs 8j + 2(lane%4) + {0,1});
+  // the 4 lanes of a quad together hold 8 consecutive columns of a row -- one octet record.
+  const int c = wg;
+  const long long row_a = (long long)qb * QBLK + c * 64 + warp * 16 + (lane >> 2);   // rows row_a, row_a + 8
+  const bool quad_leader = (lane & 3) == 0;
+  float thr[2] = {INFINITY, INFINITY};
+  if (MODE == MODE_FILTER) {
 #pragma unroll
-        for (int ab = 0; ab < 2; ++ab) {
-          const uint32_t d_tmem = tmem_base + (uint32_t)((ab * 2 + buf) * TILE_N);
+    for (int rr = 0; rr < 2; ++rr) if (row_a + 8 * rr < p.Q) thr[rr] = p.thr[row_a + 8 * rr];
+  }
+  const unsigned int cap = (unsigned int)p.cap_part;
+  unsigned int cnt[4] = {0u, 0u, 0u, 0u}, ovf = 0u;      // segment s = (row rr, column half h) = 2 rr + h
+  float binm[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+  int in_group = 0, bin_out = 0;
+
+  mbar_wait(a_full, 0);
+  // this warpgroup's 64-row slice of A block c/2 (image layout [block][K slab][16 KB]): 8 swizzle groups of 1024 B
+  const uint32_t a0 = smem_u32(sA + (c >> 1) * KB * SLAB_BYTES + (c & 1) * 8192);
+  int stage = 0; uint32_t phase = 0;
+  for (int it = 0; it < n_iter; ++it) {
+    const int u = u_begin + it;
+    const long long tile = (long long)u * p.stride;
+    const long long col0 = tile * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
+    mbar_wait(&full[stage], phase);
+    float acc[64];
+    wgmma_fence();
 #pragma unroll
-          for (int kb = 0; kb < KB; ++kb) {
-            const uint64_t a_desc = make_smem_desc(smem_u32(sA + (ab * KB + kb) * SLAB_BYTES));
-            const uint64_t b_desc = make_smem_desc(smem_u32(sB + (stage * KB + kb) * SLAB_BYTES));
+    for (int kb = 0; kb < KB; ++kb) {
+      const uint64_t a_desc = make_smem_desc(a0 + kb * SLAB_BYTES);
+      const uint64_t b_desc = make_smem_desc(smem_u32(sB + (stage * KB + kb) * SLAB_BYTES));
 #pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4)  // 4 x (K=16 fp16 = 32 B) inside the 128-byte swizzle row
-              umma_f16(d_tmem, a_desc + (uint64_t)(k4 * 2), b_desc + (uint64_t)(k4 * 2), p.idesc,
-                        (uint32_t)((kb | k4) != 0));
-          }
+      for (int k4 = 0; k4 < 4; ++k4)  // 4 x (K=16 fp16 = 32 B) inside the 128-byte swizzle row
+        wgmma_m64n128_ss(acc, a_desc + (uint64_t)(k4 * 2), b_desc + (uint64_t)(k4 * 2), (uint32_t)((kb | k4) != 0));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have retired: the smem slot may be refilled
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+
+    if (MODE != MODE_FILTER) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) binm[2 * rr + (j >> 3)] = max3(binm[2 * rr + (j >> 3)], acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+      if (++in_group == p.group || it == n_iter - 1) {   // close the bin after `group` tiles (loop-uniform)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) {
+          const float m = quad_max(binm[s]);
+          const long long row = row_a + 8 * (s >> 1);
+          if (quad_leader && row < p.Q)
+            p.binmax[row * p.bins_ld + (long long)part * p.bins_per_part * 2 + (s & 1) + 2 * bin_out] = m;
+          binm[s] = -INFINITY;
         }
-        umma_commit(&empty[stage]);   // smem slot free once these MMAs retire
-        umma_commit(&t_full[buf]);    // accumulators ready for the epilogue
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        ++bin_out; in_group = 0;
       }
-    }
-  } else if (warp >= EPI_WARP0) {
-    // ===== epilogue: one query row per thread =====
-    // 16 epilogue warps: (column half, A block, TMEM lane quadrant); a thread owns one query row x 64 columns of
-    // every tile, so four warps per scheduler overlap their TMEM-load latency with each other's math.
-    const int ew = warp - EPI_WARP0;       // 0..15
-    const int half = ew >> 3, ab = (ew >> 2) & 1, quad = ew & 3;  // TMEM lane quadrant == warp % 4
-    const long long row = (long long)qb * QBLK + ab * TILE_M + quad * 32 + lane;
-    const bool row_ok = row < p.Q;
-    float thr = INFINITY;
-    if (MODE == MODE_FILTER && row_ok) thr = p.thr[row];
-    float* my_s = nullptr; unsigned int* my_i = nullptr;
-    unsigned int my_cnt = 0, my_ovf = 0;
-    const unsigned int cap = (unsigned int)p.cap_part;
-    if (MODE == MODE_FILTER) {
-      const long long seg = (((long long)row * p.parts + part) * 2 + half) * p.cap_part;
-      my_s = p.cand_s + seg * 8; my_i = p.cand_i + seg;
-    }
-    float binm = -INFINITY;
-    int in_group = 0, bin_out = 0;
-    float* my_bins = nullptr;
-    if (MODE == MODE_SAMPLE) my_bins = p.binmax + row * p.bins_ld + (long long)part * p.bins_per_part * 2 + half;
-    for (int it = 0; it < n_iter; ++it) {
-      const int buf = it & 1;
-      const uint32_t tphase = (it >> 1) & 1;
-      const int u = u_begin + it;
-      const long long tile = (long long)u * p.stride;
-      const long long col0 = tile * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
-      mbar_wait(&t_full[buf], tphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((ab * 2 + buf) * TILE_N);
-      {
-        const int h = half;
-        uint32_t r[64];
-        tmem_ld64(taddr + h * 64, r);
-        tmem_ld_wait64(r);
-        // this warp's TMEM reads of the accumulator buffer are complete: release it before the math
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&t_empty[buf]);
+    } else {
+      // Each lane marks the octets (row rr, column group j) where one of its two scores passes; one warp-wide OR of those
+      // 32-bit masks leaves the few octets that any lane of the warp hit (a warp of 16 rows meets a survivor in most tiles,
+      // but in few of its 32 octet slots).  Only those take a ballot, which makes the decision quad-uniform; each lane of a
+      // surviving octet stores its two scores, the quad leader the octet's first index.
+      unsigned int mine = 0u;
 #pragma unroll
-        for (int c2 = 0; c2 < 2; ++c2) {
-          float v[32];
+      for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[c2 * 32 + j]);
-          // 4 quarter maxima of 8, then their max (FMNMX3 trees)
-          float qmx[4];
+        for (int j = 0; j < 16; ++j)
+          mine |= (fmaxf(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]) >= thr[rr]) ? (1u << (16 * rr + j)) : 0u;
+      const unsigned int hit = __reduce_or_sync(0xffffffffu, mine);
+      if (hit) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            qmx[i] = max3(max3(v[8 * i], v[8 * i + 1], v[8 * i + 2]), max3(v[8 * i + 3], v[8 * i + 4], v[8 * i + 5]),
-                          fmaxf(v[8 * i + 6], v[8 * i + 7]));
-          const float m = fmaxf(max3(qmx[0], qmx[1], qmx[2]), qmx[3]);
-          if (MODE != MODE_FILTER) {
-            binm = fmaxf(binm, m);
-          } else {
-            // Survivors are rare.  Every branch below is WARP-UNIFORM: one vote on the chunk max, then one
-            // REDUX.OR of the per-lane 4-bit quarter mask; the per-lane work is predicated stores only.
-            if (__any_sync(0xffffffffu, m >= thr)) {
-              unsigned int qmask = 0;
+        for (int rr = 0; rr < 2; ++rr) {
+          const long long seg_row = ((row_a + 8 * rr) * p.parts + part) * 2;
 #pragma unroll
-              for (int i = 0; i < 4; ++i) qmask |= (qmx[i] >= thr) ? (1u << i) : 0u;
-              const unsigned int umask = __reduce_or_sync(0xffffffffu, qmask);
-              const bool room = my_cnt + 4u <= cap;    // worst case of this visit (4 octets) fits
-              my_ovf |= (!room && m >= thr) ? 1u : 0u;
-              const unsigned int idx0 = (unsigned int)(col0 + h * 64 + c2 * 32);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                if (umask & (1u << i)) {             // uniform: some lane's octet i has a survivor
-                  if (room && qmx[i] >= thr) {       // per lane: append my whole octet (predicated, no loop)
-                    float4* dst = reinterpret_cast<float4*>(my_s + (size_t)my_cnt * 8);
-                    dst[0] = make_float4(v[8 * i], v[8 * i + 1], v[8 * i + 2], v[8 * i + 3]);
-                    dst[1] = make_float4(v[8 * i + 4], v[8 * i + 5], v[8 * i + 6], v[8 * i + 7]);
-                    my_i[my_cnt] = idx0 + 8 * i;
-                    ++my_cnt;
-                  }
-                }
+          for (int j = 0; j < 16; ++j) {
+            if (!((hit >> (16 * rr + j)) & 1u)) continue;   // warp-uniform
+            const float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
+            const unsigned int vote = __ballot_sync(0xffffffffu, (mine >> (16 * rr + j)) & 1u);
+            if ((vote >> (lane & ~3)) & 0xFu) {
+              const int s = 2 * rr + (j >> 3);
+              if (cnt[s] < cap) {
+                const long long seg = (seg_row + (j >> 3)) * p.cap_part + cnt[s];
+                reinterpret_cast<float2*>(p.cand_s + seg * 8)[lane & 3] = make_float2(v0, v1);
+                if (quad_leader) p.cand_i[seg] = (unsigned int)(col0 + 8 * j);
+                ++cnt[s];
+              } else {
+                ovf |= 1u << s;
               }
             }
           }
         }
       }
-      if (MODE == MODE_SAMPLE) {   // close the bin after `group` tiles (loop-uniform)
-        if (++in_group == p.group || it == n_iter - 1) {
-          if (row_ok) my_bins[2 * bin_out] = binm;
-          ++bin_out; in_group = 0; binm = -INFINITY;
-        }
-      }
-    }
-    if (MODE == MODE_SAMPLE) {
-      if (row_ok) for (; bin_out < p.bins_per_part; ++bin_out) my_bins[2 * bin_out] = -INFINITY;  // bins this part did not fill
-    } else {
-      p.count[((long long)row * p.parts + part) * 2 + half] = my_ovf ? (cap + 1u) : my_cnt;
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+  if (MODE == MODE_SAMPLE) {
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {   // bins this part did not fill
+      const long long row = row_a + 8 * (s >> 1);
+      if (quad_leader && row < p.Q)
+        for (int b = bin_out; b < p.bins_per_part; ++b)
+          p.binmax[row * p.bins_ld + (long long)part * p.bins_per_part * 2 + (s & 1) + 2 * b] = -INFINITY;
+    }
+  } else if (quad_leader) {
+#pragma unroll
+    for (int s = 0; s < 4; ++s)
+      p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] = ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1095,7 +1067,6 @@ static int run_call(const Call& c) {
   sp.qimg = qimg; sp.cimg = cimg; sp.Q = c.Q; sp.N = c.N; sp.nqb = pl.nqb; sp.n_tiles = pl.n_tiles;
   sp.binmax = binmax; sp.bins_ld = pl.bins_ld; sp.group = pl.group; sp.bins_per_part = pl.bins_per_part;
   sp.thr = thr; sp.count = count; sp.cand_s = cand_s; sp.cand_i = cand_i; sp.cap_part = pl.cap_part;
-  sp.idesc = IDESC_F16_M128_N128;
   prof_mark(st, 1);
   // (1) sampled pass -> bin maxima -> k-th largest -> threshold
   int rc = launch_scan_mode(pl, sp, st, MODE_SAMPLE);

@@ -1,8 +1,8 @@
-"""Top-K retrieval layers: the B200 mirror of tensorflow_recommenders/layers/factorized_top_k.py.
+"""Top-K retrieval layers: the H100 mirror of tensorflow_recommenders/layers/factorized_top_k.py.
 
 Same classes, constructor arguments, method names and error behaviour as the reference
 (`TopK` :140-333, `Streaming` :336-512, `BruteForce` :515-610, `ScaNN` stub :613-796); tensors are CUDA
-`torch.Tensor`s and the arithmetic runs in libtfrs_b200.so (exact fp32 scan or tcgen05 screening +
+`torch.Tensor`s and the arithmetic runs in libtfrs_b200.so (exact fp32 scan or wgmma screening +
 exact rescoring).  Results follow tf.math.top_k's contract: scores descending, ties -> lower index.
 """
 from __future__ import annotations
@@ -265,7 +265,7 @@ class Streaming(TopK):
   """Retrieves K highest scoring items and their ids from a large dataset (factorized_top_k.py:336-512).
 
   Dataset batches (the README uses 128 rows) are coalesced into chunks of `_coalesce_rows`; every chunk is scanned by
-  the tcgen05 screening kernel (its fp16 image is built on the fly) with the running row counter as index offset and
+  the wgmma screening kernel (its fp16 image is built on the fly) with the running row counter as index offset and
   merged into the carried [Q,k] state -- ties resolve to the lower running index, i.e. state first (:462-463), so the
   result equals BruteForce's.  Batches that live in host memory are staged through pinned double buffers so the copy of
   chunk i+1 overlaps the scan of chunk i (corpora larger than HBM).  Small chunks use the exact CUDA-core scan, which

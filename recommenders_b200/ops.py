@@ -93,7 +93,7 @@ def topk_scan(q: torch.Tensor, corpus: torch.Tensor, k: int, index_offset: int =
 
 
 def index_build(corpus: torch.Tensor, reuse_slot: Optional[str] = None) -> torch.Tensor:
-  """Builds the tensor-core screening image (fp16 UMMA tiles + norm bound) of a corpus.  `reuse_slot` builds it in a
+  """Builds the tensor-core screening image (fp16 GMMA tiles + norm bound) of a corpus.  `reuse_slot` builds it in a
   per-stream scratch buffer instead of a fresh allocation (Streaming's per-chunk images)."""
   corpus = f32c(corpus, "candidates")
   N, d = corpus.shape
@@ -107,7 +107,7 @@ def index_build(corpus: torch.Tensor, reuse_slot: Optional[str] = None) -> torch
 
 def topk_tc(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor, k: int, index_offset: int = 0,
             out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-  """tcgen05 screening + exact rescoring; bit-identical to topk_scan."""
+  """wgmma screening + exact rescoring; bit-identical to topk_scan."""
   q = f32c(q, "queries"); corpus = f32c(corpus, "candidates")
   Q, d = q.shape; N = corpus.shape[0]
   if out is None:

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on a B200)")
+  config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

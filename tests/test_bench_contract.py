@@ -1,4 +1,4 @@
-"""The committed bench lines (profiles/r02_bench_n1_final.json = `python bench.py`, r02_bench_reference_arm.json =
+"""The committed bench lines (profiles/h100_bench_n1.json = `python bench.py`, h100_bench_reference_arm.json =
 `python bench.py --impl reference`) carry every key of the bench contract and are internally consistent."""
 import json
 import os
@@ -12,7 +12,7 @@ def _load(name):
 
 
 def test_committed_bench_line_follows_the_contract():
-  d = _load("r02_bench_n1_final.json")
+  d = _load("h100_bench_n1.json")
   for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
               "dtype", "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline", "outputs_match_oracle"):
     assert key in d, key
@@ -35,9 +35,9 @@ def test_committed_bench_line_follows_the_contract():
 
 
 def test_committed_reference_arm_line():
-  r = _load("r02_bench_reference_arm.json")
+  r = _load("h100_bench_reference_arm.json")
   assert r["impl"] == "reference" and r["gpu_launches"] == 0
   assert r["e2e"]["h2d_bytes_per_step"] == 0 and r["e2e"]["d2h_bytes_per_step"] == 0 and r["e2e"]["value"] == r["value"]
   assert r["cpu_baseline"]["value"] == r["value"] and r["cpu_baseline"]["cores"] >= 1
-  ours = _load("r02_bench_n1_final.json")
+  ours = _load("h100_bench_n1.json")
   assert r["metric"] == ours["metric"] and r["unit"] == ours["unit"] and r["config"]["workload"] == ours["config"]["workload"]

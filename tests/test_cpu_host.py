@@ -37,11 +37,11 @@ def test_library_builds_and_exports_every_declared_symbol():
   assert l.tfrs_launch_count() == 0
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
   from recommenders_b200 import build
   out = subprocess.run(["cuobjdump", "-lelf", build.build()], capture_output=True, text=True).stdout
   archs = set(re.findall(r"sm_(\d+a?)", out))
-  assert archs == {"100a"}, archs
+  assert archs == {"90a"}, archs
 
 
 def test_no_cpu_fallback():

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): every kernel of libtfrs_b200.so, called through the C ABI
+"""GPU parity tests (run with -m gpu on an H100): every kernel of libtfrs_b200.so, called through the C ABI
 (via recommenders_b200.ops), against the CPU oracle on the same seeded inputs.
 Bar: bit-exact for scores / indices / gathered rows / Adagrad state; 1e-5 relative for the fp32
 softmax loss, its gradients and the Cross layer (tolerance stated per test)."""
@@ -172,7 +172,7 @@ def test_errors_cross_the_abi(ops):
 
 
 def test_cross_tensor_core_matches_cuda_core(ops):
-  """The tcgen05 Cross forward (fp16 hi/lo split) against the exact CUDA-core kernel: 1e-5 of the output scale."""
+  """The wgmma Cross forward (fp16 hi/lo split) against the exact CUDA-core kernel: 1e-5 of the output scale."""
   rng = np.random.RandomState(0)
   B, D = 8192, 845
   x0 = cu(rng.uniform(size=(B, D)).astype(np.float32)); x = cu(rng.normal(size=(B, D)).astype(np.float32))
@@ -216,7 +216,7 @@ def test_gather_uniform_tables_fast_path(ops, idt):
                                                        (1024, 1024, 64, None, False, 0.5), (700, 9000, 100, 0.05, True, 0.1),
                                                        (2500, 2500, 32, None, True, 1.0)])
 def test_inbatch_softmax_tensor_core_forward(ops, B, C, d, temp, weighted, scale):
-  """tcgen05 forward (hi/lo fp16 split, online log-sum-exp epilogue) vs the float64 oracle: 1e-5 relative on the
+  """wgmma forward (hi/lo fp16 split, online log-sum-exp epilogue) vs the float64 oracle: 1e-5 relative on the
   loss, 1e-5 absolute-or-relative on every row's logsumexp; and it must agree with the exact CUDA-core forward."""
   rng = np.random.RandomState(B + C + d)
   q = rng.normal(size=(B, d)).astype(np.float32) * scale; c = rng.normal(size=(C, d)).astype(np.float32) * scale
@@ -245,7 +245,7 @@ def test_inbatch_softmax_tensor_core_forward(ops, B, C, d, temp, weighted, scale
                                                        (700, 5000, 40, 0.05, True, 0.1), (2500, 2500, 32, None, True, 1.5),
                                                        (1300, 1300, 64, 0.1, True, 0.3)])
 def test_inbatch_softmax_tensor_core_backward(ops, B, C, d, temp, weighted, scale):
-  """tcgen05 backward (S = X.Y^T, G written back into TMEM, dX += G.Y with G from TMEM) vs the float64 oracle:
+  """wgmma backward (S = X.Y^T in registers, dX += G.Y with G as the register A operand) vs the float64 oracle:
   1e-5 of the gradient scale on dq and dc, with lse from the tensor-core forward and a non-unit upstream gradient."""
   rng = np.random.RandomState(B + C + d + 1)
   q = rng.normal(size=(B, d)).astype(np.float32) * scale; c = rng.normal(size=(C, d)).astype(np.float32) * scale

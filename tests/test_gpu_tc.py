@@ -1,4 +1,4 @@
-"""GPU parity tests of the tensor-core top-K path (tcgen05 screening + exact re-scoring), through the C ABI.
+"""GPU parity tests of the tensor-core top-K path (wgmma screening + exact re-scoring), through the C ABI.
 Bar: bit-exact ids and scores against the CPU oracle and against the exact CUDA-core path."""
 import numpy as np
 import pytest

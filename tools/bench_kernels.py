@@ -18,7 +18,7 @@ try:
   peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
 except Exception:
   pass
-HBM = peaks.get("hbm_gbs", 6650.0)
+HBM = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet when not measured
 
 
 def timeit(fn, iters=20, warm=5):
@@ -83,7 +83,7 @@ def cross3():
 with torch.no_grad():
   t = timeit(cross3, iters=5 if not quick else 3, warm=2)
 flops = 3 * 2.0 * B * Dc * Dc
-out["cfg5_cross_fwd_3layers"] = {"seconds": t, "TFLOPs": flops / t / 1e12, "flops": flops, "path": "tcgen05 fp16 hi/lo split GEMM + fused epilogue (B>=1024), exact CUDA-core SGEMM otherwise"}
+out["cfg5_cross_fwd_3layers"] = {"seconds": t, "TFLOPs": flops / t / 1e12, "flops": flops, "path": "wgmma fp16 hi/lo split GEMM + fused epilogue (B>=1024), exact CUDA-core SGEMM otherwise"}
 # one Cross layer forward + backward (the training step's share), then the low-rank variants (p = 256) -- SURVEY 8f-4
 go = torch.randn((B, Dc), generator=g, device=dev)
 def cross_fb():
@@ -109,7 +109,7 @@ with torch.no_grad():
   t0 = timeit(lowrank3_unfused, iters=3, warm=1)
 fl = 3 * 2 * 2.0 * B * Dc * P
 out["cfg5_multilayer_dcn_p256_fwd_3layers"] = {"seconds": t, "TFLOPs": fl / t / 1e12, "flops": fl, "unfused_cuda_core_seconds": t0,
-                                               "path": "2 tcgen05 split-fp16 GEMMs per layer, cross formula in the second one's epilogue"}
+                                               "path": "2 wgmma split-fp16 GEMMs per layer, cross formula in the second one's epilogue"}
 def lowrank_fb():
   ys = [t.detach().requires_grad_(True) for t in (x0, x0, Us[0], Vs[0], bs[0])]
   ops.cross_lowrank(ys[0], ys[1], ys[2], ys[3], ys[4], 0.0).backward(go)
@@ -149,7 +149,7 @@ def softmax_fwd_bwd():
 
 t = timeit(softmax_fwd_bwd, iters=5 if not quick else 3, warm=2)
 out["cfg3_inbatch_softmax_fwd_bwd"] = {"seconds": t, "TFLOPs": 8.0 * Bt * Bt * d / t / 1e12, "flops": 8.0 * Bt * Bt * d,
-                                       "path": "tcgen05 split-fp16 forward (online log-sum-exp) + tcgen05 backward (G in TMEM)"}
+                                       "path": "wgmma split-fp16 forward (online log-sum-exp) + wgmma backward (G as the register A operand)"}
 with torch.no_grad():
   t = timeit(lambda: ops.inbatch_softmax_tc(qe, ce), iters=10, warm=3)
   out["cfg3_inbatch_softmax_fwd_only"] = {"seconds": t, "TFLOPs": 2.0 * Bt * Bt * d / t / 1e12}
