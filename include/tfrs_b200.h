@@ -377,6 +377,59 @@ int tfrs_cross_lowrank_tc_bwd_f32(const float* x0, const float* x, const float* 
                                   void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K6  Dense layer (tf.keras.layers.Dense inside layers/blocks.py:24-61 MLP and the ranking models,
+ * experimental/models/ranking.py:27-257):   y = act(x . W + bias)
+ *   x [B,K], W [K,N] ([in,out], Keras layout), bias [N] nullable, act = TFRS_ACT_*.
+ * Tensor cores (B >= 1024, K >= 64, N >= 64; tfrs_dense_uses_tc): the split-fp16 wgmma GEMM of the Cross backward with
+ * bias + activation in the epilogue (fp32 parity, ~2^-21 relative); K > 1024 is accumulated in chunks of 1024, summed in
+ * fixed order, and the bias + activation applied in that reduction.  Otherwise exact CUDA-core kernels: every output is
+ * the canonical sequential fmaf chain over k from +0.0f, then + bias, then the activation (a warp per row when N <= 16).
+ * `logits` (nullable, [B,N]) receives z = x.W + bias when act is sigmoid: the binary cross-entropy of a sigmoid output
+ * is computed from it (tf-keras `_keras_logits`).
+ * Backward from the saved OUTPUT y:  dz = dy * act'(y) + dlogits  (relu' = [y > 0], sigmoid' = y (1 - y); dy and dlogits
+ * are nullable, at least one is given);  db = colsum(dz);  dx = dz . W^T;  dW = x^T . dz (batch chunks, fixed-order sum).
+ * dx / dW / db are nullable.  Deterministic, no float atomics.
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_ACT_LINEAR = 0, TFRS_ACT_RELU = 1, TFRS_ACT_SIGMOID = 2 };
+int tfrs_dense_uses_tc(int64_t B, int K, int N);
+size_t tfrs_dense_fwd_workspace_bytes(int64_t B, int K, int N);
+int tfrs_dense_fwd_f32(const float* x, const float* W, const float* bias, int64_t B, int K, int N, int activation, float* y,
+                       float* logits, void* ws, size_t ws_bytes, void* stream);
+size_t tfrs_dense_bwd_workspace_bytes(int64_t B, int K, int N);
+int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y, const float* dy, const float* dlogits, int64_t B, int K,
+                       int N, int activation, float* dx, float* dW, float* dbias, void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Ranking loss + metrics (tasks/ranking.py:26-119 with the tf.keras losses / metrics the tutorials pass).
+ * One pass over the B predictions computes the per-example loss, the reduced loss (fixed-order reduction to a device
+ * scalar) and, in the same launch, the batch statistics of the ranking metrics:
+ *   loss_kind TFRS_LOSS_BCE         BinaryCrossentropy(from_logits=False): p = clip(pred, 1e-7, 1 - 1e-7),
+ *                                   l = -(y log(p + 1e-7) + (1 - y) log(1 - p + 1e-7))
+ *             TFRS_LOSS_BCE_LOGITS  BinaryCrossentropy on logits: l = max(z, 0) - z y + log1p(exp(-|z|))
+ *             TFRS_LOSS_MSE         MeanSquaredError: l = (pred - y)^2
+ *   reduction TFRS_REDUCTION_NONE (per_example only), _SUM (sum_i w_i l_i), _SUM_OVER_BATCH_SIZE (sum_i w_i l_i / B).
+ * `loss_in` is what the loss reads (the logits for BCE_LOGITS), `pred` what the metrics read; weights nullable (= 1).
+ * stats (nullable, float64 [TFRS_RANKING_STATS + 2 T]) is WRITTEN with this batch's totals:
+ *   [0] sum w   [1] sum w [(pred > threshold) == y]   [2] sum w pred   [3] sum w y   [4] sum w (pred - y)^2
+ *   [5 .. 5+T) sum w y per AUC bucket, [5+T .. 5+2T) sum w (1 - y) per bucket; bucket = max(ceil(pred (T-1)) - 1, 0)
+ *   (tf-keras AUC's evenly-spaced-threshold update, num_thresholds = T).  Per-block partials, fixed-order sums.
+ * Backward: dL/d loss_in = g * w * dl/dx (* 1/B for SUM_OVER_BATCH_SIZE); g is a device scalar, or [B] for NONE.
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_LOSS_BCE = 0, TFRS_LOSS_BCE_LOGITS = 1, TFRS_LOSS_MSE = 2 };
+enum { TFRS_REDUCTION_NONE = 0, TFRS_REDUCTION_SUM = 1, TFRS_REDUCTION_SUM_OVER_BATCH_SIZE = 2 };
+#define TFRS_RANKING_STATS 5
+size_t tfrs_ranking_workspace_bytes(int64_t B, int num_thresholds);
+int tfrs_ranking_loss_fwd_f32(const float* loss_in, const float* pred, const float* labels, const float* weights, int64_t B,
+                              int loss_kind, int reduction, float* per_example, float* loss, double* stats, float threshold,
+                              int num_thresholds, void* ws, size_t ws_bytes, void* stream);
+int tfrs_ranking_loss_bwd_f32(const float* loss_in, const float* labels, const float* weights, int64_t B, int loss_kind,
+                              int reduction, const float* grad, float* dloss_in, void* stream);
+/* The metric statistics alone (a loss the library does not own) -- same layout and numbers as above.  The caller's metric
+ * objects add them into their device-resident sums; nothing synchronises. */
+int tfrs_ranking_metrics_f32(const float* pred, const float* labels, const float* weights, int64_t B, double* stats,
+                                    float threshold, int num_thresholds, void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DLRM DotInteraction (layers/feature_interaction/dot_interaction.py:53-104; SURVEY 8f-4): feats [B,F,d] ->
  * pairwise dots e_i.e_j of every sample; output = lower triangle in (i,j) row-major order without
  * (self_interaction=0) or with the diagonal, [B, out_dim], or the full [B,F*F] matrix with the excluded part

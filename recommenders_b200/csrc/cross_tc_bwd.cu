@@ -16,6 +16,7 @@
 #include "tc_ptx.cuh"
 #include "tc_split.cuh"
 #include "cross_tc.cuh"
+#include "dense.cuh"
 
 namespace tfrs {
 namespace tc {
@@ -24,7 +25,8 @@ constexpr int SG_THREADS2 = 544;
 constexpr int SG_STAGES2 = 2;
 constexpr int SG_STAGE_BYTES = 6 * 16384;  // A: 2 blocks x (hi, lo); B: (hi, lo)
 constexpr int DW_CHUNK_SLABS = 16;         // 1024 batch rows per accumulation chain
-enum { SG_DX = 1, SG_DW = 2, SG_PLAIN = 3, SG_CROSS = 4 };
+// SG_DENSE + act: the Dense layer (K6), y = act(acc + bias); SG_DENSE + TFRS_ACT_SIGMOID also stores the logits into prod
+enum { SG_DX = 1, SG_DW = 2, SG_PLAIN = 3, SG_CROSS = 4, SG_DENSE = 8 };
 
 struct SgParams {
   const unsigned char* aimg; const unsigned char* bimg;  // [tile128][kb_total][hi|lo][16 KB]
@@ -125,6 +127,10 @@ split_gemm_kernel(const SgParams p) {
         pv = fmaf(p.diag, xv, pv);
         if (p.prod) p.prod[rr * p.ld_out + col] = pv;
         p.out[rr * p.ld_out + col] = fmaf(x0v, pv, xv);
+      } else if (MODE >= SG_DENSE) {    // DENSE: y = act(acc + bias)   (Keras Dense: MatMul, BiasAdd, activation)
+        const float z = fmaf(acc[i], unscale, p.bias ? __ldg(p.bias + col) : 0.f);
+        if (MODE == SG_DENSE + TFRS_ACT_SIGMOID && p.prod) p.prod[rr * p.ld_out + col] = z;
+        p.out[rr * p.ld_out + col] = dense_act(MODE - SG_DENSE, z);
       } else {                          // DX: dx = acc + diag * gp + g
         float v = fmaf(acc[i], unscale, __ldg(p.e1 + rr * p.ld1 + col));
         if (p.diag != 0.f) v = fmaf(p.diag, __ldg(p.e0 + rr * p.ld0 + col), v);
@@ -210,11 +216,17 @@ static int sg_launch(int mode, const SgParams& p, cudaStream_t st) {
   TFRS_DYN_SMEM(split_gemm_kernel<SG_DW>, (int)smem);
   TFRS_DYN_SMEM(split_gemm_kernel<SG_PLAIN>, (int)smem);
   TFRS_DYN_SMEM(split_gemm_kernel<SG_CROSS>, (int)smem);
+  TFRS_DYN_SMEM(split_gemm_kernel<SG_DENSE + TFRS_ACT_LINEAR>, (int)smem);
+  TFRS_DYN_SMEM(split_gemm_kernel<SG_DENSE + TFRS_ACT_RELU>, (int)smem);
+  TFRS_DYN_SMEM(split_gemm_kernel<SG_DENSE + TFRS_ACT_SIGMOID>, (int)smem);
   const long long items = (long long)p.n_mb * p.n_nt * p.n_kc;
   int grid = sm_count(); if (grid > items) grid = (int)items;
   if (mode == SG_DX) split_gemm_kernel<SG_DX><<<grid, SG_THREADS2, smem, st>>>(p);
   else if (mode == SG_DW) split_gemm_kernel<SG_DW><<<grid, SG_THREADS2, smem, st>>>(p);
   else if (mode == SG_PLAIN) split_gemm_kernel<SG_PLAIN><<<grid, SG_THREADS2, smem, st>>>(p);
+  else if (mode == SG_DENSE + TFRS_ACT_LINEAR) split_gemm_kernel<SG_DENSE + TFRS_ACT_LINEAR><<<grid, SG_THREADS2, smem, st>>>(p);
+  else if (mode == SG_DENSE + TFRS_ACT_RELU) split_gemm_kernel<SG_DENSE + TFRS_ACT_RELU><<<grid, SG_THREADS2, smem, st>>>(p);
+  else if (mode == SG_DENSE + TFRS_ACT_SIGMOID) split_gemm_kernel<SG_DENSE + TFRS_ACT_SIGMOID><<<grid, SG_THREADS2, smem, st>>>(p);
   else split_gemm_kernel<SG_CROSS><<<grid, SG_THREADS2, smem, st>>>(p);
   TFRS_LAUNCH_CHECK();
   return TFRS_OK;
@@ -250,6 +262,20 @@ sg_reduce_chunks_strided_kernel(const float* __restrict__ partial, long long M, 
   out[(e / N) * ld + (e % N)] = a;
 }
 
+// The same fixed-order sum, then the Dense epilogue: y = act(sum + bias[n]); logits (nullable) = sum + bias[n]
+__global__ void __launch_bounds__(256)
+sg_reduce_chunks_dense_kernel(const float* __restrict__ partial, long long M, long long N, int chunks, const float* __restrict__ bias,
+                              int act, float* __restrict__ out, float* __restrict__ logits, long long ld) {
+  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (e >= M * N) return;
+  float a = partial[e];
+  for (int z = 1; z < chunks; ++z) a += partial[(long long)z * M * N + e];
+  const long long n = e % N, o = (e / N) * ld + n;
+  const float zv = bias ? a + bias[n] : a;
+  if (logits) logits[o] = zv;
+  out[o] = dense_act(act, zv);
+}
+
 static int gt_image(const GemmOperand& op, long long rows, long long K, int kb, long long n_tiles128, CxStats* st_, unsigned char* img,
                     cudaStream_t st) {
   // max |element|: the operand's memory is [rows, K] (ld) or, transposed, [K, rows] (ld)
@@ -275,7 +301,7 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
   if (!ws || ws_bytes < pl.total) { set_error("gemm_tc: workspace too small"); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
   TFRS_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "gemm_tc: workspace must be 16-byte aligned");
   TFRS_CHECK_ARG(N < (1ll << 31) && M < (1ll << 31), "gemm_tc: M / N too large");
-  if (ep.mode != GEMM_EPI_PLAIN && pl.n_kc > 1) { set_error("gemm_tc: fused epilogues need K <= %d", DW_CHUNK_SLABS * 64); return TFRS_ERR_UNSUPPORTED; }
+  if (ep.mode != GEMM_EPI_PLAIN && ep.mode != GEMM_EPI_DENSE && pl.n_kc > 1) { set_error("gemm_tc: fused epilogues need K <= %d", DW_CHUNK_SLABS * 64); return TFRS_ERR_UNSUPPORTED; }
   unsigned char* w8 = (unsigned char*)ws;
   CxStats* ast = (CxStats*)(w8 + pl.o_st); CxStats* bst = (CxStats*)(w8 + pl.o_st + 1024);
   TFRS_CUDA(cudaMemsetAsync(w8 + pl.o_st, 0, 2048, st));
@@ -291,11 +317,16 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
     p.kb_chunk = DW_CHUNK_SLABS; p.n_kc = pl.n_kc; p.out = (float*)(w8 + pl.o_partial); p.ld_out = N;
     rc = sg_launch(SG_DW, p, st);
     if (rc) return rc;
-    sg_reduce_chunks_strided_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, out, ld_out);
+    if (ep.mode == GEMM_EPI_DENSE)   // bias + activation applied to the reduced sum
+      sg_reduce_chunks_dense_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.bias, ep.act, out, ep.prod,
+                                                                                     ld_out);
+    else
+      sg_reduce_chunks_strided_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, out, ld_out);
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }
   p.kb_chunk = pl.kb; p.n_kc = 1; p.out = out; p.ld_out = ld_out;
+  if (ep.mode == GEMM_EPI_DENSE) return sg_launch(SG_DENSE + ep.act, p, st);
   return sg_launch(ep.mode == GEMM_EPI_PLAIN ? SG_PLAIN : (ep.mode == GEMM_EPI_CROSS ? SG_CROSS : SG_DX), p, st);
 }
 

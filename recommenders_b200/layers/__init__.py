@@ -1,4 +1,5 @@
 """Layers namespace, shaped like tensorflow_recommenders/layers/__init__.py:18-23."""
+from . import blocks
 from . import embedding
 from . import factorized_top_k
 from . import feature_interaction

@@ -214,6 +214,133 @@ class FactorizedTopK(Factorized):
     ops.hits_accumulate(first, finite, w, self._ks, acc)
 
 
+# ------------------------------------------------------------------------------------------------
+# ranking metrics (the tf.keras metrics of tasks/ranking.py's tutorials and experimental/models/ranking.py)
+# ------------------------------------------------------------------------------------------------
+class _RankingMetric:
+  """A metric whose state is a slice of the ranking statistics (`ops.ranking_metrics`, layout in include/tfrs_b200.h):
+  a float64 device accumulator that update_state adds to without synchronising; result() reads it once.
+  `tasks.Ranking` feeds every such metric of a call from the loss kernel's single launch (`_add`)."""
+
+  threshold: Optional[float] = None        # the BinaryAccuracy threshold the statistics must use (None: any)
+  num_thresholds: Optional[int] = None     # the AUC bucket count the statistics must use (None: any)
+
+  def __init__(self, name: str):
+    self.name = name
+    self._acc = None
+    self._host = None
+
+  def _slots(self, num_thresholds: int) -> slice:
+    raise NotImplementedError()
+
+  def reset_states(self) -> None:
+    if self._acc is not None:
+      self._acc.zero_()
+    self._host = None
+
+  reset_state = reset_states
+
+  def _add(self, stats: torch.Tensor) -> None:
+    part = stats[self._slots((stats.numel() - ops.RANKING_STATS) // 2)]
+    if self._acc is None or self._acc.device != stats.device or self._acc.shape != part.shape:
+      self._acc = torch.zeros_like(part)
+    self._acc.add_(part)
+    self._host = None
+
+  def update_state(self, y_true, y_pred, sample_weight=None) -> None:
+    with torch.no_grad():
+      self._add(ops.ranking_metrics(y_pred.detach(), torch.as_tensor(y_true, device=y_pred.device), sample_weight,
+                                    0.5 if self.threshold is None else self.threshold,
+                                    2 if self.num_thresholds is None else self.num_thresholds))
+
+  def _values(self) -> np.ndarray:
+    if self._acc is None:
+      return None
+    if self._host is None:
+      self._host = self._acc.cpu().numpy()   # the one synchronisation
+    return self._host
+
+
+def _div_no_nan(a: float, b: float) -> float:
+  return a / b if b else 0.0
+
+
+class BinaryAccuracy(_RankingMetric):
+  """tf.keras.metrics.BinaryAccuracy: weighted mean of [(y_pred > threshold) == y_true]."""
+
+  def __init__(self, name: str = "binary_accuracy", dtype=None, threshold: float = 0.5):
+    super().__init__(name)
+    self.threshold = float(threshold)
+
+  def _slots(self, T):
+    return slice(0, 2)
+
+  def result(self) -> float:
+    v = self._values()
+    return 0.0 if v is None else _div_no_nan(v[1], v[0])
+
+
+class MeanSquaredError(_RankingMetric):
+  """tf.keras.metrics.MeanSquaredError: weighted mean of (y_pred - y_true)^2."""
+
+  def __init__(self, name: str = "mean_squared_error", dtype=None):
+    super().__init__(name)
+
+  def _slots(self, T):
+    return slice(0, 5)
+
+  def result(self) -> float:
+    v = self._values()
+    return 0.0 if v is None else _div_no_nan(v[4], v[0])
+
+
+class RootMeanSquaredError(MeanSquaredError):
+  """tf.keras.metrics.RootMeanSquaredError: sqrt of the weighted mean squared error."""
+
+  def __init__(self, name: str = "root_mean_squared_error", dtype=None):
+    super().__init__(name)
+
+  def result(self) -> float:
+    return float(np.sqrt(super().result()))
+
+
+class AUC(_RankingMetric):
+  """tf.keras.metrics.AUC with curve="ROC", summation_method="interpolation" and evenly spaced thresholds: every prediction
+  adds its weighted label / (1 - label) to bucket max(ceil(p (T - 1)) - 1, 0); TP / FP at threshold i are the sums over
+  buckets >= i; result = sum_i (fpr_i - fpr_i+1) (tpr_i + tpr_i+1) / 2 (divide-no-nan rates)."""
+
+  def __init__(self, num_thresholds: int = 200, curve: str = "ROC", summation_method: str = "interpolation", name: Optional[str] = None,
+               dtype=None, thresholds=None, multi_label: bool = False, num_labels=None, label_weights=None, from_logits: bool = False):
+    if curve != "ROC" or summation_method != "interpolation" or multi_label or thresholds is not None or label_weights is not None \
+        or from_logits:
+      raise NotImplementedError("AUC: only curve='ROC', summation_method='interpolation', evenly spaced thresholds, "
+                                "multi_label=False are implemented")
+    if num_thresholds <= 1:
+      raise ValueError("Argument `num_thresholds` must be an integer > 1. "
+                       f"Received: num_thresholds={num_thresholds}")
+    super().__init__(name if name is not None else "auc")
+    self.num_thresholds = int(num_thresholds)
+
+  def _slots(self, T):
+    return slice(ops.RANKING_STATS, ops.RANKING_STATS + 2 * T)
+
+  def bucket_counts(self):
+    """(weighted positives, weighted negatives) per bucket, float64 NumPy arrays of length num_thresholds."""
+    v = self._values()
+    T = self.num_thresholds
+    if v is None:
+      return np.zeros(T), np.zeros(T)
+    return v[:T], v[T:]
+
+  def result(self) -> float:
+    pos, neg = self.bucket_counts()
+    tp = np.cumsum(pos[::-1])[::-1]; fp = np.cumsum(neg[::-1])[::-1]
+    P, N = tp[0], fp[0]
+    tpr = tp / P if P else np.zeros_like(tp)
+    fpr = fp / N if N else np.zeros_like(fp)
+    return float(np.sum((fpr[:-1] - fpr[1:]) * (tpr[:-1] + tpr[1:]) / 2.0))
+
+
 def _flat_device(w, device) -> torch.Tensor:
   t = w if isinstance(w, torch.Tensor) else torch.as_tensor(np.asarray(w))
   return t.to(device=device, dtype=torch.float32).reshape(-1)

@@ -820,5 +820,180 @@ def dot_interaction(feats: torch.Tensor, self_interaction: bool = False, skip_ga
   return _DotInteraction.apply(feats, bool(self_interaction), bool(skip_gather))
 
 
+# ------------------------------------------------------------------------------------------------
+# K6 Dense layer
+# ------------------------------------------------------------------------------------------------
+ACT_LINEAR, ACT_RELU, ACT_SIGMOID = 0, 1, 2
+DENSE_ACTIVATIONS = {None: ACT_LINEAR, "linear": ACT_LINEAR, "relu": ACT_RELU, "sigmoid": ACT_SIGMOID}
+
+
+class _Dense(torch.autograd.Function):
+  """act(x @ W + bias) with W [in, out]; returns (y, logits) where logits = x @ W + bias for a sigmoid layer (an empty,
+  non-differentiable tensor otherwise).  The backward works from the saved OUTPUT y and adds the logits' gradient."""
+
+  @staticmethod
+  def forward(ctx, x, W, bias, act):
+    x = f32c(x, "x"); W = f32c(W, "kernel")
+    b = None if bias is None else f32c(bias, "bias")
+    B, K = x.shape
+    if W.dim() != 2 or W.shape[0] != K:
+      raise ValueError(f"dense: kernel must be [{K}, units], got {tuple(W.shape)}")
+    N = W.shape[1]
+    if b is not None and b.numel() != N:
+      raise ValueError(f"dense: bias must have {N} entries, got {b.numel()}")
+    y = torch.empty((B, N), dtype=torch.float32, device=x.device)
+    logits = torch.empty((B, N) if act == ACT_SIGMOID else (0,), dtype=torch.float32, device=x.device)
+    if B:
+      ws = workspace(max(lib().tfrs_dense_fwd_workspace_bytes(B, K, N), 256), x.device, "dense")
+      check(lib().tfrs_dense_fwd_f32(ptr(x), ptr(W), ptr(b), B, K, N, act, ptr(y), ptr(logits) if act == ACT_SIGMOID else None,
+                                     ptr(ws), ws.numel(), stream()), "dense_fwd")
+    ctx.save_for_backward(x, W, y)
+    ctx.act = act
+    ctx.has_bias = b is not None
+    ctx.set_materialize_grads(False)
+    if act != ACT_SIGMOID:
+      ctx.mark_non_differentiable(logits)
+    return y, logits
+
+  @staticmethod
+  def backward(ctx, gy, gz):
+    x, W, y = ctx.saved_tensors
+    B, K = x.shape; N = W.shape[1]
+    n0, n1, n2 = ctx.needs_input_grad[:3]
+    dx = torch.empty_like(x) if n0 else None
+    dW = torch.empty_like(W) if n1 else None
+    db = torch.empty((N,), dtype=torch.float32, device=x.device) if (n2 and ctx.has_bias) else None
+    if gz is not None and gz.numel() == 0:
+      gz = None
+    if gy is None and gz is None:
+      return None, None, None, None
+    if B == 0:
+      for t in (dx, dW, db):
+        if t is not None:
+          t.zero_()
+      return dx, dW, db, None
+    gy = None if gy is None else f32c(gy, "grad")
+    gz = None if gz is None else f32c(gz, "grad_logits")
+    ws = workspace(lib().tfrs_dense_bwd_workspace_bytes(B, K, N), x.device, "dense_bwd")
+    check(lib().tfrs_dense_bwd_f32(ptr(x), ptr(W), ptr(y), ptr(gy), ptr(gz), B, K, N, ctx.act, ptr(dx), ptr(dW), ptr(db), ptr(ws),
+                                   ws.numel(), stream()), "dense_bwd")
+    return dx, dW, db, None
+
+
+def dense_uses_tc(B: int, K: int, N: int) -> bool:
+  return bool(lib().tfrs_dense_uses_tc(B, K, N))
+
+
+def dense(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor] = None, activation: Optional[str] = None) -> torch.Tensor:
+  """act(x @ W + bias), W [in, out] (tf.keras.layers.Dense); activation None / "linear" / "relu" / "sigmoid" run fused.
+
+  A sigmoid output carries its logits (`_tfrs_logits`, honoured only for that very tensor, unmodified: `_version` +
+  `data_ptr` check): the binary cross-entropy of this package then uses the logits form, as tf-keras does with
+  `_keras_logits`, and its gradient reaches the logits without passing through the sigmoid."""
+  if activation not in DENSE_ACTIVATIONS:
+    raise ValueError(f"dense: activation {activation!r} is not fused (use None and apply it afterwards)")
+  act = DENSE_ACTIVATIONS[activation]
+  lead = x.shape[:-1]
+  x2 = x if x.dim() == 2 else x.reshape(-1, x.shape[-1])
+  y, z = _Dense.apply(x2, W, bias, act)
+  if x.dim() != 2:
+    y = y.reshape(*lead, y.shape[-1])
+    z = z.reshape(*lead, z.shape[-1]) if act == ACT_SIGMOID else z
+  if act == ACT_SIGMOID:
+    y._tfrs_logits = (z, y._version, y.data_ptr())
+  return y
+
+
+def attached_logits(pred: torch.Tensor) -> Optional[torch.Tensor]:
+  """The logits a fused sigmoid Dense attached to `pred`, if `pred` is that very tensor, unmodified."""
+  hint = getattr(pred, "_tfrs_logits", None)
+  if hint is not None and hint[1] == pred._version and hint[2] == pred.data_ptr() and hint[0].shape == pred.shape:
+    return hint[0]
+  return None
+
+
+# ------------------------------------------------------------------------------------------------
+# ranking loss + metrics
+# ------------------------------------------------------------------------------------------------
+LOSS_BCE, LOSS_BCE_LOGITS, LOSS_MSE = 0, 1, 2
+REDUCTION_NONE, REDUCTION_SUM, REDUCTION_SUM_OVER_BATCH_SIZE = 0, 1, 2
+RANKING_STATS = 5   # [sum w, sum w correct, sum w pred, sum w label, sum w (pred - label)^2], then the AUC buckets
+
+
+def _flat_weights(sample_weight, B: int, device) -> Optional[torch.Tensor]:
+  if sample_weight is None:
+    return None
+  w = sample_weight if isinstance(sample_weight, torch.Tensor) else torch.as_tensor(sample_weight, dtype=torch.float32)
+  w = w.to(device=device, dtype=torch.float32).reshape(-1)
+  if w.numel() == 1 and B != 1:
+    w = w.expand(B)
+  if w.numel() != B:
+    raise ValueError(f"sample_weight must have one entry per example (got {w.numel()}, expected {B})")
+  return w.contiguous()
+
+
+class _RankingLoss(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, loss_in, labels, weights, kind, reduction, pred, stats, threshold, num_thresholds):
+    x = f32c(loss_in, "predictions").reshape(-1)
+    B = x.numel()
+    y = f32c(labels, "labels").reshape(-1)
+    if y.numel() != B:
+      raise ValueError(f"labels and predictions must have the same number of entries ({y.numel()} vs {B})")
+    w = _flat_weights(weights, B, x.device)
+    per = torch.empty((B,), dtype=torch.float32, device=x.device) if reduction == REDUCTION_NONE else None
+    loss = torch.empty((1,), dtype=torch.float32, device=x.device) if reduction != REDUCTION_NONE else None
+    p = None if pred is None else f32c(pred, "predictions").reshape(-1)
+    T = int(num_thresholds) if stats is not None else 0
+    ws = workspace(lib().tfrs_ranking_workspace_bytes(B, T), x.device, "ranking")
+    check(lib().tfrs_ranking_loss_fwd_f32(ptr(x), ptr(p), ptr(y), ptr(w), B, kind, reduction, ptr(per), ptr(loss), ptr(stats),
+                                          c_f(threshold), T, ptr(ws), ws.numel(), stream()), "ranking_loss_fwd")
+    ctx.save_for_backward(x, y, w if w is not None else torch.empty(0, device=x.device))
+    ctx.has_w = w is not None
+    ctx.kind, ctx.reduction, ctx.shape = kind, reduction, loss_in.shape
+    return per if reduction == REDUCTION_NONE else loss.view(())
+
+  @staticmethod
+  def backward(ctx, g):
+    x, y, w = ctx.saved_tensors
+    B = x.numel()
+    g = f32c(g, "grad").reshape(-1)
+    dx = torch.empty_like(x)
+    check(lib().tfrs_ranking_loss_bwd_f32(ptr(x), ptr(y), ptr(w) if ctx.has_w else None, B, ctx.kind, ctx.reduction, ptr(g), ptr(dx),
+                                          stream()), "ranking_loss_bwd")
+    return dx.view(ctx.shape), None, None, None, None, None, None, None, None
+
+
+def ranking_loss(loss_in: torch.Tensor, labels: torch.Tensor, sample_weight=None, kind: int = LOSS_BCE,
+                 reduction: int = REDUCTION_SUM_OVER_BATCH_SIZE, pred: Optional[torch.Tensor] = None,
+                 stats: Optional[torch.Tensor] = None, threshold: float = 0.5, num_thresholds: int = 200) -> torch.Tensor:
+  """Keras BinaryCrossentropy / MeanSquaredError on [B] or [B, 1] predictions (one example per row): the reduced loss
+  (0-dim) or, for REDUCTION_NONE, the weighted per-example losses [B].  `stats` (float64 [RANKING_STATS + 2 T], nullable)
+  receives the metric statistics of `pred` from the same launch."""
+  return _RankingLoss.apply(loss_in, labels, sample_weight, int(kind), int(reduction), pred, stats, float(threshold),
+                            int(num_thresholds))
+
+
+def ranking_stats_buffer(num_thresholds: int, device) -> torch.Tensor:
+  return torch.empty((RANKING_STATS + 2 * int(num_thresholds),), dtype=torch.float64, device=device)
+
+
+def ranking_metrics(pred: torch.Tensor, labels: torch.Tensor, sample_weight=None, threshold: float = 0.5,
+                    num_thresholds: int = 200) -> torch.Tensor:
+  """The metric statistics of one batch (layout: include/tfrs_b200.h, ranking loss + metrics) as a float64 device tensor."""
+  p = f32c(pred, "predictions").reshape(-1)
+  B = p.numel()
+  y = f32c(labels, "labels").reshape(-1)
+  if y.numel() != B:
+    raise ValueError(f"labels and predictions must have the same number of entries ({y.numel()} vs {B})")
+  w = _flat_weights(sample_weight, B, p.device)
+  stats = ranking_stats_buffer(num_thresholds, p.device)
+  ws = workspace(lib().tfrs_ranking_workspace_bytes(B, num_thresholds), p.device, "ranking")
+  check(lib().tfrs_ranking_metrics_f32(ptr(p), ptr(y), ptr(w), B, ptr(stats), c_f(threshold), int(num_thresholds), ptr(ws), ws.numel(),
+                                       stream()), "ranking_metrics")
+  return stats
+
+
 def launch_count() -> int:
   return int(lib().tfrs_launch_count())

@@ -1,10 +1,11 @@
-"""Tasks: mirror of tensorflow_recommenders/tasks/{base,retrieval}.py."""
+"""Tasks: mirror of tensorflow_recommenders/tasks/{base,retrieval,ranking}.py."""
 from __future__ import annotations
 
 from typing import Callable, List, Optional, Sequence, Text, Union
 
 import torch
 
+from . import losses as tfrs_losses
 from . import metrics as tfrs_metrics
 from . import ops
 from .layers import loss as loss_layers
@@ -150,6 +151,87 @@ class Retrieval(torch.nn.Module, Task):
       if compute_batch_metrics:
         for metric in self._batch_metrics:
           metric.update_state(labels, scores.detach(), sample_weight=sample_weight)
+    return loss
+
+  def forward(self, *args, **kwargs):
+    return self.call(*args, **kwargs)
+
+
+class Ranking(torch.nn.Module, Task):
+  """A ranking task (tasks/ranking.py:26-119): loss of the predictions + ranking / prediction / label / loss metrics.
+
+  A loss object of this package (`losses.BinaryCrossentropy` -- the default -- or `losses.MeanSquaredError`) runs in the
+  fused ranking-loss kernel, and that same launch produces the batch statistics of every package metric of the call
+  (BinaryAccuracy, AUC, (Root)MeanSquaredError, and `Mean` as a prediction / label metric); the metrics add them into their
+  device-resident sums.  Any other callable loss, or any other object with `update_state`, is called as is."""
+
+  def __init__(self, loss: Optional[Callable] = None, metrics: Optional[List] = None, prediction_metrics: Optional[List] = None,
+               label_metrics: Optional[List] = None, loss_metrics: Optional[List] = None, name: Optional[Text] = None) -> None:
+    super().__init__()
+    self.name = name
+    self._loss = loss if loss is not None else tfrs_losses.BinaryCrossentropy()
+    self._ranking_metrics = metrics or []
+    self._prediction_metrics = prediction_metrics or []
+    self._label_metrics = label_metrics or []
+    self._loss_metrics = loss_metrics or []
+
+  @property
+  def metrics(self):
+    """Keras `layer.metrics` order: ranking, prediction, label, loss metrics."""
+    return list(self._ranking_metrics) + list(self._prediction_metrics) + list(self._label_metrics) + list(self._loss_metrics)
+
+  def _stats_plan(self):
+    """(threshold, num_thresholds, metrics served by one statistics launch): the first BinaryAccuracy threshold and AUC bucket
+    count fix the launch; package metrics that need other values update themselves."""
+    thr = T = None
+    fused = []
+    for m in self._ranking_metrics:
+      if not isinstance(m, tfrs_metrics._RankingMetric):
+        continue
+      if m.threshold is not None and thr is not None and m.threshold != thr:
+        continue
+      if m.num_thresholds is not None and T is not None and m.num_thresholds != T:
+        continue
+      thr = m.threshold if m.threshold is not None else thr
+      T = m.num_thresholds if m.num_thresholds is not None else T
+      fused.append(m)
+    means = [m for m in self._prediction_metrics + self._label_metrics if type(m) is tfrs_metrics.Mean]
+    if not fused and not means:
+      return None
+    return (0.5 if thr is None else thr), (2 if T is None else T), fused
+
+  def call(self, labels: torch.Tensor, predictions: torch.Tensor, sample_weight: Optional[torch.Tensor] = None,
+           training: bool = False, compute_metrics: bool = True) -> torch.Tensor:
+    own_loss = isinstance(self._loss, tfrs_losses.Loss)
+    if not isinstance(labels, torch.Tensor):
+      labels = torch.as_tensor(labels, dtype=torch.float32, device=predictions.device)
+    plan = self._stats_plan() if compute_metrics else None
+    stats = None
+    if own_loss:
+      stats = None if plan is None else ops.ranking_stats_buffer(plan[1], predictions.device)
+      loss = self._loss._compute(labels, predictions, sample_weight, stats, *(plan[:2] if plan else ()))
+    else:
+      loss = self._loss(labels, predictions, sample_weight=sample_weight)
+    if not compute_metrics:
+      return loss
+    with torch.no_grad():
+      if plan is not None and stats is None:
+        stats = ops.ranking_metrics(predictions.detach(), labels, sample_weight, plan[0], plan[1])
+      fused = set(map(id, plan[2])) if plan else set()
+      for metric in self._ranking_metrics:
+        if id(metric) in fused:
+          metric._add(stats)
+        else:
+          metric.update_state(y_true=labels, y_pred=predictions.detach(), sample_weight=sample_weight)
+      for metrics, slot, values in ((self._prediction_metrics, 2, predictions), (self._label_metrics, 3, labels)):
+        for metric in metrics:
+          if type(metric) is tfrs_metrics.Mean:   # weighted sum and weight sum straight from the statistics
+            metric._total = metric._total + stats[slot]
+            metric._count = metric._count + stats[0]
+          else:
+            metric.update_state(values.detach(), sample_weight=sample_weight)
+      for metric in self._loss_metrics:
+        metric.update_state(loss.detach())  # a scalar that is already the weighted loss
     return loss
 
   def forward(self, *args, **kwargs):

@@ -1,6 +1,6 @@
 """Secondary measurements for BASELINE.md §4 (configs 3 and 5): embedding gather GB/s, sparse Adagrad,
 in-batch softmax step, Cross layer.  CUDA events, warm-up, inputs larger than L2 or rotated between
-iterations.  Prints one JSON object.   usage: python tools/bench_kernels.py [--quick]"""
+iterations.  Prints one JSON object.   usage: python tools/bench_kernels.py [--quick] [--top-stack-only]"""
 import json
 import os
 import sys
@@ -36,6 +36,43 @@ def timeit(fn, iters=20, warm=5):
 
 out = {"hbm_peak_gbs": HBM}
 g = torch.Generator(device=dev); g.manual_seed(7)
+
+# ---- config 5 top stack (K6): MLP 845 -> 512 (relu) -> 256 (relu) -> 1 (sigmoid) at B = 65536, forward and forward + backward
+#      (dx of the stack input, dW, db of every layer).  `--top-stack-only` prints this leg alone.
+Bm, dims = (65536, [845, 512, 256, 1]) if not quick else (8192, [845, 512, 256, 1])
+xm = torch.rand((Bm, dims[0]), generator=g, device=dev)
+Wm = [(torch.randn((dims[i], dims[i + 1]), generator=g, device=dev) / dims[i] ** 0.5).requires_grad_(True) for i in range(3)]
+bm = [torch.zeros((dims[i + 1],), device=dev, requires_grad=True) for i in range(3)]
+gm = torch.randn((Bm, 1), generator=g, device=dev)
+acts = ["relu", "relu", "sigmoid"]
+
+
+def top_stack(x):
+  for W, b, a in zip(Wm, bm, acts):
+    x = ops.dense(x, W, b, a)
+  return x
+
+
+def top_stack_fb():
+  x = xm.detach().requires_grad_(True)
+  top_stack(x).backward(gm)
+
+
+with torch.no_grad():
+  t_f = timeit(lambda: top_stack(xm), iters=10 if not quick else 3, warm=3)
+t_fb = timeit(top_stack_fb, iters=10 if not quick else 3, warm=3)
+fl_f = sum(2.0 * Bm * dims[i] * dims[i + 1] for i in range(3))
+PEAK_FP16 = peaks.get("bf16_tflops", 989.0)   # H100 SXM data sheet dense FP16 when not measured
+out["cfg5_top_stack"] = {"fwd_seconds": t_f, "fwd_bwd_seconds": t_fb, "fwd_flops": fl_f, "fwd_bwd_flops": 3 * fl_f,
+                         "fwd_TFLOPs": fl_f / t_f / 1e12, "fwd_bwd_TFLOPs": 3 * fl_f / t_fb / 1e12,
+                         "fwd_bwd_frac_of_fp16_peak": 3 * fl_f / t_fb / 1e12 / PEAK_FP16, "peak_tflops": PEAK_FP16,
+                         "shape": f"B={Bm}, {'->'.join(map(str, dims))}",
+                         "path": "wgmma split-fp16 GEMMs (each product executed 3x) for the 512 / 256 layers, exact warp-per-row "
+                                 "kernel for the 1-unit layer; algorithmic flops"}
+del xm, Wm, bm, gm
+if "--top-stack-only" in sys.argv:
+  print(json.dumps(out))
+  sys.exit(0)
 
 # ---- config 5 gather: 26 tables 1M x 32, 65536 ids each -> [65536, 26*32 (+13 dense, ld 848)]
 F, V, D, B = (26, 1_000_000, 32, 65536) if not quick else (26, 100_000, 32, 8192)
