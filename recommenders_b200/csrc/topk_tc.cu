@@ -27,14 +27,17 @@
 // of the exact top-K has screening score >= tau - 2*eps_q >= L_q - 2*eps_q, so it is in the list and in
 // the re-scored band.
 //
-// Scan kernel shape (per CTA, 1 CTA / SM, 544 threads): 256 queries (two 128-row A blocks, resident in smem)
-// x a contiguous range of 128-row corpus tiles streamed through a 4-6 stage bulk-TMA ring; warp 16 = TMA
-// producer (one thread), warpgroups 0-3 = one 64-query slice each: wgmma m64n128k16 (fp16 -> fp32 in registers),
-// then the epilogue on the register fragment.  The four consumer warpgroups run independently, so one's MMAs
-// overlap another's epilogue; each B tile in smem feeds all four (256 query rows per 16 KB of L2->smem traffic).
+// Scan kernel shape (per CTA, 1 CTA / SM, 512 threads = 16 warps, so 128 registers per thread): 256 queries (two
+// 128-row A blocks) x a contiguous range of 128-row corpus tiles streamed through a 4-6 stage bulk-TMA ring, which
+// thread 0 drives between its own MMAs.  Warpgroups 0-3 own one 64-query slice each and run every tile as two
+// 64-column halves (wgmma m64n64k16, fp16 -> fp32 in two 32-register accumulator sets): the MMAs of the next half are
+// in flight while the epilogue of the current one runs, so no warpgroup waits for its own MMAs before its epilogue.
+// For d <= 64 a warpgroup's A slice lives in registers (RS wgmma, half the smem reads of SS); for d <= 128 it stays in
+// smem.  Each B tile in smem feeds all four (256 query rows per 16 KB of L2->smem traffic).
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
+#include <type_traits>
 #include "rowselect.cuh"
 #include "tc_ptx.cuh"
 
@@ -47,7 +50,7 @@ constexpr int QBLK = 256;            // queries per CTA (2 A blocks)
 constexpr int KSLAB = 64;            // fp16 elements per 128-byte swizzle row
 constexpr int SLAB_BYTES = TILE_N * 128;  // 16 KB: 128 rows x 128 B
 constexpr int HEADER_BYTES = 1024;
-constexpr int THREADS = 544;         // 4 consumer warpgroups + 1 producer warp
+constexpr int THREADS = 512;         // 4 consumer warpgroups (16 warps: 128 registers per thread)
 constexpr int CONSUMER_WARPS = 16;
 constexpr int CAND_CAP = 2048;       // octet records kept per query across all segments (sizing of cap_part)
 constexpr int MAX_SAMPLE_STRIDE = 4;
@@ -230,40 +233,37 @@ tc_scan_kernel(const ScanParams p) {
   const int u_begin = (int)((long long)part * p.n_seq / p.parts);
   const int u_end = (int)((long long)(part + 1) * p.n_seq / p.parts);
   const int n_iter = u_end - u_begin;
+  const bool issuer = threadIdx.x == 0;   // also drives the bulk-TMA ring
 
-  if (threadIdx.x == 0) {
+  if (issuer) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
     mbar_init(a_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  if (wg == 4) {
-    // ===== bulk-TMA producer =====
-    if (threadIdx.x == 512) {
-      mbar_expect_tx(a_full, 2 * KB * SLAB_BYTES);
-      bulk_g2s(sA, p.qimg + (long long)qb * 2 * KB * SLAB_BYTES, 2 * KB * SLAB_BYTES, a_full);
-      int stage = 0; uint32_t phase = 0;
-      const uint64_t pol = l2_policy_evict_first();
-      for (int it = 0; it < n_iter; ++it) {
-        const long long tile = (long long)(u_begin + it) * p.stride;
-        mbar_wait(&empty[stage], phase ^ 1);
-        mbar_expect_tx(&full[stage], KB * SLAB_BYTES);
-        if (MODE == MODE_FILTER)   // streamed once per pass: evict-first, so the survivor records stay in L2 for the select kernel
-          bulk_g2s_hint(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage], pol);
-        else
-          bulk_g2s(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-    return;
+  // tile `it` of this part -> ring slot `stage` (issuer only)
+  auto load_tile = [&](int it, int stage) {
+    const long long tile = (long long)(u_begin + it) * p.stride;
+    mbar_expect_tx(&full[stage], KB * SLAB_BYTES);
+    if (MODE == MODE_FILTER)   // streamed once per pass: evict-first, so the survivor records stay in L2 for the select kernel
+      bulk_g2s_hint(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage],
+                    l2_policy_evict_first());
+    else
+      bulk_g2s(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage]);
+  };
+  if (issuer) {
+    mbar_expect_tx(a_full, 2 * KB * SLAB_BYTES);
+    bulk_g2s(sA, p.qimg + (long long)qb * 2 * KB * SLAB_BYTES, 2 * KB * SLAB_BYTES, a_full);
+    for (int it = 0; it < STAGES && it < n_iter; ++it) load_tile(it, it);
   }
 
-  // ===== consumers: warpgroup c computes the 64 query rows [64 c, 64 c + 64) of the CTA's 256 against each tile and runs
-  // the epilogue on its register fragment: a thread holds rows r and r + 8 x 32 columns (pairs 8j + 2(lane%4) + {0,1});
-  // the 4 lanes of a quad together hold 8 consecutive columns of a row -- one octet record.
-  const int c = wg;
-  const long long row_a = (long long)qb * QBLK + c * 64 + warp * 16 + (lane >> 2);   // rows row_a, row_a + 8
+  // Warpgroup wg computes the 64 query rows [64 wg, 64 wg + 64) of the CTA's 256 against each tile, as two 64-column
+  // halves (m64n64k16, one 32-register accumulator set each).  The MMAs of the next half are issued before the epilogue
+  // of the current one, so every warpgroup keeps the tensor pipe busy while it runs its own epilogue.  A thread holds rows
+  // r and r + 8 x 16 columns of a half (pairs 8j + 2(lane%4) + {0,1}, j < 8); the 4 lanes of a quad together hold 8
+  // consecutive columns of a row -- one octet record.
+  const long long row_a = (long long)qb * QBLK + wg * 64 + warp * 16 + (lane >> 2);   // rows row_a, row_a + 8
   const bool quad_leader = (lane & 3) == 0;
   float thr[2] = {INFINITY, INFINITY};
   if (MODE == MODE_FILTER) {
@@ -276,37 +276,43 @@ tc_scan_kernel(const ScanParams p) {
   int in_group = 0, bin_out = 0;
 
   mbar_wait(a_full, 0);
-  // this warpgroup's 64-row slice of A block c/2 (image layout [block][K slab][16 KB]): 8 swizzle groups of 1024 B
-  const uint32_t a0 = smem_u32(sA + (c >> 1) * KB * SLAB_BYTES + (c & 1) * 8192);
-  int stage = 0; uint32_t phase = 0;
-  for (int it = 0; it < n_iter; ++it) {
-    const int u = u_begin + it;
-    const long long tile = (long long)u * p.stride;
-    const long long col0 = tile * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
-    mbar_wait(&full[stage], phase);
-    float acc[64];
+  // this warpgroup's 64-row slice of A block wg/2 (image layout [block][K slab][16 KB]): 8 swizzle groups of 1024 B
+  const uint32_t a0 = smem_u32(sA + (wg >> 1) * KB * SLAB_BYTES + (wg & 1) * 8192);
+  // KB == 1: the slice stays the same for the whole scan, so it lives in registers (RS wgmma), which halves the
+  // shared-memory reads per MMA; one ldmatrix_x4 per K step of 16.  Lane t addresses row 16 warp + 8 ((t/8) & 1) + t%8,
+  // 16-byte chunk 2 k4 + t/16 of the swizzled slice.
+  uint32_t afrag[4][4];
+  if (KB == 1) {
+    const int r = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) ldmatrix_x4(afrag[k4], a0 + r * 128 + (((2 * k4 + (lane >> 4)) ^ (lane & 7)) * 16));
+  }
+  // the MMAs of one 64-column half of the tile in ring slot `stage`; one commit group
+  auto issue = [&](float (&acc)[32], int stage, int h) {
     wgmma_fence();
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) {
-      const uint64_t a_desc = make_smem_desc(a0 + kb * SLAB_BYTES);
-      const uint64_t b_desc = make_smem_desc(smem_u32(sB + (stage * KB + kb) * SLAB_BYTES));
+      const uint64_t b_desc = make_smem_desc(smem_u32(sB + (stage * KB + kb) * SLAB_BYTES + h * 8192));
 #pragma unroll
-      for (int k4 = 0; k4 < 4; ++k4)  // 4 x (K=16 fp16 = 32 B) inside the 128-byte swizzle row
-        wgmma_m64n128_ss(acc, a_desc + (uint64_t)(k4 * 2), b_desc + (uint64_t)(k4 * 2), (uint32_t)((kb | k4) != 0));
+      for (int k4 = 0; k4 < 4; ++k4) {  // 4 x (K=16 fp16 = 32 B) inside the 128-byte swizzle row
+        if (KB == 1)
+          wgmma_m64n64_rs(acc, afrag[k4], b_desc + (uint64_t)(k4 * 2), (uint32_t)(k4 != 0));
+        else
+          wgmma_m64n64_ss(acc, make_smem_desc(a0 + kb * SLAB_BYTES) + (uint64_t)(k4 * 2), b_desc + (uint64_t)(k4 * 2),
+                          (uint32_t)((kb | k4) != 0));
+      }
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    acc_fence(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have retired: the smem slot may be refilled
-    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-
+  };
+  // the epilogue of half H of tile `it` (first column col0)
+  auto epilogue = [&](const float (&acc)[32], long long col0, int it, auto half) {
+    constexpr int H = decltype(half)::value;
     if (MODE != MODE_FILTER) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
+      for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr) binm[2 * rr + (j >> 3)] = max3(binm[2 * rr + (j >> 3)], acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
-      if (++in_group == p.group || it == n_iter - 1) {   // close the bin after `group` tiles (loop-uniform)
+        for (int rr = 0; rr < 2; ++rr) binm[2 * rr + H] = max3(binm[2 * rr + H], acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+      if (H == 1 && (++in_group == p.group || it == n_iter - 1)) {   // close the bin after `group` tiles (loop-uniform)
 #pragma unroll
         for (int s = 0; s < 4; ++s) {
           const float m = quad_max(binm[s]);
@@ -318,32 +324,40 @@ tc_scan_kernel(const ScanParams p) {
         ++bin_out; in_group = 0;
       }
     } else {
-      // Each lane marks the octets (row rr, column group j) where one of its two scores passes; one warp-wide OR of those
-      // 32-bit masks leaves the few octets that any lane of the warp hit (a warp of 16 rows meets a survivor in most tiles,
-      // but in few of its 32 octet slots).  Only those take a ballot, which makes the decision quad-uniform; each lane of a
-      // surviving octet stores its two scores, the quad leader the octet's first index.
-      unsigned int mine = 0u;
+      // Common path: a max tree over each row's 16 scores, one compare per row and one warp vote.  A warp of 16 rows meets
+      // a survivor in about one half tile in two.  Only then each lane marks the octets (row rr, column group j) where one
+      // of its two scores passes, one warp-wide OR leaves the octets any lane hit, and those take a ballot, which makes the
+      // decision quad-uniform; each lane of a surviving octet stores its two scores, the quad leader the octet's first index.
+      float pm[2][8];
+      bool pass = false;
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr)
+      for (int rr = 0; rr < 2; ++rr) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
-          mine |= (fmaxf(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]) >= thr[rr]) ? (1u << (16 * rr + j)) : 0u;
-      const unsigned int hit = __reduce_or_sync(0xffffffffu, mine);
-      if (hit) {
+        for (int j = 0; j < 8; ++j) pm[rr][j] = fmaxf(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+        const float m = fmaxf(fmaxf(fmaxf(pm[rr][0], pm[rr][1]), fmaxf(pm[rr][2], pm[rr][3])),
+                              fmaxf(fmaxf(pm[rr][4], pm[rr][5]), fmaxf(pm[rr][6], pm[rr][7])));
+        pass |= m >= thr[rr];
+      }
+      if (__any_sync(0xffffffffu, pass)) {
+        unsigned int mine = 0u;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) mine |= (pm[rr][j] >= thr[rr]) ? (1u << (8 * rr + j)) : 0u;
+        const unsigned int hit = __reduce_or_sync(0xffffffffu, mine);
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
-          const long long seg_row = ((row_a + 8 * rr) * p.parts + part) * 2;
+          const long long seg_row = ((row_a + 8 * rr) * p.parts + part) * 2 + H;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (!((hit >> (16 * rr + j)) & 1u)) continue;   // warp-uniform
-            const float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
-            const unsigned int vote = __ballot_sync(0xffffffffu, (mine >> (16 * rr + j)) & 1u);
+          for (int j = 0; j < 8; ++j) {
+            if (!((hit >> (8 * rr + j)) & 1u)) continue;   // warp-uniform
+            const unsigned int vote = __ballot_sync(0xffffffffu, (mine >> (8 * rr + j)) & 1u);
             if ((vote >> (lane & ~3)) & 0xFu) {
-              const int s = 2 * rr + (j >> 3);
+              const int s = 2 * rr + H;
               if (cnt[s] < cap) {
-                const long long seg = (seg_row + (j >> 3)) * p.cap_part + cnt[s];
-                reinterpret_cast<float2*>(p.cand_s + seg * 8)[lane & 3] = make_float2(v0, v1);
-                if (quad_leader) p.cand_i[seg] = (unsigned int)(col0 + 8 * j);
+                const long long seg = seg_row * p.cap_part + cnt[s];
+                reinterpret_cast<float2*>(p.cand_s + seg * 8)[lane & 3] = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+                if (quad_leader) p.cand_i[seg] = (unsigned int)(col0 + 64 * H + 8 * j);
                 ++cnt[s];
               } else {
                 ovf |= 1u << s;
@@ -353,6 +367,52 @@ tc_scan_kernel(const ScanParams p) {
         }
       }
     }
+  };
+
+  float acc0[32], acc1[32];   // column halves 0 / 1 of the current tile
+  int stage = 0; uint32_t phase = 0;
+  int prev_stage = 0; uint32_t prev_phase = 0;   // ring slot (and its fill parity) of the previous tile
+  // One tile; half 0 of it is in acc0 and complete on entry.  Each epilogue runs while the MMAs of the next half are in
+  // flight.  Nothing is in flight across the loop's back edge and the last tile is a separate instantiation: ptxas
+  // serializes the wgmma when an accumulator is in flight at a loop head or only on some paths.
+  auto tile_step = [&](int it, auto last_tile) {
+    constexpr bool LAST = decltype(last_tile)::value;
+    const long long col0 = (long long)(u_begin + it) * p.stride * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
+    issue(acc1, stage, 1);
+    epilogue(acc0, col0, it, std::integral_constant<int, 0>{});
+    const int next_stage = stage + 1 == STAGES ? 0 : stage + 1;
+    const uint32_t next_phase = stage + 1 == STAGES ? phase ^ 1 : phase;
+    if (!LAST) {
+      mbar_wait(&full[next_stage], next_phase);
+      issue(acc0, next_stage, 0);
+      wgmma_wait<1>();          // half 1 has retired, half 0 of the next tile is in flight
+    } else {
+      wgmma_wait<0>();
+    }
+    acc_fence(acc1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[stage]);   // both halves' MMAs on this slot have retired: it may be refilled
+    // Refill one tile behind: the previous tile's slot, which the other warpgroups have had a whole tile's time to
+    // release, so the issuer rarely waits on the slowest warpgroup.
+    if (!LAST && issuer && it >= 1 && it - 1 + STAGES < n_iter) {
+      mbar_wait(&empty[prev_stage], prev_phase);
+      load_tile(it - 1 + STAGES, prev_stage);
+    }
+    prev_stage = stage; prev_phase = phase;
+    stage = next_stage; phase = next_phase;
+    epilogue(acc1, col0, it, std::integral_constant<int, 1>{});
+    if (!LAST) {
+      wgmma_wait<0>();
+      acc_fence(acc0);
+    }
+  };
+  if (n_iter > 0) {
+    mbar_wait(&full[0], 0);
+    issue(acc0, 0, 0);
+    wgmma_wait<0>();
+    acc_fence(acc0);
+    for (int it = 0; it + 1 < n_iter; ++it) tile_step(it, std::false_type{});
+    tile_step(n_iter - 1, std::true_type{});
   }
   if (MODE == MODE_SAMPLE) {
 #pragma unroll
