@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define TFRS_B200_VERSION 100 /* 0.1.0 */
+#define TFRS_B200_VERSION 101 /* 0.1.1 */
 
 enum {
   TFRS_OK = 0,
@@ -325,23 +325,17 @@ int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* W, const fl
                        int64_t B, int D, int64_t ld, float diag_scale, float* dx0, float* dx, float* dW,
                        float* dbias, void* ws, size_t ws_bytes, void* stream);
 
-/* K5 on the tensor cores (forward): the same cross formula as tfrs_cross_fwd_f32, computed as one wgmma
- * GEMM on exactly-rescaled fp16 hi/lo splits of x and W (3 MMAs per K step, fp32 accumulation in registers;
- * ~2^-21 relative error, inside the 1e-5 bar) with the formula fused in the epilogue.
- * tfrs_cross_tc_weight_build turns W [D,D] ([in,out]) into the K-major image of W^T; rebuild it whenever
- * W changes.  `ws` holds the per-call image of x. */
-size_t tfrs_cross_tc_weight_bytes(int D);
-int tfrs_cross_tc_weight_build(const float* W, int D, void* wbuf, size_t bytes, void* stream);
-size_t tfrs_cross_tc_workspace_bytes(int64_t B, int D);
-int tfrs_cross_tc_fwd_f32(const float* x0, const float* x, const void* wbuf, const float* bias, int64_t B, int D,
-                          int64_t ld, float diag_scale, float* out, float* prod, void* ws, size_t ws_bytes,
-                          void* stream);
-/* The same forward for a STACK of cross layers (the reference chains `x = cross(x0, x)`): `out_amax_bits` (nullable, one
- * uint32 on the device) receives max |out| as float bits, accumulated by the epilogue; passing it as `x_amax_bits` of the
+/* K5 on the tensor cores (forward): the same cross formula as tfrs_cross_fwd_f32, computed as one wgmma GEMM on
+ * exactly-rescaled fp16 hi/lo splits of x and W (3 MMAs per K step, fp32 accumulation in registers; ~2^-21 relative
+ * error, inside the 1e-5 bar) with the formula fused in the epilogue.  W [D,D] ([in,out]) is taken as stored; `ws`
+ * holds the per-call images of x and W.
+ * For a STACK of cross layers (the reference chains `x = cross(x0, x)`): `out_amax_bits` (nullable, one uint32 on the
+ * device) receives max |out| as float bits, accumulated by the epilogue; passing it as `x_amax_bits` (nullable) of the
  * next layer replaces that layer's pass over x for the power-of-two rescale statistic (identical bits, identical result). */
-int tfrs_cross_tc_fwd_ex_f32(const float* x0, const float* x, const void* wbuf, const float* bias, int64_t B, int D,
-                             int64_t ld, float diag_scale, float* out, float* prod, const unsigned int* x_amax_bits,
-                             unsigned int* out_amax_bits, void* ws, size_t ws_bytes, void* stream);
+size_t tfrs_cross_tc_workspace_bytes(int64_t B, int D);
+int tfrs_cross_tc_fwd_f32(const float* x0, const float* x, const float* W, const float* bias, int64_t B, int D, int64_t ld,
+                          float diag_scale, float* out, float* prod, const unsigned int* x_amax_bits, unsigned int* out_amax_bits,
+                          void* ws, size_t ws_bytes, void* stream);
 
 /* K5b with both GEMMs on the tensor cores (same contract and outputs as tfrs_cross_bwd_f32): dx = gp.W^T + diag*gp + g
  * and dW = x^T.gp as split-fp16 wgmma GEMMs (dW accumulates the batch in chunks of 1024 rows, partials summed in

@@ -81,11 +81,8 @@ _SIGNATURES = {
     "tfrs_sparse_adagrad_workspace_bytes": (c_sz, [c_l, c_i]),
     "tfrs_sparse_adagrad_f32": (c_i, [c_p, c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_f, c_i, c_p, c_sz, c_p]),
     "tfrs_cross_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p]),
-    "tfrs_cross_tc_weight_bytes": (c_sz, [c_i]),
-    "tfrs_cross_tc_weight_build": (c_i, [c_p, c_i, c_p, c_sz, c_p]),
     "tfrs_cross_tc_workspace_bytes": (c_sz, [c_l, c_i]),
-    "tfrs_cross_tc_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_cross_tc_fwd_ex_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_cross_tc_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_cross_bwd_workspace_bytes": (c_sz, [c_l, c_i]),
     "tfrs_cross_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_cross_tc_bwd_workspace_bytes": (c_sz, [c_l, c_i]),

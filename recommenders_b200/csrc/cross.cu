@@ -1,11 +1,12 @@
-// cross.cu -- K5/K5b: DCN-v2 cross layer, full-rank (layers/feature_interaction/dcn.py:176-186).
+// cross.cu -- K5/K5b: DCN-v2 cross layer, full-rank (layers/feature_interaction/dcn.py:176-186) and low-rank.
 //   fwd: out = x0 * (x . W + bias + diag_scale * x) + x     W is [in,out] (Keras Dense, dcn.py:121-130)
-//        one exact SGEMM whose epilogue applies bias / diag / x0 / residual, so the [B,D] product
-//        never makes a separate HBM round trip (the reference runs MatMul, BiasAdd, Mul, Add).
+//        one GEMM whose epilogue applies bias / diag / x0 / residual, so the [B,D] product never makes a separate HBM
+//        round trip (the reference runs MatMul, BiasAdd, Mul, Add): the exact SGEMM (sgemm.cuh) for small shapes, the
+//        split-fp16 tensor-core GEMM (split_gemm.cu) otherwise.
 //   bwd: gp = g*x0 ; dx0 = g*prod ; dx = gp . W^T + diag*gp + g ; dW = x^T . gp (deterministic split-K) ;
 //        dbias = colsum(gp) (two-level fixed-order reduction).
 #include "sgemm.cuh"
-#include "cross_tc.cuh"
+#include "split_gemm.cuh"
 
 namespace tfrs {
 
@@ -159,10 +160,28 @@ extern "C" int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* 
   return TFRS_OK;
 }
 
-// ---- K5b with the two GEMMs on the tensor cores (cross_tc_bwd.cu); same contract and outputs as tfrs_cross_bwd_f32
+// ---- K5 / K5b on the tensor cores: one split-fp16 GEMM forward, two backward; same contract and outputs as the exact path
+extern "C" size_t tfrs_cross_tc_workspace_bytes(int64_t B, int D) {
+  return tc::gemm_tc_workspace(B, D, D, tc::GEMM_EPI_CROSS);
+}
+
+extern "C" int tfrs_cross_tc_fwd_f32(const float* x0, const float* x, const float* W, const float* bias, int64_t B, int D, int64_t ld,
+                                     float diag_scale, float* out, float* prod, const unsigned int* x_amax_bits,
+                                     unsigned int* out_amax_bits, void* ws, size_t ws_bytes, void* stream) {
+  TFRS_CHECK_ARG(x0 && x && W && out, "cross_tc_fwd: NULL pointer");
+  TFRS_CHECK_ARG(B > 0 && D > 0 && ld >= D, "cross_tc_fwd: bad shape");
+  TFRS_CHECK_ARG(diag_scale >= 0.f, "`diag_scale` should be non-negative. Got `diag_scale` = %g", diag_scale);
+  // image row of the B operand = output column n, reduction index k: W[k*D + n]
+  return tc::gemm_tc(tc::GemmOperand{x, ld, false, x_amax_bits}, tc::GemmOperand{W, D, true}, B, D, D,
+                     tc::GemmEpilogue{tc::GEMM_EPI_CROSS, x0, ld, x, ld, bias, diag_scale, prod, 0, out_amax_bits}, out, ld, ws,
+                     ws_bytes, (cudaStream_t)stream);
+}
+
+// gp | colsum partials | max |gp| | one GEMM workspace shared by the dx and dW calls
 extern "C" size_t tfrs_cross_tc_bwd_workspace_bytes(int64_t B, int D) {
   if (B <= 0 || D <= 0) return 0;
-  return align_up((size_t)B * D * 4, 1024) + align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024) + tc::cross_tc_bwd_gemm_workspace(B, D);
+  const size_t dx_ws = tc::gemm_tc_workspace(B, D, D, tc::GEMM_EPI_DX), dw_ws = tc::gemm_tc_workspace(D, D, B);
+  return align_up((size_t)B * D * 4, 1024) + align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024) + 1024 + (dx_ws > dw_ws ? dx_ws : dw_ws);
 }
 
 extern "C" int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const float* W, const float* prod,
@@ -177,15 +196,23 @@ extern "C" int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const floa
   unsigned char* w = (unsigned char*)ws;
   float* gp = (float*)w; w += align_up((size_t)B * D * 4, 1024);
   float* colpart = (float*)w; w += align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024);
-  const size_t gemm_ws = ws_bytes - (size_t)(w - (unsigned char*)ws);
+  unsigned int* gp_amax = (unsigned int*)w; w += 1024;
+  const size_t gws = ws_bytes - (size_t)(w - (unsigned char*)ws);
   const long long total = (long long)B * D;
   const unsigned blocks = (unsigned)(ceil_div(total, 256) < 148 * 16 ? ceil_div(total, 256) : 148 * 16);
-  // max |gp| is produced by the element-wise pass itself (first word of the GEMM workspace = its CxStats slot)
-  TFRS_CUDA(cudaMemsetAsync(w, 0, 4096, st));
-  cross_bwd_elem<<<blocks, 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, (dx || dW) ? (unsigned int*)w : nullptr);
+  // max |gp| comes out of the element-wise pass: the two GEMMs skip their statistics pass over gp
+  TFRS_CUDA(cudaMemsetAsync(gp_amax, 0, sizeof(unsigned int), st));
+  cross_bwd_elem<<<blocks, 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, gp_amax);
   TFRS_LAUNCH_CHECK();
-  if (dx || dW) {
-    int rc = tc::cross_tc_bwd_gemms(x, W, gp, dout, B, D, ld, diag_scale, dx, dW, w, gemm_ws, st);
+  int rc;
+  if (dx) {   // dx[b, i] = sum_o gp[b, o] W[i, o] + diag gp[b, i] + g[b, i]
+    rc = tc::gemm_tc(tc::GemmOperand{gp, D, false, gp_amax}, tc::GemmOperand{W, D, false}, B, D, D,
+                     tc::GemmEpilogue{tc::GEMM_EPI_DX, gp, D, dout, ld, nullptr, diag_scale, nullptr}, dx, ld, w, gws, st);
+    if (rc) return rc;
+  }
+  if (dW) {   // dW[i, o] = sum_b x[b, i] gp[b, o]
+    rc = tc::gemm_tc(tc::GemmOperand{x, ld, true}, tc::GemmOperand{gp, D, true, gp_amax}, D, D, B,
+                     tc::GemmEpilogue{tc::GEMM_EPI_PLAIN, nullptr, 0, nullptr, 0, nullptr, 0.f, nullptr}, dW, D, w, gws, st);
     if (rc) return rc;
   }
   if (dbias) {

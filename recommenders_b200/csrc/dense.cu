@@ -1,12 +1,12 @@
 // dense.cu -- K6: the Dense layer of the ranking MLPs (tf.keras.layers.Dense in layers/blocks.py:24-61 and
 // experimental/models/ranking.py:27-257):  y = act(x . W + bias),  W [in, out] as Keras stores it.
-//   tensor cores (B >= 1024, K >= 64, N >= 64): split-fp16 wgmma GEMM (cross_tc_bwd.cu) with a DENSE epilogue;
+//   tensor cores (B >= 1024, K >= 64, N >= 64): split-fp16 wgmma GEMM (split_gemm.cu) with a DENSE epilogue;
 //   otherwise exact CUDA-core kernels whose outputs are the canonical sequential fmaf chain + bias + activation
 //   (a warp per row for narrow layers, N <= 16, e.g. the Dense(1) logit layer; the exact SGEMM above that).
 //   bwd: dz = dy * act'(y) + dlogits (from the saved output) ; db = colsum(dz) (two-level fixed-order float64 reduction) ;
 //        dx = dz . W^T ; dW = x^T . dz (batch cut into chunks, partials summed in fixed order).  No float atomics.
 #include "sgemm.cuh"
-#include "cross_tc.cuh"
+#include "split_gemm.cuh"
 #include "dense.cuh"
 
 namespace tfrs {

@@ -1,5 +1,5 @@
 // dense.cuh -- activations of the Dense layer (K6), shared by the exact kernels (dense.cu) and the DENSE epilogues of the
-// split-fp16 tensor-core GEMM (cross_tc_bwd.cu).
+// split-fp16 tensor-core GEMM (split_gemm.cu).
 #pragma once
 #include "common.cuh"
 

@@ -329,10 +329,10 @@ extern "C" int tfrs_inbatch_softmax_tc_fwd_ex(const float* q, const float* c, in
   TFRS_LAUNCH_CHECK();
   {
     long long chunks = pl.Bp / 128 * 128 * (long long)pl.kb * 8;
-    cx_split_image_kernel<false><<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(q, B, d, d, pl.kb, pl.Bp / 128, qst, qimg);
+    cx_split_image_kernel<<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(q, B, d, d, pl.kb, pl.Bp / 128, qst, qimg);
     TFRS_LAUNCH_CHECK();
     chunks = pl.n_ctiles * 128 * (long long)pl.kb * 8;
-    cx_split_image_kernel<false><<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(c, C, d, d, pl.kb, pl.n_ctiles, cst, cimg);
+    cx_split_image_kernel<<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(c, C, d, d, pl.kb, pl.n_ctiles, cst, cimg);
     TFRS_LAUNCH_CHECK();
   }
   SoftmaxTcParams p{};

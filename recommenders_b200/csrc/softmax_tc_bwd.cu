@@ -341,9 +341,9 @@ extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, in
   TFRS_LAUNCH_CHECK();
   cx_exp_kernel<<<1, 1, 0, st>>>(cst);
   TFRS_LAUNCH_CHECK();
-  cx_split_image_kernel<false><<<(unsigned)ceil_div(pl.q_tiles * 128 * 8, 256), 256, 0, st>>>(q, B, d, d, 1, pl.q_tiles, qst, qimg);
+  cx_split_image_kernel<<<(unsigned)ceil_div(pl.q_tiles * 128 * 8, 256), 256, 0, st>>>(q, B, d, d, 1, pl.q_tiles, qst, qimg);
   TFRS_LAUNCH_CHECK();
-  cx_split_image_kernel<false><<<(unsigned)ceil_div(pl.c_tiles * 128 * 8, 256), 256, 0, st>>>(c, C, d, d, 1, pl.c_tiles, cst, cimg);
+  cx_split_image_kernel<<<(unsigned)ceil_div(pl.c_tiles * 128 * 8, 256), 256, 0, st>>>(c, C, d, d, 1, pl.c_tiles, cst, cimg);
   TFRS_LAUNCH_CHECK();
   sb_wstats_kernel<<<1, 1024, 0, st>>>(sample_weight, B, wst);
   TFRS_LAUNCH_CHECK();

@@ -49,9 +49,8 @@ static __global__ void cx_exp_kernel(CxStats* st) {
   st->exp = ok ? (CX_TARGET_EXP - x) : 0;
 }
 
-// fp32 [rows, D] (row stride ld; or its transpose when TRANSPOSED) -> hi/lo fp16 tile image:
+// fp32 [rows, K] (row stride ld) -> hi/lo fp16 tile image:
 //   tile t (128 rows) : slab s (64 K) : {hi, lo} : 128 rows x 128 B, 16-byte chunk j of row r at chunk j ^ (r & 7)
-template <bool TRANSPOSED>
 static __global__ void __launch_bounds__(256)
 cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long long ld, int kb, long long n_tiles,
                       const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
@@ -71,7 +70,7 @@ cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       float f = 0.f;
-      if (row < rows && k0 + j < K) f = TRANSPOSED ? src[(long long)(k0 + j) * ld + row] : src[row * ld + k0 + j];
+      if (row < rows && k0 + j < K) f = src[row * ld + k0 + j];
       const float v = ldexpf(f, sexp);
       const __half h = __float2half_rn(v);
       hi[j] = h;

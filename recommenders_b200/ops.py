@@ -641,15 +641,6 @@ def sparse_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.Tensor,
 # Cross layers at least this large run their forward GEMM on the tensor cores (fp16 hi/lo split, fp32 accumulate).
 CROSS_TC_MIN_B = 1024
 CROSS_TC_MIN_D = 64
-def cross_weight_image(W: torch.Tensor) -> torch.Tensor:
-  """K-major fp16 hi/lo image of W^T for the tensor-core Cross kernel, rebuilt on every call: the split is
-  O(D^2) against the O(B*D^2) GEMM (2.9 MB at D=845), and a cache keyed on (data_ptr, _version) can serve a stale
-  image after the allocator recycles an address or after an in-place `.data` update."""
-  D = W.shape[0]
-  nb = lib().tfrs_cross_tc_weight_bytes(D)
-  buf = workspace(nb, W.device, f"cross_w{D}")
-  check(lib().tfrs_cross_tc_weight_build(ptr(W), D, ptr(buf), nb, stream()), "cross_tc_weight_build")
-  return buf
 
 
 class _Cross(torch.autograd.Function):
@@ -667,11 +658,9 @@ class _Cross(torch.autograd.Function):
     # statistic instead of a pass over its input (0 on the exact path: "unknown")
     out_amax = torch.zeros((1,), dtype=torch.int32, device=x0.device)
     if ctx.used_tc:
-      wimg = cross_weight_image(W)
-      wsb = lib().tfrs_cross_tc_workspace_bytes(B, D)
-      ws = workspace(wsb, x0.device, "cross_tc")
-      check(lib().tfrs_cross_tc_fwd_ex_f32(ptr(x0), ptr(x), ptr(wimg), ptr(b), B, D, D, c_f(diag_scale), ptr(out), ptr(prod),
-                                           ptr(x_amax), ptr(out_amax), ptr(ws), ws.numel(), stream()), "cross_tc_fwd")
+      ws = workspace(lib().tfrs_cross_tc_workspace_bytes(B, D), x0.device, "cross_tc")
+      check(lib().tfrs_cross_tc_fwd_f32(ptr(x0), ptr(x), ptr(W), ptr(b), B, D, D, c_f(diag_scale), ptr(out), ptr(prod),
+                                        ptr(x_amax), ptr(out_amax), ptr(ws), ws.numel(), stream()), "cross_tc_fwd")
     else:
       check(lib().tfrs_cross_fwd_f32(ptr(x0), ptr(x), ptr(W), ptr(b), B, D, D, c_f(diag_scale), ptr(out), ptr(prod),
                                      stream()), "cross_fwd")

@@ -32,7 +32,7 @@ def test_library_builds_and_exports_every_declared_symbol():
   assert set(declared) == set(_ffi.EXPORTS), set(declared) ^ set(_ffi.EXPORTS)
   # no-compute calls are safe without a GPU
   l = _ffi.lib()
-  assert l.tfrs_version() == 100
+  assert l.tfrs_version() == 101
   assert l.tfrs_topk_scan_workspace_bytes(4096, 1000000, 64, 100) > 0
   assert l.tfrs_launch_count() == 0
 

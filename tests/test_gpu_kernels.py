@@ -144,7 +144,8 @@ def test_inbatch_softmax_loss_and_grads(ops, B, C, d, temp, weighted):
 
 
 @pytest.mark.parametrize("B,D,diag,bias", [(1, 3, 0.0, False), (257, 845, 0.0, True), (100, 64, 1.0, True), (5000, 130, 0.5, False),
-                                           (4096, 845, 0.0, True), (1500, 64, 0.25, False), (2048, 200, 0.0, True)])
+                                           (4096, 845, 0.0, True), (1500, 64, 0.25, False), (2048, 200, 0.0, True),
+                                           (2048, 1100, 0.25, True)])   # D > 1024: one accumulation chain over all of K
 def test_cross_fwd_bwd(ops, B, D, diag, bias):
   """1e-5 relative to the output scale (fp32 kernel vs float64 oracle)."""
   rng = np.random.RandomState(B + D)

@@ -159,6 +159,16 @@ def test_gemm_tc_vs_float64(ops, M, N, K, ta, tb):
   _close(out.cpu().numpy(), ref, 1e-5, "gemm_tc")   # split-fp16 products: ~2^-21 relative to |a||b|
 
 
+def test_gemm_tc_transposed_operand_of_tiny_magnitude(ops):
+  """max |a| ~ 1e-36 < 2^-113: the power-of-two rescale 2^exp is not a finite float on its own, yet the transposed
+  operands (both read transposed here) must give finite images and the usual 1e-5 accuracy."""
+  M, N, K = 257, 64, 5000
+  a = _rand((K, M), 71, 1e-36); b = _rand((K, N), 72)
+  out = ops.gemm_tc(a, b, True, False)
+  ref = a.cpu().numpy().astype(np.float64).T @ b.cpu().numpy().astype(np.float64)
+  _close(out.cpu().numpy(), ref, 1e-5, "gemm_tc")
+
+
 def _lowrank_ref_grads(x0, x, U, V, b, g, diag):
   x0, x, U, V, g = (np.asarray(a, np.float64) for a in (x0, x, U, V, g))
   t = x @ U
