@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define TFRS_B200_VERSION 101 /* 0.1.1 */
+#define TFRS_B200_VERSION 102 /* 0.1.2 */
 
 enum {
   TFRS_OK = 0,
@@ -234,46 +234,35 @@ int tfrs_inbatch_softmax_bwd(const float* q, const float* c, int64_t B, int64_t 
                              const float* grad_loss, float* dq, float* dc, void* ws, size_t ws_bytes,
                              void* stream);
 
-/* K3 forward on the tensor cores (same contract and outputs as tfrs_inbatch_softmax_fwd; d <= 128):
- * hi/lo fp16 split of q and c (|err| <= 2^-21 |q||c| on a score), wgmma GEMM with fp32 register accumulation and
- * an online log-sum-exp epilogue -- the [B,C] logits are never written.  `candidate_bias` (nullable, [C]) is added
- * to every logit of its column after the temperature: with bias_j = -log(clip(p_j, 1e-6, 1)) it is the
- * sampling-probability correction of tasks/retrieval.py:190-192 / layers/loss.py:150-158.  Returns TFRS_ERR_UNSUPPORTED
- * (workspace_bytes == 0) outside its shape range; the caller then uses tfrs_inbatch_softmax_fwd. */
-size_t tfrs_inbatch_softmax_tc_workspace_bytes(int64_t B, int64_t C, int d);
-int tfrs_inbatch_softmax_tc_fwd(const float* q, const float* c, int64_t B, int64_t C, int d,
-                                float inv_temperature, const float* sample_weight, const float* candidate_bias,
-                                float* loss, float* lse, void* ws, size_t ws_bytes, void* stream);
-
-/* K3b on the tensor cores (same contract and outputs as tfrs_inbatch_softmax_bwd; d <= 64): two launches of one
- * flash-attention-backward-shaped kernel -- S = X.Y^T (wgmma, split fp16 operands), G built on the register
- * fragment of S, dX += G.Y with G as the register A operand of the next wgmma and the Y tile as an MN-major
- * operand; X = q gives dq, X = c gives dc.  Deterministic (no atomics).  workspace_bytes == 0 / TFRS_ERR_UNSUPPORTED
- * outside its range. */
-size_t tfrs_inbatch_softmax_tc_bwd_workspace_bytes(int64_t B, int64_t C, int d);
-int tfrs_inbatch_softmax_tc_bwd(const float* q, const float* c, int64_t B, int64_t C, int d,
-                                float inv_temperature, const float* sample_weight, const float* candidate_bias,
-                                const float* lse, const float* grad_loss, float* dq, float* dc, void* ws,
-                                size_t ws_bytes, void* stream);
-
-/* The remaining tfrs.tasks.Retrieval loss options inside the tensor-core loss (SURVEY 8f-3), forward and backward:
- *   candidate_ids  (nullable, int64 [C])     remove_accidental_hits: every candidate j != i whose id equals the id of query
- *                                            i's positive (candidate i) gets logit MIN_FLOAT (tasks/retrieval.py:194-200,
- *                                            layers/loss.py:114-147; `logits + dup * MIN_FLOAT` rounds to MIN_FLOAT in fp32)
- *   score_mask     (nullable, uint8 [B, C])  where(mask, s, MIN_FLOAT) (retrieval.py:202-203); row-major, nonzero = keep
- * applied after the temperature and the bias, in the reference's order.  The ids / keep-bits are tested against the fp32
- * accumulators in registers: no [B,C] logits, labels or masks are materialised (the byte mask is packed to bits once).
- * Masked entries get zero gradient.  Same shape limits as the plain entry points; *_ex_workspace_bytes sizes `ws`. */
-size_t tfrs_inbatch_softmax_tc_ex_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask);
-int tfrs_inbatch_softmax_tc_fwd_ex(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                   const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
-                                   const uint8_t* score_mask, float* loss, float* lse, void* ws, size_t ws_bytes,
-                                   void* stream);
-size_t tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask);
-int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                   const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
-                                   const uint8_t* score_mask, const float* lse, const float* grad_loss, float* dq, float* dc,
-                                   void* ws, size_t ws_bytes, void* stream);
+/* K3 on the tensor cores, forward (same contract and outputs as tfrs_inbatch_softmax_fwd; d <= 128) and backward (same as
+ * tfrs_inbatch_softmax_bwd; d <= 64).
+ *   forward:  hi/lo fp16 split of q and c (|err| <= 2^-21 |q||c| on a score), wgmma GEMM with fp32 register accumulation
+ *             and an online log-sum-exp epilogue -- the [B,C] logits are never written.
+ *   backward: two launches of one flash-attention-backward-shaped kernel -- S = X.Y^T (wgmma, split fp16 operands), G built
+ *             on the register fragment of S, dX += G.Y with G as the register A operand of the next wgmma and the Y tile as
+ *             an MN-major operand; X = q gives dq, X = c gives dc.  Deterministic (no atomics).
+ * The tfrs.tasks.Retrieval loss options (SURVEY 8f-3), each nullable:
+ *   candidate_bias (float [C])       added to every logit of its column after the temperature: with
+ *                                    bias_j = -log(clip(p_j, 1e-6, 1)) it is the sampling-probability correction of
+ *                                    tasks/retrieval.py:190-192 / layers/loss.py:150-158
+ *   candidate_ids  (int64 [C])       remove_accidental_hits: every candidate j != i whose id equals the id of query i's
+ *                                    positive (candidate i) gets logit MIN_FLOAT (tasks/retrieval.py:194-200,
+ *                                    layers/loss.py:114-147; `logits + dup * MIN_FLOAT` rounds to MIN_FLOAT in fp32)
+ *   score_mask     (uint8 [B, C])    where(mask, s, MIN_FLOAT) (retrieval.py:202-203); row-major, nonzero = keep
+ * ids and mask are applied after the temperature and the bias, in the reference's order.  The ids / keep-bits are tested against the fp32 accumulators in
+ * registers: no [B,C] logits, labels or masks are materialised (the byte mask is packed to bits once).  Masked entries get
+ * zero gradient.  *_workspace_bytes sizes `ws` for the options given (has_ids = candidate_ids != NULL, has_mask =
+ * score_mask != NULL); it returns 0, and the call TFRS_ERR_UNSUPPORTED, outside the shape range; the caller then uses
+ * tfrs_inbatch_softmax_fwd / _bwd. */
+size_t tfrs_inbatch_softmax_tc_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask);
+int tfrs_inbatch_softmax_tc_fwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
+                                const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
+                                const uint8_t* score_mask, float* loss, float* lse, void* ws, size_t ws_bytes, void* stream);
+size_t tfrs_inbatch_softmax_tc_bwd_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask);
+int tfrs_inbatch_softmax_tc_bwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
+                                const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
+                                const uint8_t* score_mask, const float* lse, const float* grad_loss, float* dq, float* dc,
+                                void* ws, size_t ws_bytes, void* stream);
 
 /* Multi-head queries (tasks/retrieval.py:172-176): q is [B,H,d] and  scores_ij = max_h q_ih . c_j  ("maxsim") before the same
  * loss.  Exact fp32 path: row blocks of the [B*H, C] head scores stay L2-resident, the head maximum is folded while the

@@ -65,14 +65,10 @@ _SIGNATURES = {
     "tfrs_inbatch_softmax_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
     "tfrs_inbatch_softmax_fwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_inbatch_softmax_bwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_inbatch_softmax_tc_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
-    "tfrs_inbatch_softmax_tc_fwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_inbatch_softmax_tc_bwd_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
-    "tfrs_inbatch_softmax_tc_bwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_inbatch_softmax_tc_ex_workspace_bytes": (c_sz, [c_l, c_l, c_i, c_i, c_i]),
-    "tfrs_inbatch_softmax_tc_fwd_ex": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes": (c_sz, [c_l, c_l, c_i, c_i, c_i]),
-    "tfrs_inbatch_softmax_tc_bwd_ex": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_inbatch_softmax_tc_workspace_bytes": (c_sz, [c_l, c_l, c_i, c_i, c_i]),
+    "tfrs_inbatch_softmax_tc_fwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_inbatch_softmax_tc_bwd_workspace_bytes": (c_sz, [c_l, c_l, c_i, c_i, c_i]),
+    "tfrs_inbatch_softmax_tc_bwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_inbatch_softmax_maxsim_workspace_bytes": (c_sz, [c_l, c_i, c_l, c_i]),
     "tfrs_inbatch_softmax_maxsim_fwd": (c_i, [c_p, c_p, c_l, c_i, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_inbatch_softmax_maxsim_bwd": (c_i, [c_p, c_p, c_l, c_i, c_l, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),

@@ -50,6 +50,18 @@ __host__ __device__ __forceinline__ bool better(float sa, long long ia, float sb
 
 int sm_count();  // SMs of the CURRENT device (cached per device)
 
+// 256-thread blocks for a grid-stride loop over n elements: one element per thread, at most 16 blocks per SM
+static inline unsigned elementwise_grid(long long n) {
+  const long long want = ceil_div(n, 256), cap = (long long)sm_count() * 16;
+  return (unsigned)(want < cap ? want : cap);
+}
+
+// Fixed-order reductions (reduce.cu), one launch each.
+// out[m*ld + n] = sum_z partial[z][m*N + n] over z = 0 .. parts-1 ascending, in fp32
+int reduce_parts(const float* partial, long long M, long long N, int parts, float* out, long long ld, cudaStream_t st);
+// loss[0] = sum_i v[i * stride] over i < n, in fp64 and a fixed order
+int reduce_loss(const float* v, long long n, long long stride, float* loss, cudaStream_t st);
+
 // Hook of the sharded scan (topk_tc.cu <-> comm.cu): all device pointers; thr[q] = L_q - margin_q in the shard's screening
 // units (scores scaled by 2^(*exp_corpus + qexp[q])), cut[q] = 2 eps_q.  The hook may raise thr[].
 typedef int (*ThrHook)(void* ctx, float* thr, const float* margin, const float* cut, const int* qexp, const int* exp_corpus,

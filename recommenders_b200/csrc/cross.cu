@@ -83,18 +83,16 @@ cross_colsum_partial(const float* __restrict__ gp, long long B, int D, long long
   partial[(long long)blockIdx.y * D + n] = a;
 }
 
-// out[e] = sum_z partial[z][e]  (z ascending)
-__global__ void __launch_bounds__(256)
-cross_reduce_splits(const float* __restrict__ partial, long long elems, int splits, float* __restrict__ out) {
-  long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (e >= elems) return;
-  float a = partial[e];
-  for (int z = 1; z < splits; ++z) a += partial[(long long)z * elems + e];
-  out[e] = a;
-}
-
-static int cross_splits(long long B) { long long z = ceil_div(B, 4096); return (int)(z < 1 ? 1 : (z > 16 ? 16 : z)); }
 constexpr int CROSS_COL_SPLITS = 64;
+
+// dbias = colsum(gp): row-split partials, then their fixed-order sum
+static int cross_colsum(const float* gp, long long B, int D, float* colpart, float* dbias, cudaStream_t st) {
+  const long long rps = ceil_div(B, CROSS_COL_SPLITS);
+  const int used = (int)ceil_div(B, rps);
+  cross_colsum_partial<<<dim3((unsigned)ceil_div(D, 256), (unsigned)used), 256, 0, st>>>(gp, B, D, rps, colpart);
+  TFRS_LAUNCH_CHECK();
+  return reduce_parts(colpart, 1, D, used, dbias, D, st);
+}
 
 }  // namespace tfrs
 using namespace tfrs;
@@ -112,7 +110,7 @@ extern "C" int tfrs_cross_fwd_f32(const float* x0, const float* x, const float* 
 
 extern "C" size_t tfrs_cross_bwd_workspace_bytes(int64_t B, int D) {
   if (B <= 0 || D <= 0) return 256;
-  return align_up((size_t)B * D * 4, 256) + align_up((size_t)cross_splits(B) * D * D * 4, 256) +
+  return align_up((size_t)B * D * 4, 256) + align_up((size_t)sgemm_batch_splits(B) * D * D * 4, 256) +
          align_up((size_t)CROSS_COL_SPLITS * D * 4, 256);
 }
 
@@ -126,13 +124,11 @@ extern "C" int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* 
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* w = (unsigned char*)ws;
   float* gp = (float*)w; w += align_up((size_t)B * D * 4, 256);
-  const int Z = cross_splits(B);
+  const int Z = sgemm_batch_splits(B);
   float* part = (float*)w; w += align_up((size_t)Z * D * D * 4, 256);
   float* colpart = (float*)w;
 
-  long long total = (long long)B * D;
-  unsigned blocks = (unsigned)(ceil_div(total, 256) < 148 * 16 ? ceil_div(total, 256) : 148 * 16);
-  cross_bwd_elem<<<blocks, 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, nullptr);
+  cross_bwd_elem<<<elementwise_grid((long long)B * D), 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, nullptr);
   TFRS_LAUNCH_CHECK();
   int rc;
   if (dx) {
@@ -140,24 +136,10 @@ extern "C" int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* 
     if (rc) return rc;
   }
   if (dW) {
-    rc = launch_sgemm<true, false>(x, ld, gp, D, D, D, (int)B, Z, EpiStoreSplit{part, D, (long long)D * D}, st);
+    rc = launch_sgemm_split_k<true, false>(x, ld, gp, D, D, D, (int)B, Z, part, dW, st);
     if (rc) return rc;
-    // launch_sgemm may use fewer splits than Z when B is small; recompute what it used
-    int kps = (int)(ceil_div(ceil_div(B, Z), SG_BK) * SG_BK);
-    int used = Z > 1 ? (int)ceil_div(B, kps) : 1;
-    cross_reduce_splits<<<(unsigned)ceil_div((long long)D * D, 256), 256, 0, st>>>(part, (long long)D * D, used, dW);
-    TFRS_LAUNCH_CHECK();
   }
-  if (dbias) {
-    long long rps = ceil_div(B, CROSS_COL_SPLITS);
-    int used = (int)ceil_div(B, rps);
-    dim3 grid((unsigned)ceil_div(D, 256), (unsigned)used);
-    cross_colsum_partial<<<grid, 256, 0, st>>>(gp, B, D, rps, colpart);
-    TFRS_LAUNCH_CHECK();
-    cross_reduce_splits<<<(unsigned)ceil_div(D, 256), 256, 0, st>>>(colpart, D, used, dbias);
-    TFRS_LAUNCH_CHECK();
-  }
-  return TFRS_OK;
+  return dbias ? cross_colsum(gp, B, D, colpart, dbias, st) : TFRS_OK;
 }
 
 // ---- K5 / K5b on the tensor cores: one split-fp16 GEMM forward, two backward; same contract and outputs as the exact path
@@ -198,11 +180,9 @@ extern "C" int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const floa
   float* colpart = (float*)w; w += align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024);
   unsigned int* gp_amax = (unsigned int*)w; w += 1024;
   const size_t gws = ws_bytes - (size_t)(w - (unsigned char*)ws);
-  const long long total = (long long)B * D;
-  const unsigned blocks = (unsigned)(ceil_div(total, 256) < 148 * 16 ? ceil_div(total, 256) : 148 * 16);
   // max |gp| comes out of the element-wise pass: the two GEMMs skip their statistics pass over gp
   TFRS_CUDA(cudaMemsetAsync(gp_amax, 0, sizeof(unsigned int), st));
-  cross_bwd_elem<<<blocks, 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, gp_amax);
+  cross_bwd_elem<<<elementwise_grid((long long)B * D), 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, gp_amax);
   TFRS_LAUNCH_CHECK();
   int rc;
   if (dx) {   // dx[b, i] = sum_o gp[b, o] W[i, o] + diag gp[b, i] + g[b, i]
@@ -215,16 +195,7 @@ extern "C" int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const floa
                      tc::GemmEpilogue{tc::GEMM_EPI_PLAIN, nullptr, 0, nullptr, 0, nullptr, 0.f, nullptr}, dW, D, w, gws, st);
     if (rc) return rc;
   }
-  if (dbias) {
-    long long rps = ceil_div(B, CROSS_COL_SPLITS);
-    int used = (int)ceil_div(B, rps);
-    dim3 grid((unsigned)ceil_div(D, 256), (unsigned)used);
-    cross_colsum_partial<<<grid, 256, 0, st>>>(gp, B, D, rps, colpart);
-    TFRS_LAUNCH_CHECK();
-    cross_reduce_splits<<<(unsigned)ceil_div(D, 256), 256, 0, st>>>(colpart, D, used, dbias);
-    TFRS_LAUNCH_CHECK();
-  }
-  return TFRS_OK;
+  return dbias ? cross_colsum(gp, B, D, colpart, dbias, st) : TFRS_OK;
 }
 
 // ---- general tensor-core GEMM (the low-rank Cross projections; ops.matmul on large shapes) --------------------------------
@@ -300,9 +271,7 @@ extern "C" int tfrs_cross_lowrank_tc_bwd_f32(const float* x0, const float* x, co
   float* dt = (float*)w; w += align_up((size_t)B * p * 4, 1024);
   float* colpart = (float*)w; w += align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024);
   const size_t gws = ws_bytes - (size_t)(w - (unsigned char*)ws);
-  const long long total = (long long)B * D;
-  const unsigned blocks = (unsigned)(ceil_div(total, 256) < 148 * 16 ? ceil_div(total, 256) : 148 * 16);
-  cross_bwd_elem<<<blocks, 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, nullptr);
+  cross_bwd_elem<<<elementwise_grid((long long)B * D), 256, 0, st>>>(x0, prod, dout, B, D, ld, gp, dx0, nullptr);
   TFRS_LAUNCH_CHECK();
   const tc::GemmEpilogue plain{tc::GEMM_EPI_PLAIN, nullptr, 0, nullptr, 0, nullptr, 0.f, nullptr};
   int rc;
@@ -323,14 +292,5 @@ extern "C" int tfrs_cross_lowrank_tc_bwd_f32(const float* x0, const float* x, co
                      tc::GemmEpilogue{tc::GEMM_EPI_DX, gp, D, dout, ld, nullptr, diag_scale, nullptr}, dx, ld, w, gws, st);
     if (rc) return rc;
   }
-  if (dbias) {
-    long long rps = ceil_div(B, CROSS_COL_SPLITS);
-    int used = (int)ceil_div(B, rps);
-    dim3 grid((unsigned)ceil_div(D, 256), (unsigned)used);
-    cross_colsum_partial<<<grid, 256, 0, st>>>(gp, B, D, rps, colpart);
-    TFRS_LAUNCH_CHECK();
-    cross_reduce_splits<<<(unsigned)ceil_div(D, 256), 256, 0, st>>>(colpart, D, used, dbias);
-    TFRS_LAUNCH_CHECK();
-  }
-  return TFRS_OK;
+  return dbias ? cross_colsum(gp, B, D, colpart, dbias, st) : TFRS_OK;
 }

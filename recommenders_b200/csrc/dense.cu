@@ -84,23 +84,12 @@ dense_colsum_reduce(const double* __restrict__ partial, int N, int splits, float
   out[n] = (float)a;
 }
 
-__global__ void __launch_bounds__(256)
-dense_reduce_splits(const float* __restrict__ partial, long long elems, int splits, float* __restrict__ out) {
-  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (e >= elems) return;
-  float a = partial[e];
-  for (int z = 1; z < splits; ++z) a += partial[(long long)z * elems + e];
-  out[e] = a;
-}
-
-static int dense_splits(long long B) { long long z = ceil_div(B, 4096); return (int)(z < 1 ? 1 : (z > 16 ? 16 : z)); }
-
 static size_t dense_bwd_gemm_ws(long long B, int K, int N) {
   if (dense_tc(B, K, N)) {
     const size_t a = tc::gemm_tc_workspace(B, K, N), b = tc::gemm_tc_workspace(K, N, B);
     return a > b ? a : b;
   }
-  return (size_t)dense_splits(B) * K * N * 4;
+  return (size_t)sgemm_batch_splits(B) * K * N * 4;
 }
 
 }  // namespace tfrs
@@ -151,8 +140,7 @@ extern "C" int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y
   double* colpart = (double*)w; w += align_up((size_t)DENSE_COL_SPLITS * N * 8, 1024);
   const size_t gws = ws_bytes - (size_t)(w - (unsigned char*)ws);
   const long long total = (long long)B * N;
-  const unsigned blocks = (unsigned)(ceil_div(total, 256) < 132 * 16 ? ceil_div(total, 256) : 132 * 16);
-  dense_dz_kernel<<<blocks, 256, 0, st>>>(y, dy, dlogits, total, activation, dz);
+  dense_dz_kernel<<<elementwise_grid(total), 256, 0, st>>>(y, dy, dlogits, total, activation, dz);
   TFRS_LAUNCH_CHECK();
   int rc;
   if (dense_tc(B, K, N)) {
@@ -171,15 +159,8 @@ extern "C" int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y
       if (rc) return rc;
     }
     if (dW) {
-      float* part = (float*)w;
-      const int Z = dense_splits(B);
-      rc = launch_sgemm<true, false>(x, K, dz, N, K, N, (int)B, Z, EpiStoreSplit{part, N, (long long)K * N}, st);
+      rc = launch_sgemm_split_k<true, false>(x, K, dz, N, K, N, (int)B, sgemm_batch_splits(B), (float*)w, dW, st);
       if (rc) return rc;
-      // launch_sgemm may use fewer splits than Z when B is small; recompute what it used
-      const int kps = (int)(ceil_div(ceil_div(B, Z), SG_BK) * SG_BK);
-      const int used = Z > 1 ? (int)ceil_div(B, kps) : 1;
-      dense_reduce_splits<<<(unsigned)ceil_div((long long)K * N, 256), 256, 0, st>>>(part, (long long)K * N, used, dW);
-      TFRS_LAUNCH_CHECK();
     }
   }
   if (dbias) {

@@ -52,18 +52,6 @@ hardneg_fwd_kernel(const float* __restrict__ top_s, const long long* __restrict_
   }
 }
 
-// loss = sum of the row losses, fixed order, fp64
-__global__ void __launch_bounds__(1024)
-hardneg_reduce_kernel(const float* __restrict__ coef, long long B, int stride, float* __restrict__ loss) {
-  __shared__ double red[1024];
-  double a = 0.0;
-  for (long long i = threadIdx.x; i < B; i += 1024) a += (double)coef[i * stride + stride - 1];
-  red[threadIdx.x] = a;
-  __syncthreads();
-  for (int s = 512; s > 0; s >>= 1) { if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s]; __syncthreads(); }
-  if (threadIdx.x == 0) loss[0] = (float)red[0];
-}
-
 // one warp per query: dq_i (registers, fixed order) and the scattered dc contributions
 __global__ void __launch_bounds__(256)
 hardneg_bwd_kernel(const float* __restrict__ q, const float* __restrict__ c, long long B, int d,
@@ -105,9 +93,7 @@ extern "C" int tfrs_hardneg_loss_fwd(const float* top_scores, const int64_t* top
   hardneg_fwd_kernel<<<(unsigned)ceil_div(B * 32, 256), 256, 0, st>>>(top_scores, (const long long*)top_idx, B, k1, positive_scores,
                                                                        inv_temperature, sample_weight, coef);
   TFRS_LAUNCH_CHECK();
-  hardneg_reduce_kernel<<<1, 1024, 0, st>>>(coef, B, k1 + 2, loss);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
+  return reduce_loss(coef + k1 + 1, B, k1 + 2, loss, st);   // the row losses, fixed order, fp64
 }
 
 extern "C" int tfrs_hardneg_loss_bwd(const float* q, const float* c, int64_t B, int64_t C, int d, const int64_t* top_idx, int k1,

@@ -164,27 +164,28 @@ struct EpiStoreSplit {  // partial[z][m*ldc + n] = v   (deterministic split-K; r
   }
 };
 
-// out[e] (+)= sum_z partial[z][e]  (z ascending: deterministic split-K reduction)
-static __global__ void __launch_bounds__(256)
-reduce_splits_kernel(const float* __restrict__ partial, long long elems, int splits, float* __restrict__ out) {
-  long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (e >= elems) return;
-  float a = partial[e];
-  for (int z = 1; z < splits; ++z) a += partial[(long long)z * elems + e];
-  out[e] = a;
-}
-
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// Host launcher.  splits > 1 => K is cut into `splits` ranges (multiple of 16), blockIdx.z = range.
+// How launch_sgemm cuts K for a request of `splits` ranges: kps indices per range (a multiple of SG_BK) and the number of
+// ranges it runs, which is never more than requested.
+struct SgemmSplit { int kps, splits; };
+static inline SgemmSplit sgemm_split(int K, int splits) {
+  if (splits <= 1 || K <= 0) return {K > 0 ? K : SG_BK, 1};
+  const int kps = (int)(ceil_div(ceil_div(K, splits), SG_BK) * SG_BK);
+  return {kps, (int)ceil_div(K, kps)};
+}
+
+// Split count for a reduction over the batch (K = B): ranges of about 4096 rows, at most 16.
+static inline int sgemm_batch_splits(long long B) { long long z = ceil_div(B, 4096); return (int)(z < 1 ? 1 : (z > 16 ? 16 : z)); }
+
+// Host launcher.  splits > 1 => K is cut as sgemm_split says, blockIdx.z = range.
 template <bool TA, bool TB, class Epi>
 static inline int launch_sgemm(const float* A, long long lda, const float* B, long long ldb, int M, int N, int K,
                                int splits, Epi epi, cudaStream_t st) {
   if (M <= 0 || N <= 0) return TFRS_OK;
-  int kps = K;
-  if (splits > 1) { kps = (int)(ceil_div(ceil_div(K, splits), SG_BK) * SG_BK); splits = (int)ceil_div(K, kps); }
-  else splits = 1;
-  if (kps <= 0) kps = SG_BK;
+  const SgemmSplit sp = sgemm_split(K, splits);
+  const int kps = sp.kps;
+  splits = sp.splits;
   bool vecA = !TA && (lda % 4 == 0) && aligned16(A);
   bool vecB = TB && (ldb % 4 == 0) && aligned16(B);
   const bool skinny = N <= 64;  // 64-column tiles: no half-empty tiles for the [*, d] outputs of the backward passes
@@ -194,6 +195,17 @@ static inline int launch_sgemm(const float* A, long long lda, const float* B, lo
   else sgemm_kernel<TA, TB, SG_BN, Epi><<<grid, SG_THREADS, 0, st>>>(A, lda, B, ldb, M, N, K, kps, vecA, vecB, epi);
   TFRS_LAUNCH_CHECK();
   return TFRS_OK;
+}
+
+// Exact split-K:  out[M,N] (contiguous) = the per-range chains of launch_sgemm summed in fixed order (range ascending).
+// `partial` holds `splits` x M x N floats; the launch may use fewer ranges, never more.
+template <bool TA, bool TB>
+static inline int launch_sgemm_split_k(const float* A, long long lda, const float* B, long long ldb, int M, int N, int K, int splits,
+                                       float* partial, float* out, cudaStream_t st) {
+  const long long elems = (long long)M * N;
+  const int rc = launch_sgemm<TA, TB>(A, lda, B, ldb, M, N, K, splits, EpiStoreSplit{partial, N, elems}, st);
+  if (rc) return rc;
+  return reduce_parts(partial, M, N, sgemm_split(K, splits).splits, out, N, st);
 }
 
 }  // namespace tfrs

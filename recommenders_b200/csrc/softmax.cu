@@ -58,16 +58,6 @@ sm_row_lse(const float* __restrict__ S, long long ldS, int C, long long row0, fl
   }
 }
 
-__global__ void __launch_bounds__(1024) sm_reduce_loss(const float* __restrict__ rowloss, long long B, float* __restrict__ loss) {
-  __shared__ double red[1024];
-  double a = 0.0;
-  for (long long i = threadIdx.x; i < B; i += 1024) a += (double)rowloss[i];
-  red[threadIdx.x] = a;
-  __syncthreads();
-  for (int s = 512; s > 0; s >>= 1) { if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s]; __syncthreads(); }
-  if (threadIdx.x == 0) loss[0] = (float)red[0];
-}
-
 // one CTA per row of the block: G = (exp(s - lse) - [j == i]) * w_i * grad_loss * invT, in place
 __global__ void __launch_bounds__(SM_THREADS)
 sm_make_grad(float* __restrict__ S, long long ldS, int C, int R, long long row0, float invT,
@@ -200,9 +190,7 @@ extern "C" int tfrs_inbatch_softmax_fwd(const float* q, const float* c, int64_t 
     sm_row_lse<<<rows, SM_THREADS, 0, st>>>(S, C, (int)C, r0, inv_temperature, sample_weight, lse, rowloss);
     TFRS_LAUNCH_CHECK();
   }
-  sm_reduce_loss<<<1, 1024, 0, st>>>(rowloss, B, loss);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
+  return reduce_loss(rowloss, B, 1, loss, st);
 }
 
 extern "C" int tfrs_inbatch_softmax_bwd(const float* q, const float* c, int64_t B, int64_t C, int d,
@@ -222,16 +210,9 @@ extern "C" int tfrs_inbatch_softmax_bwd(const float* q, const float* c, int64_t 
     sm_make_grad<<<(unsigned)rows, SM_THREADS, 0, st>>>(S, C, (int)C, rows, r0, inv_temperature, sample_weight, lse, grad_loss);
     TFRS_LAUNCH_CHECK();
     // dq[r0:r0+rows] = G . c      (M=rows, N=d, K=C; A=G row-major, B=c [C,d] not transposed); deterministic split-K
-    {
-      float* part = (float*)((unsigned char*)ws + align_up((size_t)R * C * 4, 256) + align_up((size_t)B * 4, 256));
-      const long long elems = (long long)rows * d;
-      rc = launch_sgemm<false, false>(S, C, c, d, rows, d, (int)C, SM_DQ_SPLITS, EpiStoreSplit{part, d, elems}, st);
-      if (rc) return rc;
-      int kps = (int)(ceil_div(ceil_div(C, SM_DQ_SPLITS), SG_BK) * SG_BK);
-      int used = (int)ceil_div(C, kps);
-      reduce_splits_kernel<<<(unsigned)ceil_div(elems, 256), 256, 0, st>>>(part, elems, used, dq + r0 * d);
-      TFRS_LAUNCH_CHECK();
-    }
+    float* part = (float*)((unsigned char*)ws + align_up((size_t)R * C * 4, 256) + align_up((size_t)B * 4, 256));
+    rc = launch_sgemm_split_k<false, false>(S, C, c, d, rows, d, (int)C, SM_DQ_SPLITS, part, dq + r0 * d, st);
+    if (rc) return rc;
     // dc (+)= G^T . q_blk         (M=C, N=d, K=rows; A=G read transposed)
     rc = launch_sgemm<true, false>(S, C, q + r0 * d, d, (int)C, d, rows, 1, EpiAccum{dc, d, r0 > 0}, st);
     if (rc) return rc;
@@ -269,9 +250,7 @@ extern "C" int tfrs_inbatch_softmax_maxsim_fwd(const float* q, const float* c, i
     sm_row_lse_maxsim<<<nq, SM_THREADS, 0, st>>>(S, C, (int)C, H, q0, inv_temperature, sample_weight, lse, rowloss);
     TFRS_LAUNCH_CHECK();
   }
-  sm_reduce_loss<<<1, 1024, 0, st>>>(rowloss, B, loss);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
+  return reduce_loss(rowloss, B, 1, loss, st);
 }
 
 extern "C" int tfrs_inbatch_softmax_maxsim_bwd(const float* q, const float* c, int64_t B, int H, int64_t C, int d,
@@ -293,12 +272,8 @@ extern "C" int tfrs_inbatch_softmax_maxsim_bwd(const float* q, const float* c, i
     if (rc) return rc;
     sm_make_grad_maxsim<<<(unsigned)nq, SM_THREADS, 0, st>>>(S, C, (int)C, H, q0, inv_temperature, sample_weight, lse, grad_loss);
     TFRS_LAUNCH_CHECK();
-    const long long elems = (long long)rows * d;
-    rc = launch_sgemm<false, false>(S, C, c, d, rows, d, (int)C, SM_DQ_SPLITS, EpiStoreSplit{part, d, elems}, st);
+    rc = launch_sgemm_split_k<false, false>(S, C, c, d, rows, d, (int)C, SM_DQ_SPLITS, part, dq + q0 * H * d, st);
     if (rc) return rc;
-    const int kps = (int)(ceil_div(ceil_div(C, SM_DQ_SPLITS), SG_BK) * SG_BK);
-    reduce_splits_kernel<<<(unsigned)ceil_div(elems, 256), 256, 0, st>>>(part, elems, (int)ceil_div(C, kps), dq + q0 * H * d);
-    TFRS_LAUNCH_CHECK();
     rc = launch_sgemm<true, false>(S, C, qb, d, (int)C, d, rows, 1, EpiAccum{dc, d, q0 > 0}, st);
     if (rc) return rc;
   }

@@ -234,32 +234,15 @@ smtc_combine_kernel(const float2* __restrict__ partial, int n_partials, const fl
   rowloss[row] = (w ? w[row] : 1.0f) * (((M - pos[row]) + lg) * 0.6931471805599453f);
 }
 
-__global__ void __launch_bounds__(1024) smtc_reduce_loss(const float* __restrict__ rowloss, long long B, float* __restrict__ loss) {
-  __shared__ double red[1024];
-  double a = 0.0;
-  for (long long i = threadIdx.x; i < B; i += 1024) a += (double)rowloss[i];
-  red[threadIdx.x] = a;
-  __syncthreads();
-  for (int s = 512; s > 0; s >>= 1) { if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s]; __syncthreads(); }
-  if (threadIdx.x == 0) loss[0] = (float)red[0];
-}
-
 struct SxPlan { int kb, nqb, parts; long long Bp, n_ctiles, idpad; size_t smem, o_qst, o_cst, o_qimg, o_cimg, o_partial, o_pos, o_rowloss, o_bias, o_idlo, o_idhi, o_mbits, total; };
 
-static bool sx_plan(long long B, long long C, int d, SxPlan& pl, bool has_ids = false, bool has_mask = false) {
+static bool sx_plan(long long B, long long C, int d, SxPlan& pl, bool has_ids, bool has_mask) {
   if (B <= 0 || C < B || d <= 0 || d > 128) return false;
   pl.kb = (int)ceil_div(d, 64);
   pl.nqb = (int)ceil_div(B, 256);
   pl.Bp = (long long)pl.nqb * 256;
   pl.n_ctiles = ceil_div(C, 128);
-  // candidate parts: minimise waves x (tiles per CTA + ~6 tile times of fixed cost: A load, pipeline fill, partials)
-  int parts = 1; double best = 1e30;
-  const int sms = sm_count();
-  for (int c = 1; c <= 16 && c <= pl.n_ctiles; ++c) {
-    const double cost = (double)ceil_div((long long)pl.nqb * c, sms) * ((double)ceil_div(pl.n_ctiles, c) + 6.0);
-    if (cost < best * 0.97) { best = cost; parts = c; }
-  }
-  pl.parts = parts;
+  pl.parts = stream_parts(pl.nqb, pl.n_ctiles);
   pl.smem = (size_t)(2 + sx_stages(pl.kb)) * pl.kb * 32768 + 1024 + 256;
   if (pl.smem > 227 * 1024) return false;
   size_t o = 0;
@@ -267,7 +250,7 @@ static bool sx_plan(long long B, long long C, int d, SxPlan& pl, bool has_ids = 
   pl.o_qst = take(sizeof(CxStats)); pl.o_cst = take(sizeof(CxStats));
   pl.o_qimg = take(cx_img_bytes(pl.Bp, d));
   pl.o_cimg = take(cx_img_bytes(pl.n_ctiles * 128, d));
-  pl.o_partial = take((size_t)pl.Bp * parts * 2 * sizeof(float2));
+  pl.o_partial = take((size_t)pl.Bp * pl.parts * 2 * sizeof(float2));
   pl.o_pos = take((size_t)pl.Bp * 4);
   pl.o_rowloss = take((size_t)pl.Bp * 4);
   pl.o_bias = take((size_t)pl.n_ctiles * 128 * 4);
@@ -284,11 +267,6 @@ static bool sx_plan(long long B, long long C, int d, SxPlan& pl, bool has_ids = 
 using namespace tfrs;
 using namespace tfrs::tc;
 
-extern "C" size_t tfrs_inbatch_softmax_tc_workspace_bytes(int64_t B, int64_t C, int d) {
-  SxPlan pl;
-  return sx_plan(B, C, d, pl) ? pl.total : 0;
-}
-
 // cbias2[i] = bias[i] * log2(e) for i < C, 0 on the padding (and everywhere when bias == NULL)
 __global__ void __launch_bounds__(256)
 smtc_bias_kernel(const float* __restrict__ bias, long long C, long long Cpad, float* __restrict__ cbias2) {
@@ -296,15 +274,15 @@ smtc_bias_kernel(const float* __restrict__ bias, long long C, long long Cpad, fl
   if (i < Cpad) cbias2[i] = (bias && i < C) ? bias[i] * SX_LOG2E : 0.f;
 }
 
-extern "C" size_t tfrs_inbatch_softmax_tc_ex_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask) {
+extern "C" size_t tfrs_inbatch_softmax_tc_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask) {
   SxPlan pl;
   return sx_plan(B, C, d, pl, has_ids != 0, has_mask != 0) ? pl.total : 0;
 }
 
-extern "C" int tfrs_inbatch_softmax_tc_fwd_ex(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                              const float* sample_weight, const float* candidate_bias,
-                                              const int64_t* candidate_ids, const uint8_t* score_mask, float* loss, float* lse,
-                                              void* ws, size_t ws_bytes, void* stream) {
+extern "C" int tfrs_inbatch_softmax_tc_fwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
+                                           const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
+                                           const uint8_t* score_mask, float* loss, float* lse, void* ws, size_t ws_bytes,
+                                           void* stream) {
   TFRS_CHECK_ARG(q && c && loss && lse, "inbatch_softmax_tc_fwd: NULL pointer");
   SxPlan pl;
   const bool ext = candidate_ids || score_mask;
@@ -319,22 +297,10 @@ extern "C" int tfrs_inbatch_softmax_tc_fwd_ex(const float* q, const float* c, in
   float2* partial = (float2*)(w + pl.o_partial);
   float* pos = (float*)(w + pl.o_pos); float* rowloss = (float*)(w + pl.o_rowloss);
   TFRS_CUDA(cudaMemsetAsync(w, 0, 2048, st));  // both stats blocks
-  cx_amax_kernel<<<cx_amax_grid(B), 256, 0, st>>>(q, B, d, d, qst);
-  TFRS_LAUNCH_CHECK();
-  cx_amax_kernel<<<cx_amax_grid(C), 256, 0, st>>>(c, C, d, d, cst);
-  TFRS_LAUNCH_CHECK();
-  cx_exp_kernel<<<1, 1, 0, st>>>(qst);
-  TFRS_LAUNCH_CHECK();
-  cx_exp_kernel<<<1, 1, 0, st>>>(cst);
-  TFRS_LAUNCH_CHECK();
-  {
-    long long chunks = pl.Bp / 128 * 128 * (long long)pl.kb * 8;
-    cx_split_image_kernel<<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(q, B, d, d, pl.kb, pl.Bp / 128, qst, qimg);
-    TFRS_LAUNCH_CHECK();
-    chunks = pl.n_ctiles * 128 * (long long)pl.kb * 8;
-    cx_split_image_kernel<<<(unsigned)ceil_div(chunks, 256), 256, 0, st>>>(c, C, d, d, pl.kb, pl.n_ctiles, cst, cimg);
-    TFRS_LAUNCH_CHECK();
-  }
+  int rc = split_image(q, d, false, nullptr, B, d, pl.kb, pl.Bp / 128, qst, qimg, st);
+  if (rc) return rc;
+  rc = split_image(c, d, false, nullptr, C, d, pl.kb, pl.n_ctiles, cst, cimg, st);
+  if (rc) return rc;
   SoftmaxTcParams p{};
   p.qimg = qimg; p.cimg = cimg; p.qst = qst; p.cst = cst; p.B = B; p.C = C; p.nqb = pl.nqb; p.parts = pl.parts; p.kb = pl.kb;
   p.n_ctiles = pl.n_ctiles; p.inv_t = inv_temperature; p.partial = partial; p.pos = pos;
@@ -378,14 +344,5 @@ extern "C" int tfrs_inbatch_softmax_tc_fwd_ex(const float* q, const float* c, in
   TFRS_LAUNCH_CHECK();
   smtc_combine_kernel<<<(unsigned)ceil_div(B, 256), 256, 0, st>>>(partial, pl.parts * 2, pos, sample_weight, B, lse, rowloss);
   TFRS_LAUNCH_CHECK();
-  smtc_reduce_loss<<<1, 1024, 0, st>>>(rowloss, B, loss);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
-}
-
-extern "C" int tfrs_inbatch_softmax_tc_fwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                           const float* sample_weight, const float* candidate_bias, float* loss, float* lse,
-                                           void* ws, size_t ws_bytes, void* stream) {
-  return tfrs_inbatch_softmax_tc_fwd_ex(q, c, B, C, d, inv_temperature, sample_weight, candidate_bias, nullptr, nullptr, loss, lse,
-                                        ws, ws_bytes, stream);
+  return reduce_loss(rowloss, B, 1, loss, st);
 }

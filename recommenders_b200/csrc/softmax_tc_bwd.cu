@@ -247,37 +247,15 @@ sb_prep_kernel(const float* __restrict__ lse, const float* __restrict__ w, long 
   lse_pad[i] = i < B ? lse[i] : 0.f;
   w_pad[i] = i < B ? ldexpf(w ? w[i] : 1.0f, wst->exp) : 0.f;
 }
-// out[e] = sum_z partial[z][e], z ascending (deterministic)
-__global__ void __launch_bounds__(256)
-sb_reduce_parts_kernel(const float* __restrict__ partial, long long elems, int parts, float* __restrict__ out) {
-  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (e >= elems) return;
-  float a = partial[e];
-  for (int z = 1; z < parts; ++z) a += partial[(long long)z * elems + e];
-  out[e] = a;
-}
-
-// streaming-range splits per stationary block: minimise waves x (tiles per CTA + fixed cost of ~6 tile times:
-// X load, pipeline fill/drain, dX epilogue, partial reduction)
-static int sb_parts(long long n_xb, long long n_ytiles) {
-  int parts = 1; double best = 1e30;
-  const int sms = sm_count();
-  for (int c = 1; c <= 16 && c <= n_ytiles; ++c) {
-    const double cost = (double)ceil_div(n_xb * c, sms) * ((double)ceil_div(n_ytiles, c) + 6.0);
-    if (cost < best * 0.97) { best = cost; parts = c; }
-  }
-  return parts;
-}
-
 struct SbPlan {
   long long q_tiles, c_tiles; int parts_q, parts_c;
   size_t o_qst, o_cst, o_wst, o_qimg, o_cimg, o_lse, o_w, o_bias, o_partial, o_idlo, o_idhi, o_mbits, o_mbits_t, total;
 };
-static bool sb_plan(long long B, long long C, int d, SbPlan& pl, bool has_ids = false, bool has_mask = false) {
+static bool sb_plan(long long B, long long C, int d, SbPlan& pl, bool has_ids, bool has_mask) {
   if (B <= 0 || C < B || d <= 0 || d > 64) return false;
   pl.q_tiles = ceil_div(B, 128); pl.c_tiles = ceil_div(C, 128);
-  pl.parts_q = sb_parts(pl.q_tiles, pl.c_tiles);   // dq: X = q blocks, Y = c tiles
-  pl.parts_c = sb_parts(pl.c_tiles, pl.q_tiles);   // dc: X = c blocks, Y = q tiles
+  pl.parts_q = stream_parts(pl.q_tiles, pl.c_tiles);   // dq: X = q blocks, Y = c tiles
+  pl.parts_c = stream_parts(pl.c_tiles, pl.q_tiles);   // dc: X = c blocks, Y = q tiles
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += align_up(bytes, 1024); return r; };
   pl.o_qst = take(sizeof(CxStats)); pl.o_cst = take(sizeof(CxStats)); pl.o_wst = take(sizeof(CxStats));
@@ -301,26 +279,21 @@ static bool sb_plan(long long B, long long C, int d, SbPlan& pl, bool has_ids = 
 using namespace tfrs;
 using namespace tfrs::tc;
 
-extern "C" size_t tfrs_inbatch_softmax_tc_bwd_workspace_bytes(int64_t B, int64_t C, int d) {
-  SbPlan pl;
-  return sb_plan(B, C, d, pl) ? pl.total : 0;
-}
-
 // pad[i] = src[i] for i < n, 0 on the padding
 __global__ void __launch_bounds__(256) sb_pad_kernel(const float* __restrict__ src, long long n, long long npad, float* __restrict__ pad) {
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   if (i < npad) pad[i] = i < n ? src[i] : 0.f;
 }
 
-extern "C" size_t tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask) {
+extern "C" size_t tfrs_inbatch_softmax_tc_bwd_workspace_bytes(int64_t B, int64_t C, int d, int has_ids, int has_mask) {
   SbPlan pl;
   return sb_plan(B, C, d, pl, has_ids != 0, has_mask != 0) ? pl.total : 0;
 }
 
-extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                              const float* sample_weight, const float* candidate_bias,
-                                              const int64_t* candidate_ids, const uint8_t* score_mask, const float* lse,
-                                              const float* grad_loss, float* dq, float* dc, void* ws, size_t ws_bytes, void* stream) {
+extern "C" int tfrs_inbatch_softmax_tc_bwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
+                                           const float* sample_weight, const float* candidate_bias, const int64_t* candidate_ids,
+                                           const uint8_t* score_mask, const float* lse, const float* grad_loss, float* dq, float* dc,
+                                           void* ws, size_t ws_bytes, void* stream) {
   TFRS_CHECK_ARG(q && c && lse && dq && dc, "inbatch_softmax_tc_bwd: NULL pointer");
   SbPlan pl;
   const bool ext = candidate_ids || score_mask;
@@ -333,18 +306,10 @@ extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, in
   unsigned char* qimg = w8 + pl.o_qimg; unsigned char* cimg = w8 + pl.o_cimg;
   float* lse_pad = (float*)(w8 + pl.o_lse); float* w_pad = (float*)(w8 + pl.o_w); float* partial = (float*)(w8 + pl.o_partial);
   TFRS_CUDA(cudaMemsetAsync(w8, 0, 3072, st));
-  cx_amax_kernel<<<cx_amax_grid(B), 256, 0, st>>>(q, B, d, d, qst);
-  TFRS_LAUNCH_CHECK();
-  cx_amax_kernel<<<cx_amax_grid(C), 256, 0, st>>>(c, C, d, d, cst);
-  TFRS_LAUNCH_CHECK();
-  cx_exp_kernel<<<1, 1, 0, st>>>(qst);
-  TFRS_LAUNCH_CHECK();
-  cx_exp_kernel<<<1, 1, 0, st>>>(cst);
-  TFRS_LAUNCH_CHECK();
-  cx_split_image_kernel<<<(unsigned)ceil_div(pl.q_tiles * 128 * 8, 256), 256, 0, st>>>(q, B, d, d, 1, pl.q_tiles, qst, qimg);
-  TFRS_LAUNCH_CHECK();
-  cx_split_image_kernel<<<(unsigned)ceil_div(pl.c_tiles * 128 * 8, 256), 256, 0, st>>>(c, C, d, d, 1, pl.c_tiles, cst, cimg);
-  TFRS_LAUNCH_CHECK();
+  int rc = split_image(q, d, false, nullptr, B, d, 1, pl.q_tiles, qst, qimg, st);
+  if (rc) return rc;
+  rc = split_image(c, d, false, nullptr, C, d, 1, pl.c_tiles, cst, cimg, st);
+  if (rc) return rc;
   sb_wstats_kernel<<<1, 1024, 0, st>>>(sample_weight, B, wst);
   TFRS_LAUNCH_CHECK();
   sb_prep_kernel<<<(unsigned)ceil_div(pl.q_tiles * 128, 256), 256, 0, st>>>(lse, sample_weight, B, pl.q_tiles * 128, wst, lse_pad, w_pad);
@@ -393,8 +358,8 @@ extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, in
   }
   TFRS_LAUNCH_CHECK();
   if (pl.parts_q > 1) {
-    sb_reduce_parts_kernel<<<(unsigned)ceil_div(B * d, 256), 256, 0, st>>>(partial, B * (long long)d, pl.parts_q, dq);
-    TFRS_LAUNCH_CHECK();
+    rc = reduce_parts(partial, B, d, pl.parts_q, dq, d, st);
+    if (rc) return rc;
   }
   // ---- dc: X = c, Y = q (only the B query rows exist; candidates beyond B are pure negatives)
   p.ximg = cimg; p.yimg = qimg; p.xst = cst; p.yst = qst; p.n_x_rows = C; p.n_y_valid = B; p.n_ytiles = pl.q_tiles; p.n_xb = (int)pl.c_tiles;
@@ -407,16 +372,5 @@ extern "C" int tfrs_inbatch_softmax_tc_bwd_ex(const float* q, const float* c, in
     else softmax_tc_bwd_kernel<true, 0><<<g, SB_THREADS, smem, st>>>(p);
   }
   TFRS_LAUNCH_CHECK();
-  if (pl.parts_c > 1) {
-    sb_reduce_parts_kernel<<<(unsigned)ceil_div(C * d, 256), 256, 0, st>>>(partial, C * (long long)d, pl.parts_c, dc);
-    TFRS_LAUNCH_CHECK();
-  }
-  return TFRS_OK;
-}
-
-extern "C" int tfrs_inbatch_softmax_tc_bwd(const float* q, const float* c, int64_t B, int64_t C, int d, float inv_temperature,
-                                           const float* sample_weight, const float* candidate_bias, const float* lse,
-                                           const float* grad_loss, float* dq, float* dc, void* ws, size_t ws_bytes, void* stream) {
-  return tfrs_inbatch_softmax_tc_bwd_ex(q, c, B, C, d, inv_temperature, sample_weight, candidate_bias, nullptr, nullptr, lse, grad_loss,
-                                        dq, dc, ws, ws_bytes, stream);
+  return pl.parts_c > 1 ? reduce_parts(partial, C, d, pl.parts_c, dc, d, st) : TFRS_OK;
 }

@@ -157,45 +157,6 @@ split_gemm_kernel(const SgParams p) {
   }
 }
 
-// fp32 src [K, M] (row stride ld)  ->  hi/lo fp16 image of src^T: image rows = columns m of src, reduction index = rows
-// k of src.  One CTA per (64-row K slab, 128-column tile): coalesced 512-byte row reads, transpose through shared
-// memory, 128-byte swizzled row writes.
-__global__ void __launch_bounds__(256)
-cx_split_image_t_kernel(const float* __restrict__ src, long long K, int M, long long ld, int kb_total,
-                        const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
-  __shared__ float tile[64][129];
-  const int ks = blockIdx.x, mt = blockIdx.y;
-  // v * 2^exp as two exact power-of-two factors: 2^exp alone overflows when exp > 127 (max |element| < 2^-113), and exp >= -114
-  // keeps 2^exp normal, so this equals ldexpf(v, exp) -- at the price of a multiply, where ldexpf per element slows the load loop
-  const int e1 = min(st->exp, 127);
-  const float sc1 = ldexpf(1.0f, e1), sc2 = ldexpf(1.0f, st->exp - e1);
-#pragma unroll 8
-  for (int e = threadIdx.x; e < 64 * 128; e += 256) {
-    const int kk = e >> 7, mm = e & 127;
-    const long long k = (long long)ks * 64 + kk; const int m = mt * 128 + mm;
-    const float f = (k < K && m < M) ? __ldg(src + k * ld + m) : 0.f;
-    tile[kk][mm] = f * sc1 * sc2;
-  }
-  __syncthreads();
-  unsigned char* base = img + ((long long)mt * kb_total + ks) * 32768;
-#pragma unroll
-  for (int pass = 0; pass < 4; ++pass) {
-    const int r = pass * 32 + (threadIdx.x >> 3), cj = threadIdx.x & 7;
-    __align__(16) __half hi[8];
-    __align__(16) __half lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float v = tile[cj * 8 + j][r];
-      const __half h = __float2half_rn(v);
-      hi[j] = h;
-      lo[j] = __float2half_rn(v - __half2float(h));
-    }
-    unsigned char* dst = base + r * 128 + ((cj ^ (r & 7)) * 16);
-    *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(dst + 16384) = *reinterpret_cast<const uint4*>(lo);
-  }
-}
-
 static int sg_launch(int mode, const SgParams& p, cudaStream_t st) {
   const size_t smem = (size_t)SG_STAGES * SG_STAGE_BYTES + 1024 + 256;
   TFRS_DYN_SMEM(split_gemm_kernel<SG_DX>, (int)smem);
@@ -238,17 +199,7 @@ size_t gemm_tc_workspace(long long M, long long N, long long K, int mode) {
   return pl.total;
 }
 
-// out[m*ld + n] = sum_z partial[z][m][n]  (z ascending: deterministic)
-__global__ void __launch_bounds__(256)
-sg_reduce_chunks_strided_kernel(const float* __restrict__ partial, long long M, long long N, int chunks, float* __restrict__ out, long long ld) {
-  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (e >= M * N) return;
-  float a = partial[e];
-  for (int z = 1; z < chunks; ++z) a += partial[(long long)z * M * N + e];
-  out[(e / N) * ld + (e % N)] = a;
-}
-
-// The same fixed-order sum, then the Dense epilogue: y = act(sum + bias[n]); logits (nullable) = sum + bias[n]
+// The fixed-order sum of the chunk partials (as reduce_parts), then the Dense epilogue: y = act(sum + bias[n]); logits (nullable) = sum + bias[n]
 __global__ void __launch_bounds__(256)
 sg_reduce_chunks_dense_kernel(const float* __restrict__ partial, long long M, long long N, int chunks, const float* __restrict__ bias,
                               int act, float* __restrict__ out, float* __restrict__ logits, long long ld) {
@@ -262,26 +213,6 @@ sg_reduce_chunks_dense_kernel(const float* __restrict__ partial, long long M, lo
   out[o] = dense_act(act, zv);
 }
 
-static int gt_image(const GemmOperand& op, long long rows, long long K, int kb, long long n_tiles128, CxStats* st_, unsigned char* img,
-                    cudaStream_t st) {
-  // max |element|: given by the caller, or a pass over the operand's memory, [rows, K] (ld) or, transposed, [K, rows] (ld)
-  if (op.amax_bits) TFRS_CUDA(cudaMemcpyAsync(&st_->amax_bits, op.amax_bits, sizeof(unsigned int), cudaMemcpyDeviceToDevice, st));
-  else if (op.transposed) cx_amax_kernel<<<cx_amax_grid(K), 256, 0, st>>>(op.ptr, K, (int)rows, op.ld, st_);
-  else cx_amax_kernel<<<cx_amax_grid(rows), 256, 0, st>>>(op.ptr, rows, (int)K, op.ld, st_);
-  TFRS_LAUNCH_CHECK();
-  cx_exp_kernel<<<1, 1, 0, st>>>(st_);
-  TFRS_LAUNCH_CHECK();
-  if (op.transposed) {   // tiled shared-memory transpose: coalesced on both sides
-    cx_split_image_t_kernel<<<dim3((unsigned)kb, (unsigned)n_tiles128), 256, 0, st>>>(op.ptr, K, (int)rows, op.ld, kb, st_, img);
-  } else {
-    const long long chunks = n_tiles128 * 128 * (long long)kb * 8;
-    const unsigned g = (unsigned)(ceil_div(chunks, 256) < (1 << 20) ? ceil_div(chunks, 256) : (1 << 20));
-    cx_split_image_kernel<<<g, 256, 0, st>>>(op.ptr, rows, (int)K, op.ld, kb, n_tiles128, st_, img);
-  }
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
-}
-
 int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long N, long long K, const GemmEpilogue& ep,
             float* out, long long ld_out, void* ws, size_t ws_bytes, cudaStream_t st) {
   GtPlan pl; gt_plan(M, N, K, ep.mode, pl);
@@ -292,9 +223,9 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
   unsigned char* w8 = (unsigned char*)ws;
   CxStats* ast = (CxStats*)(w8 + pl.o_st); CxStats* bst = (CxStats*)(w8 + pl.o_st + 1024);
   TFRS_CUDA(cudaMemsetAsync(w8 + pl.o_st, 0, 2048, st));
-  int rc = gt_image(A, M, K, pl.kb, (long long)pl.n_mb * 2, ast, w8 + pl.o_aimg, st);
+  int rc = split_image(A.ptr, A.ld, A.transposed, A.amax_bits, M, K, pl.kb, (long long)pl.n_mb * 2, ast, w8 + pl.o_aimg, st);
   if (rc) return rc;
-  rc = gt_image(Bop, N, K, pl.kb, pl.n_nt, bst, w8 + pl.o_bimg, st);
+  rc = split_image(Bop.ptr, Bop.ld, Bop.transposed, Bop.amax_bits, N, K, pl.kb, pl.n_nt, bst, w8 + pl.o_bimg, st);
   if (rc) return rc;
   SgParams p{};
   p.aimg = w8 + pl.o_aimg; p.bimg = w8 + pl.o_bimg; p.ast = ast; p.bst = bst;
@@ -304,11 +235,10 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
     p.out = (float*)(w8 + pl.o_partial); p.ld_out = N;
     rc = sg_launch(SG_DW, p, st);
     if (rc) return rc;
-    if (ep.mode == GEMM_EPI_DENSE)   // bias + activation applied to the reduced sum
-      sg_reduce_chunks_dense_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.bias, ep.act, out, ep.prod,
-                                                                                     ld_out);
-    else
-      sg_reduce_chunks_strided_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, out, ld_out);
+    if (ep.mode != GEMM_EPI_DENSE) return reduce_parts(p.out, M, N, pl.n_kc, out, ld_out, st);
+    // bias + activation applied to the reduced sum
+    sg_reduce_chunks_dense_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.bias, ep.act, out, ep.prod,
+                                                                                   ld_out);
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }

@@ -378,18 +378,22 @@ SOFTMAX_TC_MIN_B = 512  # below this the exact CUDA-core forward is launch-laten
 
 
 def inbatch_softmax_tc(q: torch.Tensor, c: torch.Tensor, sample_weight: Optional[torch.Tensor] = None,
-                       inv_temperature: float = 1.0, candidate_bias: Optional[torch.Tensor] = None):
+                       inv_temperature: float = 1.0, candidate_bias: Optional[torch.Tensor] = None,
+                       candidate_ids: Optional[torch.Tensor] = None, score_mask: Optional[torch.Tensor] = None):
   """Tensor-core forward only (any B): returns (loss scalar, lse [B]).  Raises NotImplementedError when d > 128.
-  `candidate_bias` [C] is added to every logit of its column (after the temperature)."""
+  `candidate_bias` [C] is added to every logit of its column (after the temperature); `candidate_ids` (int64 [C]) removes
+  accidental hits and `score_mask` (uint8 [B, C], nonzero = keep) masks logits, as in inbatch_softmax_loss."""
   q = f32c(q, "query_embeddings"); c = f32c(c, "candidate_embeddings")
   B, d = q.shape; C = c.shape[0]
   w = None if sample_weight is None else f32c(sample_weight, "sample_weight").view(-1)
   loss = torch.empty((1,), dtype=torch.float32, device=q.device)
   lse = torch.empty((B,), dtype=torch.float32, device=q.device)
   cb = None if candidate_bias is None else f32c(candidate_bias, "candidate_bias").view(-1)
-  ws = workspace(max(lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d), 256), q.device, "softmax_tc")
-  check(lib().tfrs_inbatch_softmax_tc_fwd(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(cb), ptr(loss), ptr(lse),
-                                          ptr(ws), ws.numel(), stream()), "inbatch_softmax_tc_fwd")
+  wsb = lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d, int(candidate_ids is not None), int(score_mask is not None))
+  ws = workspace(wsb, q.device, "softmax_tc")
+  check(lib().tfrs_inbatch_softmax_tc_fwd(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(cb), ptr(candidate_ids),
+                                          ptr(score_mask), ptr(loss), ptr(lse), ptr(ws), ws.numel(), stream()),
+        "inbatch_softmax_tc_fwd")
   return loss.view(()), lse
 
 
@@ -431,15 +435,13 @@ class _InBatchSoftmax(torch.autograd.Function):
     if (cb is not None or ext) and not inbatch_softmax_bias_supported(B, C, d):
       raise NotImplementedError("inbatch_softmax_loss: candidate_bias / candidate_ids / score_mask need the tensor-core path "
                                 f"(B >= {SOFTMAX_TC_MIN_B}, d <= 64); got B={B}, d={d}")
-    loss = torch.empty((1,), dtype=torch.float32, device=q.device)
-    lse = torch.empty((B,), dtype=torch.float32, device=q.device)
-    tcb = lib().tfrs_inbatch_softmax_tc_ex_workspace_bytes(B, C, d, int(ids is not None), int(mask is not None)) \
-        if B >= SOFTMAX_TC_MIN_B else 0
-    if tcb:  # tensor-core forward (hi/lo fp16 split, fp32 accumulate, online log-sum-exp epilogue)
-      ws = workspace(tcb, q.device, "softmax_tc")
-      check(lib().tfrs_inbatch_softmax_tc_fwd_ex(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(cb), ptr(ids), ptr(mask),
-                                                 ptr(loss), ptr(lse), ptr(ws), ws.numel(), stream()), "inbatch_softmax_tc_fwd")
+    used_tc = B >= SOFTMAX_TC_MIN_B and \
+        lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d, int(ids is not None), int(mask is not None)) > 0
+    if used_tc:  # tensor-core forward (hi/lo fp16 split, fp32 accumulate, online log-sum-exp epilogue)
+      loss, lse = inbatch_softmax_tc(q, c, w, inv_temperature, cb, ids, mask)
     else:
+      loss = torch.empty((1,), dtype=torch.float32, device=q.device)
+      lse = torch.empty((B,), dtype=torch.float32, device=q.device)
       wsb = lib().tfrs_inbatch_softmax_workspace_bytes(B, C, d)
       ws = workspace(wsb, q.device, "softmax")
       check(lib().tfrs_inbatch_softmax_fwd(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(loss), ptr(lse),
@@ -452,7 +454,7 @@ class _InBatchSoftmax(torch.autograd.Function):
     ctx.has_ids = ids is not None
     ctx.has_mask = mask is not None
     ctx.inv_t = inv_temperature
-    ctx.used_tc = bool(tcb)
+    ctx.used_tc = used_tc
     return loss.view(())
 
   @staticmethod
@@ -460,17 +462,14 @@ class _InBatchSoftmax(torch.autograd.Function):
     q, c, lse, w, cb, ids, mask = ctx.saved_tensors
     B, d = q.shape; C = c.shape[0]
     g = f32c(g, "grad").view(1)
-    dq = torch.empty_like(q); dc = torch.empty_like(c)
-    tcb = lib().tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes(B, C, d, int(ctx.has_ids), int(ctx.has_mask)) if ctx.used_tc else 0
-    if tcb:  # tensor-core backward: same split products as the forward pass that produced `lse`
-      ws = workspace(tcb, q.device, "softmax_tc_bwd")
-      check(lib().tfrs_inbatch_softmax_tc_bwd_ex(ptr(q), ptr(c), B, C, d, c_f(ctx.inv_t), ptr(w) if ctx.has_w else None,
-                                                 ptr(cb) if ctx.has_cb else None, ptr(ids) if ctx.has_ids else None,
-                                                 ptr(mask) if ctx.has_mask else None, ptr(lse), ptr(g), ptr(dq), ptr(dc), ptr(ws),
-                                                 ws.numel(), stream()), "inbatch_softmax_tc_bwd")
+    if ctx.used_tc and lib().tfrs_inbatch_softmax_tc_bwd_workspace_bytes(B, C, d, int(ctx.has_ids), int(ctx.has_mask)):
+      # tensor-core backward: same split products as the forward pass that produced `lse`
+      dq, dc = inbatch_softmax_tc_bwd(q, c, lse, w if ctx.has_w else None, ctx.inv_t, g, cb if ctx.has_cb else None,
+                                      ids if ctx.has_ids else None, mask if ctx.has_mask else None)
       return dq, dc, None, None, None, None, None
     if ctx.has_cb or ctx.has_ids or ctx.has_mask:
       raise NotImplementedError("inbatch_softmax_loss backward with loss options needs the tensor-core path")
+    dq = torch.empty_like(q); dc = torch.empty_like(c)
     wsb = lib().tfrs_inbatch_softmax_workspace_bytes(B, C, d)
     ws = workspace(wsb, q.device, "softmax")
     check(lib().tfrs_inbatch_softmax_bwd(ptr(q), ptr(c), B, C, d, c_f(ctx.inv_t), ptr(w) if ctx.has_w else None,
@@ -492,24 +491,27 @@ def inbatch_softmax_bwd_exact(q, c, lse, sample_weight=None, inv_temperature: fl
   return dq, dc
 
 
-def inbatch_softmax_tc_bwd(q, c, lse, sample_weight=None, inv_temperature: float = 1.0, grad_loss=None, candidate_bias=None):
-  """Tensor-core backward only (any B, d <= 64): returns (dq, dc) for the given saved `lse`."""
+def inbatch_softmax_tc_bwd(q, c, lse, sample_weight=None, inv_temperature: float = 1.0, grad_loss=None, candidate_bias=None,
+                           candidate_ids: Optional[torch.Tensor] = None, score_mask: Optional[torch.Tensor] = None):
+  """Tensor-core backward only (any B, d <= 64): returns (dq, dc) for the given saved `lse`; options as inbatch_softmax_tc."""
   q = f32c(q, "query_embeddings"); c = f32c(c, "candidate_embeddings"); lse = f32c(lse, "lse")
   B, d = q.shape; C = c.shape[0]
   w = None if sample_weight is None else f32c(sample_weight, "sample_weight").view(-1)
   g = None if grad_loss is None else f32c(grad_loss, "grad").view(1)
   dq = torch.empty_like(q); dc = torch.empty_like(c)
-  ws = workspace(max(lib().tfrs_inbatch_softmax_tc_bwd_workspace_bytes(B, C, d), 256), q.device, "softmax_tc_bwd")
+  wsb = lib().tfrs_inbatch_softmax_tc_bwd_workspace_bytes(B, C, d, int(candidate_ids is not None), int(score_mask is not None))
+  ws = workspace(wsb, q.device, "softmax_tc_bwd")
   cb = None if candidate_bias is None else f32c(candidate_bias, "candidate_bias").view(-1)
-  check(lib().tfrs_inbatch_softmax_tc_bwd(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(cb), ptr(lse), ptr(g),
-                                          ptr(dq), ptr(dc), ptr(ws), ws.numel(), stream()), "inbatch_softmax_tc_bwd")
+  check(lib().tfrs_inbatch_softmax_tc_bwd(ptr(q), ptr(c), B, C, d, c_f(inv_temperature), ptr(w), ptr(cb), ptr(candidate_ids),
+                                          ptr(score_mask), ptr(lse), ptr(g), ptr(dq), ptr(dc), ptr(ws), ws.numel(), stream()),
+        "inbatch_softmax_tc_bwd")
   return dq, dc
 
 
 def inbatch_softmax_bias_supported(B: int, C: int, d: int) -> bool:
   """True when the loss with a per-candidate logit bias can run fused (tensor-core forward AND backward)."""
-  return (B >= SOFTMAX_TC_MIN_B and lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d) > 0 and
-          lib().tfrs_inbatch_softmax_tc_bwd_workspace_bytes(B, C, d) > 0)
+  return (B >= SOFTMAX_TC_MIN_B and lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d, 0, 0) > 0 and
+          lib().tfrs_inbatch_softmax_tc_bwd_workspace_bytes(B, C, d, 0, 0) > 0)
 
 
 def inbatch_softmax_loss(q: torch.Tensor, c: torch.Tensor, sample_weight: Optional[torch.Tensor] = None,

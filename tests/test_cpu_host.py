@@ -20,7 +20,7 @@ def _declared_symbols():
   return sorted(set(re.findall(r"\b(tfrs_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_builds_and_exports_every_declared_symbol():
+def test_library_builds_and_exports_exactly_the_declared_symbols():
   from recommenders_b200 import build, _ffi
   path = build.build()
   assert os.path.exists(path)
@@ -30,9 +30,12 @@ def test_library_builds_and_exports_every_declared_symbol():
   for name in declared:
     assert hasattr(lib, name), f"{name} declared in include/tfrs_b200.h but not exported"
   assert set(declared) == set(_ffi.EXPORTS), set(declared) ^ set(_ffi.EXPORTS)
+  for gone in ("tfrs_inbatch_softmax_tc_ex_workspace_bytes", "tfrs_inbatch_softmax_tc_fwd_ex",
+               "tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes", "tfrs_inbatch_softmax_tc_bwd_ex"):
+    assert not hasattr(lib, gone), f"{gone} is still exported"
   # no-compute calls are safe without a GPU
   l = _ffi.lib()
-  assert l.tfrs_version() == 101
+  assert l.tfrs_version() == 102
   assert l.tfrs_topk_scan_workspace_bytes(4096, 1000000, 64, 100) > 0
   assert l.tfrs_launch_count() == 0
 
@@ -177,7 +180,7 @@ def test_sharded_protocol_gloo(tmp_path, world):
     assert p.returncode == 0 and f"RANK_OK {r}" in o, o
 
 
-def test_host_side_planning_functions():
+def test_host_side_planning_functions_with_option_flags():
   """The *_workspace_bytes / out_dim entry points are pure host code: they run without a GPU and define which shapes
   take the tensor-core paths (0 = outside the range, the callers then use the exact kernels)."""
   from recommenders_b200 import _ffi
@@ -188,12 +191,12 @@ def test_host_side_planning_functions():
     assert lib.tfrs_dot_interaction_out_dim(F, 1, 0) == F * (F + 1) // 2
     assert lib.tfrs_dot_interaction_out_dim(F, 0, 1) == F * F and lib.tfrs_dot_interaction_out_dim(F, 1, 1) == F * F
   # in-batch softmax on tensor cores: forward d <= 128, backward d <= 64, C >= B
-  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 64) > 0
-  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 128) > 0
-  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 129) == 0
-  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(1024, 512, 64) == 0
-  assert lib.tfrs_inbatch_softmax_tc_bwd_workspace_bytes(16384, 16384, 64) > 0
-  assert lib.tfrs_inbatch_softmax_tc_bwd_workspace_bytes(16384, 16384, 65) == 0
+  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 64, 0, 0) > 0
+  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 128, 0, 0) > 0
+  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(16384, 16384, 129, 0, 0) == 0
+  assert lib.tfrs_inbatch_softmax_tc_workspace_bytes(1024, 512, 64, 0, 0) == 0
+  assert lib.tfrs_inbatch_softmax_tc_bwd_workspace_bytes(16384, 16384, 64, 0, 0) > 0
+  assert lib.tfrs_inbatch_softmax_tc_bwd_workspace_bytes(16384, 16384, 65, 0, 0) == 0
   # top-K screening path: k <= 256, d <= 128, corpus large enough
   assert lib.tfrs_topk_tc_workspace_bytes(4096, 1_000_000, 64, 100) > 0
   assert lib.tfrs_topk_tc_workspace_bytes(4096, 1_000_000, 64, 257) == 0
