@@ -300,6 +300,33 @@ int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows, int d, con
                             void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K7  ClippyAdagrad (experimental/optimizers/clippy_adagrad.py:81-249): Adagrad with one clipping factor per variable.
+ * Per touched element, with g the gradient (duplicate ids summed in order of occurrence, as K4), v the variable and
+ * a the accumulator, every step one IEEE fp32 operation:
+ *   a1 = standard ? a + g*g : a ;  p = 1 / sqrt(a1 + eps) ;  delta = (lr*g) * p
+ *   m  = (abs_thr + |v|*var_rel) + p*acc_rel ;  s = delta == 0 ? 1 : m / |delta|
+ *   scale = min(1, min over the variable's touched elements of s)     (NaN ratios are ignored, as fminf)
+ *   v' = v - delta*scale ;  a' = standard ? a1 : a + u*u,  u = clip ? g*scale : g
+ * flags: bit 0 clip_accumulator_update (clip), bit 1 use_standard_accumulator_update (standard); not both.  Thresholds
+ * must be >= 0.  The factor (1 when nothing is touched) is written to the device scalar clipping_factor_out, or kept in
+ * `ws` when it is NULL.  Deterministic (atomicMin on the factor's bit pattern, no float atomics on the state).
+ * Sparse: one table per call, the contract of tfrs_sparse_adagrad_f32 (I32/I64 ids, out-of-range ids skipped,
+ * n < 2^24, d <= 1024).
+ * Dense: every variable of one optimizer in one call; vars / grads / accums / numels are HOST arrays of nvars device
+ * pointers and element counts, clipping_factors_out a device array of nvars floats (or NULL: kept in `ws`).
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_sparse_clippy_adagrad_workspace_bytes(int64_t n, int d);
+int tfrs_sparse_clippy_adagrad_f32(float* table, float* accum, int64_t rows, int d, const void* ids, int ids_dtype,
+                                   int64_t n, const float* grad_rows, float lr, float eps, float var_rel, float acc_rel,
+                                   float abs_thr, int flags, float* clipping_factor_out, void* ws, size_t ws_bytes,
+                                   void* stream);
+size_t tfrs_clippy_adagrad_dense_workspace_bytes(int nvars);
+int tfrs_clippy_adagrad_dense_f32(float* const* vars, const float* const* grads, float* const* accums,
+                                  const int64_t* numels, int nvars, float lr, float eps, float var_rel, float acc_rel,
+                                  float abs_thr, int flags, float* clipping_factors_out, void* ws, size_t ws_bytes,
+                                  void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K5  DCN-v2 cross layer (layers/feature_interaction/dcn.py:176-186, full-rank, no preactivation):
  *   out = x0 * (x . W + bias + diag_scale * x) + x ,  W [D,D] in Keras [in,out] layout.
  * x0, x, out have row stride ld (>= D).  `prod` (nullable) receives x.W + bias + diag_scale*x for

@@ -76,7 +76,12 @@ _SIGNATURES = {
     "tfrs_hardneg_loss_bwd": (c_i, [c_p, c_p, c_l, c_l, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_p]),
     "tfrs_sparse_adagrad_workspace_bytes": (c_sz, [c_l, c_i]),
     "tfrs_sparse_adagrad_f32": (c_i, [c_p, c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_f, c_i, c_p, c_sz, c_p]),
-    "tfrs_cross_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p]),
+    "tfrs_sparse_clippy_adagrad_workspace_bytes": (c_sz, [c_l, c_i]),
+    "tfrs_sparse_clippy_adagrad_f32": (c_i, [c_p, c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_f, c_f, c_f, c_f, c_i, c_p, c_p, c_sz,
+                                             c_p]),
+    "tfrs_clippy_adagrad_dense_workspace_bytes": (c_sz, [c_i]),
+    "tfrs_clippy_adagrad_dense_f32": (c_i, [c_p, c_p, c_p, c_p, c_i, c_f, c_f, c_f, c_f, c_f, c_i, c_p, c_p, c_sz, c_p]),
+    "tfrs_cross_fwd_f32":(c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p]),
     "tfrs_cross_tc_workspace_bytes": (c_sz, [c_l, c_i]),
     "tfrs_cross_tc_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_cross_bwd_workspace_bytes": (c_sz, [c_l, c_i]),

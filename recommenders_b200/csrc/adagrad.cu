@@ -7,14 +7,13 @@
 //      legacy sqrt(acc)+eps form).  Every step is a single IEEE fp32 op (no FMA contraction) so the
 //      result is bit-identical to oracle/tfrs_oracle.c::orc_sparse_adagrad.
 // HBM-bound: algorithmic bytes = unique_rows * d * 4 * 4 (table r/w + accum r/w) + n*d*4 (grads).
-#include "common.cuh"
+#include "adagrad.cuh"
 
 namespace tfrs {
 
 constexpr int AG_TILE = 8192;       // keys per CTA tile (64 KB of shared memory)
 constexpr int AG_THREADS = 1024;
 constexpr unsigned long long AG_INVALID = ~0ull;
-constexpr unsigned long long AG_BAD_ID = 0xFFFFFFFFFFull;   // out-of-range ids sort last and are skipped by ag_apply
 
 template <typename IdT>
 __device__ __forceinline__ unsigned long long ag_key(const IdT* __restrict__ ids, long long j, long long rows) {
@@ -157,7 +156,6 @@ __global__ void ag_bitonic_global(unsigned long long* __restrict__ keys, long lo
 // occurrence -- the keys are sorted by (id, position) -- with the gradient rows of 8 members in flight per step, so a hot
 // id's chain costs one DRAM round trip per 8 members instead of two per member.  Runs longer than AG_LONG members are left
 // to ag_apply_long (a whole CTA stages their rows through shared memory).
-constexpr int AG_LONG = 64;
 __device__ __forceinline__ void ag_update(float* __restrict__ trow, float* __restrict__ arow, int c, float g, float lr, float eps, int eps_inside) {
   const float a = __fadd_rn(arow[c], __fmul_rn(g, g));
   arow[c] = a;
@@ -212,7 +210,6 @@ ag_apply(const unsigned long long* __restrict__ keys, long long n, const float* 
 // Hot ids (Zipf batches: one id can own a tenth of the batch): one CTA per long run.  All 256 threads stream the run's
 // gradient rows into a shared-memory tile (AL_ROWS rows in flight per step), then one thread per column adds the tile's
 // rows IN ORDER -- the chain is fp32 adds on shared memory, not DRAM round trips.
-constexpr int AL_THREADS = 256, AL_ROWS = 256;  // rows per tile: min(AL_ROWS, 64 KB / row bytes)
 __global__ void __launch_bounds__(AL_THREADS)
 ag_apply_long(const unsigned long long* __restrict__ keys, long long n, const float* __restrict__ grad, int d,
               float* __restrict__ table, float* __restrict__ accum, float lr, float eps, int eps_inside,
@@ -284,45 +281,20 @@ ag_apply_long(const unsigned long long* __restrict__ keys, long long n, const fl
 
 static long long ag_pow2(long long n) { long long p = 1; while (p < n) p <<= 1; return p; }
 
-}  // namespace tfrs
-using namespace tfrs;
-
-extern "C" size_t tfrs_sparse_adagrad_workspace_bytes(int64_t n, int d) {
-  (void)d;
+size_t ag_group_workspace_bytes(long long n) {
   const size_t P = (size_t)ag_pow2(n > 2 ? n : 2);
   return P * 8 /*keys*/ + P * 8 /*bucketed keys*/ + P * 4 /*ranks*/ + (P / AG_LONG + 2) * 4 /*long-run list*/ + (AB_BUCKETS + 1) * 4 + 1024;
 }
 
-extern "C" int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows, int d, const void* ids,
-                                       int ids_dtype, int64_t n, const float* grad_rows, float lr, float eps,
-                                       int eps_inside_sqrt, void* ws, size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && accum && rows > 0 && d > 0, "sparse_adagrad: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_adagrad: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_adagrad: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_adagrad: rows must be < 2^40");
-  if (n == 0) return TFRS_OK;
-  TFRS_CHECK_ARG(ids && grad_rows, "sparse_adagrad: NULL ids/grad");
-  TFRS_CHECK_ARG(d <= 1024, "sparse_adagrad: d=%d > 1024", d);
+int ag_group(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st, AgGroups* out) {
   const long long P = ag_pow2(n > 2 ? n : 2);
-  if (!ws || ws_bytes < tfrs_sparse_adagrad_workspace_bytes(n, d)) { set_error("sparse_adagrad: workspace too small"); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
-  cudaStream_t st = (cudaStream_t)stream;
   unsigned long long* keys = (unsigned long long*)ws;
   unsigned long long* bkeys = keys + P;
   unsigned int* long_count = (unsigned int*)(bkeys + P);
   unsigned int* long_list = long_count + 1;
   unsigned int* bstart = long_list + (P / AG_LONG + 1);
   unsigned int* rank = bstart + AB_BUCKETS + 1;
-  auto apply = [&]() -> int {
-    TFRS_CUDA(cudaMemsetAsync(long_count, 0, 4, st));
-    ag_apply<<<(unsigned)ceil_div(n * 32, 256), 256, 0, st>>>(keys, n, grad_rows, d, table, accum, lr, eps, eps_inside_sqrt, long_count, long_list);
-    TFRS_LAUNCH_CHECK();
-    int tile_rows = (64 * 1024) / (d * 4); if (tile_rows > AL_ROWS) tile_rows = AL_ROWS; if (tile_rows < 1) tile_rows = 1;
-    TFRS_DYN_SMEM(ag_apply_long, 64 * 1024);
-    ag_apply_long<<<(unsigned)sm_count(), AL_THREADS, (size_t)tile_rows * d * 4, st>>>(keys, n, grad_rows, d, table, accum, lr, eps, eps_inside_sqrt,
-                                                                                       long_count, long_list, tile_rows);
-    TFRS_LAUNCH_CHECK();
-    return TFRS_OK;
-  };
+  *out = AgGroups{keys, long_count, long_list};
   if (n <= AG_RANK_MAX) {
     if (ids_dtype == TFRS_I32) ag_bucket_scatter<int32_t><<<1, AB_THREADS, 0, st>>>((const int32_t*)ids, n, rows, bkeys, bstart, rank);
     else ag_bucket_scatter<int64_t><<<1, AB_THREADS, 0, st>>>((const int64_t*)ids, n, rows, bkeys, bstart, rank);
@@ -331,7 +303,7 @@ extern "C" int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows,
     TFRS_LAUNCH_CHECK();
     ag_bucket_place<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(bkeys, n, bstart, rank, keys);
     TFRS_LAUNCH_CHECK();
-    return apply();
+    return TFRS_OK;
   }
   unsigned kb = (unsigned)ceil_div(P, 256);
   if (ids_dtype == TFRS_I32) ag_build_keys<int32_t><<<kb, 256, 0, st>>>((const int32_t*)ids, n, rows, P, keys);
@@ -350,5 +322,40 @@ extern "C" int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows,
     ag_bitonic_local<<<tiles, AG_THREADS, AG_TILE * 8, st>>>(keys, P, size, size);
     TFRS_LAUNCH_CHECK();
   }
-  return apply();
+  return TFRS_OK;
+}
+
+}  // namespace tfrs
+using namespace tfrs;
+
+extern "C" size_t tfrs_sparse_adagrad_workspace_bytes(int64_t n, int d) {
+  (void)d;
+  return ag_group_workspace_bytes(n);
+}
+
+extern "C" int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows, int d, const void* ids,
+                                       int ids_dtype, int64_t n, const float* grad_rows, float lr, float eps,
+                                       int eps_inside_sqrt, void* ws, size_t ws_bytes, void* stream) {
+  TFRS_CHECK_ARG(table && accum && rows > 0 && d > 0, "sparse_adagrad: bad table");
+  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_adagrad: ids_dtype must be I32 or I64");
+  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_adagrad: n=%lld must be < 2^24", (long long)n);
+  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_adagrad: rows must be < 2^40");
+  if (n == 0) return TFRS_OK;
+  TFRS_CHECK_ARG(ids && grad_rows, "sparse_adagrad: NULL ids/grad");
+  TFRS_CHECK_ARG(d <= 1024, "sparse_adagrad: d=%d > 1024", d);
+  if (!ws || ws_bytes < tfrs_sparse_adagrad_workspace_bytes(n, d)) { set_error("sparse_adagrad: workspace too small"); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  AgGroups gr;
+  const int rc = ag_group(ids, ids_dtype, n, rows, ws, st, &gr);
+  if (rc != TFRS_OK) return rc;
+  TFRS_CUDA(cudaMemsetAsync(gr.long_count, 0, 4, st));
+  ag_apply<<<(unsigned)ceil_div(n * 32, 256), 256, 0, st>>>(gr.keys, n, grad_rows, d, table, accum, lr, eps, eps_inside_sqrt,
+                                                            gr.long_count, gr.long_list);
+  TFRS_LAUNCH_CHECK();
+  int tile_rows = (64 * 1024) / (d * 4); if (tile_rows > AL_ROWS) tile_rows = AL_ROWS; if (tile_rows < 1) tile_rows = 1;
+  TFRS_DYN_SMEM(ag_apply_long, 64 * 1024);
+  ag_apply_long<<<(unsigned)sm_count(), AL_THREADS, (size_t)tile_rows * d * 4, st>>>(gr.keys, n, grad_rows, d, table, accum, lr, eps,
+                                                                                     eps_inside_sqrt, gr.long_count, gr.long_list, tile_rows);
+  TFRS_LAUNCH_CHECK();
+  return TFRS_OK;
 }

@@ -638,6 +638,85 @@ def sparse_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.Tensor,
 
 
 # ------------------------------------------------------------------------------------------------
+# K7 ClippyAdagrad
+# ------------------------------------------------------------------------------------------------
+def _clippy_flags(clip_accumulator_update: bool, use_standard_accumulator_update: bool) -> int:
+  return (1 if clip_accumulator_update else 0) | (2 if use_standard_accumulator_update else 0)
+
+
+def _f32_inplace(t: torch.Tensor, name: str) -> torch.Tensor:
+  require_cuda(t, name)
+  if t.dtype != torch.float32 or not t.is_contiguous():
+    raise ValueError(f"{name} must be contiguous float32 (it is updated in place)")
+  return t
+
+
+def sparse_clippy_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor,
+                           lr: float, eps: float, variable_relative_threshold: float, accumulator_relative_threshold: float,
+                           absolute_threshold: float, clip_accumulator_update: bool = False,
+                           use_standard_accumulator_update: bool = False,
+                           clipping_factor: Optional[torch.Tensor] = None) -> None:
+  """ClippyAdagrad step of one embedding table on the rows `ids` (duplicates summed in order of occurrence).  The
+  variable's clipping factor is written to the 0-d float32 device tensor `clipping_factor` when given."""
+  _f32_inplace(table, "table"); _f32_inplace(accum, "accum")
+  ids = require_cuda(ids, "ids").contiguous().view(-1)
+  g = f32c(grad_rows, "grad_rows")
+  n = ids.numel(); d = table.shape[1]
+  if accum.shape != table.shape:
+    raise ValueError(f"sparse_clippy_adagrad_: accum must be {tuple(table.shape)}, got {tuple(accum.shape)}")
+  if g.shape != (n, d):
+    raise ValueError(f"sparse_clippy_adagrad_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
+  if clipping_factor is not None:
+    _f32_inplace(clipping_factor, "clipping_factor")
+    if clipping_factor.numel() != 1:
+      raise ValueError("sparse_clippy_adagrad_: clipping_factor must hold one float")
+  wsb = lib().tfrs_sparse_clippy_adagrad_workspace_bytes(n, d)
+  ws = workspace(wsb, table.device, "clippy")
+  check(lib().tfrs_sparse_clippy_adagrad_f32(
+      ptr(table), ptr(accum), table.shape[0], d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(lr), c_f(eps),
+      c_f(variable_relative_threshold), c_f(accumulator_relative_threshold), c_f(absolute_threshold),
+      _clippy_flags(clip_accumulator_update, use_standard_accumulator_update), ptr(clipping_factor), ptr(ws), ws.numel(),
+      stream()), "sparse_clippy_adagrad")
+
+
+def clippy_adagrad_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], accums: Sequence[torch.Tensor],
+                          lr: float, eps: float, variable_relative_threshold: float, accumulator_relative_threshold: float,
+                          absolute_threshold: float, clip_accumulator_update: bool = False,
+                          use_standard_accumulator_update: bool = False,
+                          clipping_factors: Optional[torch.Tensor] = None) -> None:
+  """ClippyAdagrad step of a list of dense variables in one multi-tensor call (one clipping factor per variable,
+  written to the float32 device tensor `clipping_factors` [len(variables)] when given)."""
+  nv = len(variables)
+  if len(grads) != nv or len(accums) != nv:
+    raise ValueError("clippy_adagrad_dense_: variables, grads and accums must have the same length")
+  if nv == 0:
+    return
+  dev = variables[0].device
+  gs = []
+  for i, (v, g, a) in enumerate(zip(variables, grads, accums)):
+    _f32_inplace(v, f"variables[{i}]"); _f32_inplace(a, f"accums[{i}]")
+    g = f32c(g, f"grads[{i}]")
+    if v.device != dev or g.device != dev or a.device != dev:
+      raise ValueError("clippy_adagrad_dense_: every tensor must live on one device")
+    if g.shape != v.shape or a.shape != v.shape:
+      raise ValueError(f"clippy_adagrad_dense_: grads[{i}] / accums[{i}] must have the shape {tuple(v.shape)}")
+    gs.append(g)
+  if clipping_factors is not None:
+    _f32_inplace(clipping_factors, "clipping_factors")
+    if clipping_factors.numel() != nv or clipping_factors.device != dev:
+      raise ValueError(f"clippy_adagrad_dense_: clipping_factors must hold {nv} floats on {dev}")
+  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
+  numels = (ctypes.c_int64 * nv)(*[v.numel() for v in variables])
+  wsb = lib().tfrs_clippy_adagrad_dense_workspace_bytes(nv)
+  ws = workspace(wsb, dev, "clippy")
+  check(lib().tfrs_clippy_adagrad_dense_f32(
+      arr(variables), arr(gs), arr(accums), numels, nv, c_f(lr), c_f(eps), c_f(variable_relative_threshold),
+      c_f(accumulator_relative_threshold), c_f(absolute_threshold),
+      _clippy_flags(clip_accumulator_update, use_standard_accumulator_update), ptr(clipping_factors), ptr(ws), ws.numel(),
+      stream()), "clippy_adagrad_dense")
+
+
+# ------------------------------------------------------------------------------------------------
 # K5 cross
 # ------------------------------------------------------------------------------------------------
 # Cross layers at least this large run their forward GEMM on the tensor cores (fp16 hi/lo split, fp32 accumulate).

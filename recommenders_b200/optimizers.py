@@ -6,28 +6,61 @@ tf-keras `optimizers.Adagrad` rule  var -= lr*g/sqrt(acc+eps); False is the lega
 `optimizers.legacy.Adagrad` rule  var -= lr*g/(sqrt(acc)+eps)  (SURVEY.md A10 -- third-party, unpinned)."""
 from __future__ import annotations
 
-from typing import Iterable, List
+from typing import Iterable, List, Optional, Sequence, Tuple, Union
 
 import torch
 
 from . import ops
 from .layers.embedding import Embedding
 
+Variable = Union[Embedding, torch.nn.Parameter]
 
-class Adagrad:
 
-  def __init__(self, learning_rate: float = 0.001, initial_accumulator_value: float = 0.1, epsilon: float = 1e-7,
-               eps_inside_sqrt: bool = True):
-    self.learning_rate = learning_rate
+def embedding_tables(module: torch.nn.Module) -> List[Embedding]:
+  """The embedding tables of a model (updated from their sparse (ids, rows) gradients)."""
+  return [m for m in module.modules() if isinstance(m, Embedding)]
+
+
+def dense_variables(module: torch.nn.Module) -> List[torch.nn.Parameter]:
+  """The trainable parameters of a model other than the tables' autograd anchors."""
+  anchors = {id(t._anchor) for t in embedding_tables(module)}
+  return [p for p in module.parameters() if p.requires_grad and id(p) not in anchors]
+
+
+def split_variables(variables: Iterable[Variable]) -> Tuple[List[Embedding], List[torch.nn.Parameter]]:
+  tables, dense = [], []
+  for v in variables:
+    if isinstance(v, Embedding):
+      tables.append(v)
+    elif isinstance(v, torch.Tensor):
+      dense.append(v)
+    else:
+      raise TypeError(f"cannot optimize a {type(v).__name__}: expected an Embedding or a torch.nn.Parameter")
+  return tables, dense
+
+
+def clear_grads(tables: Sequence[Embedding], dense: Sequence[torch.Tensor]) -> None:
+  for p in dense:
+    p.grad = None
+  for t in tables:
+    t.pop_sparse_grads()
+    t._anchor.grad = None
+
+
+class _AccumulatorOptimizer:
+  """Variable discovery and per-variable accumulator slots shared by Adagrad and ClippyAdagrad."""
+
+  _ACC_ATTR = "_tfrs_adagrad_acc"
+
+  def __init__(self, initial_accumulator_value: float):
     self.initial_accumulator_value = initial_accumulator_value
-    self.epsilon = epsilon
-    self.eps_inside_sqrt = eps_inside_sqrt
+    self.iterations = 0
     self._module = None
     self._dense: List[torch.nn.Parameter] = []
     self._tables: List[Embedding] = []
     self._acc = {}
 
-  def bind(self, module: torch.nn.Module) -> "Adagrad":
+  def bind(self, module: torch.nn.Module):
     """Attach to a model.  The variable lists are re-read on every step (`_refresh`), like the reference's
     `self.trainable_variables` at models/base.py:77: layers that create their weights lazily on the first
     forward (Cross, MultiLayerDCN) are picked up even when compile() ran before the first batch."""
@@ -38,33 +71,60 @@ class Adagrad:
   def _refresh(self) -> None:
     if self._module is None:
       return
-    self._tables = [m for m in self._module.modules() if isinstance(m, Embedding)]
-    anchors = {id(t._anchor) for t in self._tables}
-    self._dense = [p for p in self._module.parameters() if p.requires_grad and id(p) not in anchors]
+    self._tables = embedding_tables(self._module)
+    self._dense = dense_variables(self._module)
 
   def _accum(self, owner, like: torch.Tensor) -> torch.Tensor:
     """Accumulator slot of a variable, stored ON its owner object (an Embedding module or a Parameter) so it
     lives and dies with it -- an id()-keyed dict would hand a recycled id the previous owner's state."""
-    a = getattr(owner, "_tfrs_adagrad_acc", None)
+    a = getattr(owner, self._ACC_ATTR, None)
     if a is None or a.shape != like.shape or a.device != like.device:
       a = torch.full_like(like, self.initial_accumulator_value)
-      owner._tfrs_adagrad_acc = a
+      setattr(owner, self._ACC_ATTR, a)
       self._acc[id(owner)] = a
     return a
 
   def zero_grad(self):
     self._refresh()
-    for p in self._dense:
-      p.grad = None
-    for t in self._tables:
-      t.pop_sparse_grads()
-      t._anchor.grad = None
+    clear_grads(self._tables, self._dense)
 
   @torch.no_grad()
-  def apply_gradients(self):
-    """optimizer.apply_gradients(zip(grads, vars)) -- models/base.py:78."""
-    self._refresh()
-    for t in self._tables:
+  def apply_gradients(self, variables: Optional[Iterable[Variable]] = None):
+    """optimizer.apply_gradients(zip(grads, vars)) -- models/base.py:78.  Updates the bound model's variables, or only
+    `variables` (Embedding modules and Parameters) when given."""
+    if variables is None:
+      self._refresh()
+      tables, dense = self._tables, self._dense
+    else:
+      tables, dense = split_variables(variables)
+    self._apply(tables, dense)
+    self.iterations += 1
+
+  def step(self, variables: Optional[Iterable[Variable]] = None):
+    return self.apply_gradients(variables)
+
+  def _apply(self, tables: Sequence[Embedding], dense: Sequence[torch.nn.Parameter]) -> None:
+    raise NotImplementedError
+
+  def variables(self) -> List[torch.Tensor]:
+    """The optimizer's state: one accumulator per variable it has updated."""
+    return list(self._acc.values())
+
+  def state_dict(self):
+    return {"acc": {k: v.clone() for k, v in self._acc.items()}}
+
+
+class Adagrad(_AccumulatorOptimizer):
+
+  def __init__(self, learning_rate: float = 0.001, initial_accumulator_value: float = 0.1, epsilon: float = 1e-7,
+               eps_inside_sqrt: bool = True):
+    super().__init__(initial_accumulator_value)
+    self.learning_rate = learning_rate
+    self.epsilon = epsilon
+    self.eps_inside_sqrt = eps_inside_sqrt
+
+  def _apply(self, tables, dense):
+    for t in tables:
       grads = t.pop_sparse_grads()
       if not grads:
         continue
@@ -72,7 +132,7 @@ class Adagrad:
       rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
       ops.sparse_adagrad_(t.weight, self._accum(t, t.weight), ids, rows, self.learning_rate, self.epsilon,
                           self.eps_inside_sqrt)
-    for p in self._dense:
+    for p in dense:
       if p.grad is None:
         continue
       a = self._accum(p, p)
@@ -80,8 +140,3 @@ class Adagrad:
       a.addcmul_(g, g)
       den = (a + self.epsilon).sqrt_() if self.eps_inside_sqrt else a.sqrt().add_(self.epsilon)
       p.addcdiv_(g, den, value=-self.learning_rate)
-
-  step = apply_gradients
-
-  def state_dict(self):
-    return {"acc": {k: v.clone() for k, v in self._acc.items()}}

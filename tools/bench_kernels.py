@@ -1,6 +1,7 @@
 """Secondary measurements for BASELINE.md §4 (configs 3 and 5): embedding gather GB/s, sparse Adagrad,
-in-batch softmax step, Cross layer.  CUDA events, warm-up, inputs larger than L2 or rotated between
-iterations.  Prints one JSON object.   usage: python tools/bench_kernels.py [--quick] [--top-stack-only]"""
+in-batch softmax step, Cross layer, ClippyAdagrad.  CUDA events, warm-up, inputs larger than L2 or rotated between
+iterations.  Prints one JSON object.
+usage: python tools/bench_kernels.py [--quick] [--top-stack-only | --optimizers-only]"""
 import json
 import os
 import sys
@@ -36,6 +37,53 @@ def timeit(fn, iters=20, warm=5):
 
 out = {"hbm_peak_gbs": HBM}
 g = torch.Generator(device=dev); g.manual_seed(7)
+
+
+def optimizer_legs():
+  """Sparse Adagrad (K4) and sparse ClippyAdagrad (K7) on the same B = 16384 batches of a 1M x 64 user table, uniform and
+  Zipf(1.05) ids, then the dense ClippyAdagrad multi-tensor step of the cfg5 top stack.  Algorithmic bytes from the
+  unique rows u of each batch: Adagrad n*d*4 + 4*u*d*4; ClippyAdagrad pass A n*d*4 + 3*u*d*4, pass B 5*u*d*4."""
+  import numpy as np
+  V, d, n = (1_000_000, 64, 16384) if not quick else (100_000, 64, 4096)
+  table = (torch.rand((V, d), generator=g, device=dev) - 0.5) * 0.1
+  acc_ag = torch.full_like(table, 0.1); acc_cl = torch.full_like(table, 0.1)
+  grads = torch.randn((n, d), generator=g, device=dev) * 0.01
+  rng = np.random.RandomState(3)
+  batches = {"uniform": [torch.randint(0, V, (n,), generator=g, device=dev) for _ in range(4)],
+             "zipf": [torch.from_numpy(np.minimum(rng.zipf(1.05, size=n) - 1, V - 1)).to(dev) for _ in range(4)]}
+  res = {}
+  for kind, ids in batches.items():
+    u = sum(int(torch.unique(i).numel()) for i in ids) / len(ids)
+    it = {"i": 0}
+
+    def nxt():
+      k = it["i"] % 4; it["i"] += 1
+      return ids[k]
+    t_ag = timeit(lambda: ops.sparse_adagrad_(table, acc_ag, nxt(), grads, 0.5), iters=50, warm=5)
+    t_cl = timeit(lambda: ops.sparse_clippy_adagrad_(table, acc_cl, nxt(), grads, 0.5, 1e-7, 0.1, 1e-3, 1e-7), iters=50, warm=5)
+    b_ag = n * d * 4 + 4 * u * d * 4
+    b_cl = n * d * 4 + 8 * u * d * 4
+    res[kind] = {"unique_rows": u, "adagrad_seconds": t_ag, "adagrad_GBps_algorithmic": b_ag / t_ag / 1e9,
+                 "clippy_seconds": t_cl, "clippy_GBps_algorithmic": b_cl / t_cl / 1e9, "clippy_over_adagrad": t_cl / t_ag}
+  res["shape"] = f"table {V}x{d}, batch {n}, ids int64, 4 batches rotated"
+  out["cfg3_sparse_clippy_adagrad"] = res
+  del table, acc_ag, acc_cl, grads, batches
+  shapes = [(845, 512), (512,), (512, 256), (256,), (256, 1), (1,)]
+  vs = [torch.randn(s, generator=g, device=dev) * 0.05 for s in shapes]
+  gs = [torch.randn(s, generator=g, device=dev) * 0.01 for s in shapes]
+  accs = [torch.full(s, 0.1, device=dev) for s in shapes]
+  f = torch.zeros((len(shapes),), device=dev)
+  t = timeit(lambda: ops.clippy_adagrad_dense_(vs, gs, accs, 0.05, 1e-7, 0.1, 1e-3, 1e-7, clipping_factors=f), iters=100, warm=10)
+  N = sum(v.numel() for v in vs)
+  out["cfg5_top_stack_clippy_dense_step"] = {"seconds": t, "elements": N, "variables": len(shapes),
+                                             "GBps_algorithmic": 8 * N * 4 / t / 1e9, "launches": 3,
+                                             "note": "init + pass A + pass B; bytes 3N*4 read (A) + 3N*4 read, 2N*4 written (B)"}
+
+
+if "--optimizers-only" in sys.argv:
+  optimizer_legs()
+  print(json.dumps(out))
+  sys.exit(0)
 
 # ---- config 5 top stack (K6): MLP 845 -> 512 (relu) -> 256 (relu) -> 1 (sigmoid) at B = 65536, forward and forward + backward
 #      (dx of the stack input, dW, db of every layer).  `--top-stack-only` prints this leg alone.
@@ -204,12 +252,13 @@ def adagrad3():
 
 t = timeit(adagrad3)
 out["cfg3_sparse_adagrad_user_table"] = {"seconds": t, "rows": Bt, "GBps_algorithmic": (Bt * d * 4 * 5) / t / 1e9}
+del ut, it, uacc, iacc
+torch.cuda.empty_cache()
+optimizer_legs()
 # ---- Streaming over a corpus that lives in HOST memory (SURVEY 8f-1): 1M x 64 rows in pinned memory, dataset batches of
 #      8192 rows coalesced into 262144-row chunks, pinned double-buffered H2D overlapped with the tensor-core scan per chunk
 try:
   import recommenders_b200 as tfrs
-  del ut, it, uacc, iacc
-  torch.cuda.empty_cache()
   Ns, Qs, ks = (1_000_000, 4096, 100) if not quick else (200_000, 1024, 100)
   corpus_host = torch.randn((Ns, 64), generator=torch.Generator().manual_seed(1)).pin_memory()
   qd = torch.randn((Qs, 64), generator=g, device=dev)
