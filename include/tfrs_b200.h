@@ -440,6 +440,64 @@ int tfrs_ranking_metrics_f32(const float* pred, const float* labels, const float
                                     float threshold, int num_thresholds, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K8  UnifiedEmbedding lookup (layers/feature_multiplexing/unified_embedding.py:186-215): every chunk of a feature is
+ * tf-keras Hashing(num_bins = table rows, salt) followed by an embedding lookup in a table shared with other features.
+ *   bin = SipHash-2-4(k0 = salt[0], k1 = salt[1], message) mod num_bins   (tf.strings.to_hash_bucket_strong)
+ * message: the bytes of a TFRS_BYTES value; for TFRS_I32 / TFRS_I64 values the decimal text of tf.as_string (a leading
+ * '-' for negatives, no '+', no padding).
+ *
+ * A feature is one input stream of n values; its n_chunks slots are the next n_chunks entries of `slots` (features in
+ * order, so slots of feature k follow those of feature k-1).  Each slot names its table ([rows, dim], rows = num_bins),
+ * its salt, and where its dim columns go: out[i * ld + col_off ..].
+ *  - row_splits == NULL: out row i = table[bin(value i)] for i < n.
+ *  - row_splits != NULL ([n_bags + 1], non-decreasing from 0 to n, as tf.RaggedTensor.from_row_splits): out row b =
+ *    the bag values[row_splits[b] .. row_splits[b+1]) pooled: the rows summed in value order in fp32 from +0, then one
+ *    IEEE division by the count (MEAN) or by sqrtf(count) (SQRTN); an empty bag gives zeros.
+ * `ids` (int64 [n], nullable unless pooled) receives the bucket ids; pointing the slots of one table at consecutive
+ * ranges of one buffer gives that table's ids contiguous, in the caller's slot order.
+ * dim, col_off and ld are multiples of 4; table, out, grad and grad_rows 16-byte aligned.
+ * Launches: forward 1 for up to 64 features and 256 slots (+1 when a feature is pooled); longer calls take one (or two)
+ * per group of whole features.  Backward 1 per group.
+ * Backward: grad_rows (fp32 [n, dim]) row i = grad[i * ld + col_off ..] (unpooled) or the bag gradient of value i
+ * divided as in the forward (pooled; a value outside every bag gets zeros).  Only n, row_splits, n_bags, combiner and
+ * n_chunks of the features and dim, ld, col_off, grad and grad_rows of the slots are read.  No float atomics.
+ * Pooled features need n_bags >= 1 unless n == 0.  An empty call (n == 0 and no bags) may pass NULL outputs.
+ * tfrs_hash_bins: bins[i] = bin(value i) for one stream and one salt (I32, I64, or BYTES with offsets [n+1]).
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_BYTES = 2 };
+enum { TFRS_COMBINER_SUM = 0, TFRS_COMBINER_MEAN = 1, TFRS_COMBINER_SQRTN = 2 };
+typedef struct tfrs_ue_feature {
+  const void* values;          /* TFRS_I32 / TFRS_I64 values, or the bytes of TFRS_BYTES strings */
+  const int64_t* offsets;      /* TFRS_BYTES: [n + 1]; string i = bytes [offsets[i], offsets[i+1]) of values */
+  int64_t n;
+  const int64_t* row_splits;   /* nullable: pooled bags */
+  int64_t n_bags;
+  int32_t kind;
+  int32_t combiner;            /* TFRS_COMBINER_*, pooled features */
+  int32_t n_chunks;
+  int32_t reserved;
+} tfrs_ue_feature;
+typedef struct tfrs_ue_slot {
+  const float* table;
+  int64_t rows;                /* = num_bins */
+  uint64_t salt[2];            /* the SipHash key (k0, k1), by value */
+  float* out;
+  int64_t ld;
+  int32_t col_off;
+  int32_t dim;
+  int64_t* ids;                /* nullable unless pooled */
+  const float* grad;           /* backward: gradient of out */
+  float* grad_rows;            /* backward: [n, dim] */
+} tfrs_ue_slot;
+/* `salt` is a HOST array of two uint64 (k0, k1); values, offsets and bins are device pointers. */
+int tfrs_hash_bins(const void* values, const int64_t* offsets, int kind, int64_t n, const uint64_t* salt, int64_t num_bins,
+                   int64_t* bins, void* stream);
+int tfrs_unified_lookup_fwd_f32(const tfrs_ue_feature* features, int n_features, const tfrs_ue_slot* slots, int n_slots,
+                                void* stream);
+int tfrs_unified_lookup_bwd_f32(const tfrs_ue_feature* features, int n_features, const tfrs_ue_slot* slots, int n_slots,
+                                void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DLRM DotInteraction (layers/feature_interaction/dot_interaction.py:53-104; SURVEY 8f-4): feats [B,F,d] ->
  * pairwise dots e_i.e_j of every sample; output = lower triangle in (i,j) row-major order without
  * (self_interaction=0) or with the diagonal, [B, out_dim], or the full [B,F*F] matrix with the excluded part

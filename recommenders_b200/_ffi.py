@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("TFRS_B200_LIB", os.path.join(_HERE, "libtfrs_b200.so"
 
 _lib: Optional[ctypes.CDLL] = None
 
-I32, I64 = 0, 1
+I32, I64, BYTES = 0, 1, 2
 c_p = ctypes.c_void_p
 c_i = ctypes.c_int
 c_l = ctypes.c_int64
@@ -104,6 +104,9 @@ _SIGNATURES = {
     "tfrs_ranking_loss_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p, c_f, c_i, c_p, c_sz, c_p]),
     "tfrs_ranking_loss_bwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_ranking_metrics_f32": (c_i, [c_p, c_p, c_p, c_l, c_p, c_f, c_i, c_p, c_sz, c_p]),
+    "tfrs_hash_bins": (c_i, [c_p, c_p, c_i, c_l, c_p, c_l, c_p, c_p]),
+    "tfrs_unified_lookup_fwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
+    "tfrs_unified_lookup_bwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

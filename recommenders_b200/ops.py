@@ -6,7 +6,7 @@ autograd tape.  No CPU fallback.
 from __future__ import annotations
 
 import ctypes
-from typing import Optional, Sequence, Tuple
+from typing import NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -60,6 +60,151 @@ def gather(tables: Sequence[torch.Tensor], ids: Sequence[torch.Tensor], out: Opt
   co = (ctypes.c_int32 * nt)(*[int(c) for c in col_offsets])
   check(lib().tfrs_gather_f32(tp, rows, dm, nt, ip, code, n, ptr(out), out_ld, co, stream()), "gather")
   return out
+
+
+# ------------------------------------------------------------------------------------------------
+# K8 UnifiedEmbedding: salted SipHash bucketing fused with the shared-table gather
+# ------------------------------------------------------------------------------------------------
+COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
+
+
+class _UeFeature(ctypes.Structure):
+  _fields_ = [("values", ctypes.c_void_p), ("offsets", ctypes.c_void_p), ("n", ctypes.c_int64),
+              ("row_splits", ctypes.c_void_p), ("n_bags", ctypes.c_int64), ("kind", ctypes.c_int32),
+              ("combiner", ctypes.c_int32), ("n_chunks", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
+class _UeSlot(ctypes.Structure):
+  _fields_ = [("table", ctypes.c_void_p), ("rows", ctypes.c_int64), ("salt", ctypes.c_uint64 * 2),
+              ("out", ctypes.c_void_p), ("ld", ctypes.c_int64), ("col_off", ctypes.c_int32), ("dim", ctypes.c_int32),
+              ("ids", ctypes.c_void_p), ("grad", ctypes.c_void_p), ("grad_rows", ctypes.c_void_p)]
+
+
+def salt_key(salt) -> Tuple[int, int]:
+  """The SipHash key of a tf-keras `Hashing` salt: an int s means (s, s), a pair is (k0, k1); both as uint64."""
+  if isinstance(salt, int):
+    salt = (salt, salt)
+  k0, k1 = (int(s) for s in salt)
+  return k0 & (2**64 - 1), k1 & (2**64 - 1)
+
+
+class LookupInput(NamedTuple):
+  """One input stream: CUDA int32 / int64 `values`, or the uint8 bytes of strings with their int64 `offsets` [n+1].
+  `row_splits` (int64 [bags+1]) pools the values into bags with `combiner`."""
+  values: torch.Tensor
+  offsets: Optional[torch.Tensor] = None
+  row_splits: Optional[torch.Tensor] = None
+  combiner: str = "mean"
+
+  @property
+  def n(self) -> int:
+    return self.values.numel() if self.offsets is None else self.offsets.numel() - 1
+
+
+class LookupSlot(NamedTuple):
+  """One (feature, chunk) lookup: `table` [num_bins, dim] hashed with `salt`, written to columns [col_off, col_off+dim)
+  of the 2-D `out`; the bucket ids go to `ids` (int64 [n]) when it is given (required for pooled inputs)."""
+  input: int
+  table: torch.Tensor
+  salt: Tuple[int, int]
+  out: torch.Tensor
+  col_off: int
+  ids: Optional[torch.Tensor] = None
+
+
+def _value_kind(values: torch.Tensor, offsets: Optional[torch.Tensor]) -> int:
+  require_cuda(values, "values")
+  if offsets is not None:
+    require_cuda(offsets, "offsets")
+    if values.dtype != torch.uint8 or offsets.dtype != torch.int64:
+      raise TypeError("string values must be uint8 bytes with int64 offsets")
+    return _ffi.BYTES
+  return _ffi.ids_dtype_code(values)
+
+
+def hash_bins(values, num_bins: int, salt) -> torch.Tensor:
+  """tf-keras `Hashing(num_bins, salt=salt)` on the device: SipHash-2-4 keyed by the salt, mod num_bins, int64.  `values`
+  is a CUDA int32 / int64 tensor (hashed as its decimal text) or a (uint8 bytes, int64 offsets [n+1]) pair of strings."""
+  values, offsets = values if isinstance(values, tuple) else (values, None)
+  kind = _value_kind(values, offsets)
+  values = values.contiguous()
+  offsets = offsets.contiguous() if offsets is not None else None
+  n = values.numel() if offsets is None else offsets.numel() - 1
+  out = torch.empty(values.shape if offsets is None else (n,), dtype=torch.int64, device=values.device)
+  key = (ctypes.c_uint64 * 2)(*salt_key(salt))
+  check(lib().tfrs_hash_bins(ptr(values), ptr(offsets), kind, n, key, int(num_bins), ptr(out), stream()), "hash_bins")
+  return out
+
+
+def _out_rows(x: LookupInput) -> int:
+  return x.n if x.row_splits is None else x.row_splits.numel() - 1
+
+
+def _check_2d(t: torch.Tensor, rows: int, what: str) -> None:
+  require_cuda(t, what)
+  if t.dtype != torch.float32 or t.dim() != 2 or t.shape[0] != rows or (t.stride(1) != 1 and t.numel() > 0):
+    raise ValueError(f"unified_lookup: {what} must be 2-D float32 [{rows}, >= width] with unit inner stride")
+
+
+def _ue_structs(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], outs: Sequence[torch.Tensor]):
+  """The C descriptors of one call; slots must come grouped by input, inputs in order.  `outs[c]` is the 2-D tensor
+  slot c's columns live in: its output in the forward, the gradient of that output in the backward."""
+  order = [s.input for s in slots]
+  if order != sorted(order) or set(order) != set(range(len(inputs))):
+    raise ValueError("unified_lookup: every input needs slots, grouped by input in input order")
+  counts = [order.count(k) for k in range(len(inputs))]
+  feats = (_UeFeature * len(inputs))()
+  for k, x in enumerate(inputs):
+    f = feats[k]
+    f.kind = _value_kind(x.values, x.offsets)
+    f.values, f.offsets = x.values.data_ptr(), (x.offsets.data_ptr() if x.offsets is not None else None)
+    f.n, f.n_chunks = x.n, counts[k]
+    if x.row_splits is not None:
+      require_cuda(x.row_splits, "row_splits")
+      if x.row_splits.dtype != torch.int64 or x.row_splits.dim() != 1 or x.row_splits.numel() < 1:
+        raise TypeError("row_splits must be a non-empty 1-D int64 tensor")
+      f.row_splits, f.n_bags, f.combiner = x.row_splits.data_ptr(), x.row_splits.numel() - 1, COMBINERS[x.combiner]
+  cs = (_UeSlot * len(slots))()
+  for c, (s, o) in enumerate(zip(slots, outs)):
+    require_cuda(s.table, "table")
+    if s.table.dtype != torch.float32 or not s.table.is_contiguous() or s.table.dim() != 2:
+      raise ValueError("unified_lookup: tables must be contiguous 2-D float32")
+    _check_2d(o, _out_rows(inputs[s.input]), "each output / gradient")
+    d = cs[c]
+    d.table, d.rows, d.dim = s.table.data_ptr(), s.table.shape[0], s.table.shape[1]
+    d.salt[0], d.salt[1] = s.salt
+    d.ld, d.col_off = max(o.stride(0), o.shape[1]), s.col_off
+    if s.ids is not None:
+      require_cuda(s.ids, "ids")
+      if s.ids.dtype != torch.int64 or not s.ids.is_contiguous() or s.ids.numel() != inputs[s.input].n:
+        raise ValueError("unified_lookup: ids must be contiguous int64 with one entry per value")
+      d.ids = s.ids.data_ptr()
+  return feats, cs
+
+
+def unified_lookup(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot]) -> None:
+  """Every (feature, chunk) lookup of one UnifiedEmbedding call: out[:, col_off:col_off+dim] = table[bin(value)], or the
+  pooled bag of rows for inputs with row_splits.  One launch (two with pooled inputs)."""
+  feats, cs = _ue_structs(inputs, slots, [s.out for s in slots])
+  for c, s in enumerate(slots):
+    cs[c].out = s.out.data_ptr()
+  check(lib().tfrs_unified_lookup_fwd_f32(feats, len(inputs), cs, len(slots), stream()), "unified_lookup")
+
+
+def unified_lookup_bwd(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], grads: Sequence[torch.Tensor],
+                       grad_rows: Sequence[torch.Tensor]) -> None:
+  """grad_rows[c] ([n, dim]) = the gradient of slot c's table rows, value by value: grads[c] (the gradient of the 2-D
+  output slot c wrote into; `slots[c].out` itself is not read) at the slot's columns, divided by the combiner for pooled
+  inputs.  One launch."""
+  if len(grads) != len(slots) or len(grad_rows) != len(slots):
+    raise ValueError("unified_lookup_bwd: one gradient and one grad_rows tensor per slot")
+  feats, cs = _ue_structs(inputs, slots, grads)
+  for c, (g, r) in enumerate(zip(grads, grad_rows)):
+    require_cuda(r, "grad_rows")
+    if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (inputs[slots[c].input].n, cs[c].dim):
+      raise ValueError("unified_lookup_bwd: grad_rows must be contiguous float32 [n, dim]")
+    cs[c].grad, cs[c].grad_rows = g.data_ptr(), r.data_ptr()
+  check(lib().tfrs_unified_lookup_bwd_f32(feats, len(inputs), cs, len(slots), stream()), "unified_lookup_bwd")
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1,7 +1,7 @@
 """Secondary measurements for BASELINE.md §4 (configs 3 and 5): embedding gather GB/s, sparse Adagrad,
 in-batch softmax step, Cross layer, ClippyAdagrad.  CUDA events, warm-up, inputs larger than L2 or rotated between
 iterations.  Prints one JSON object.
-usage: python tools/bench_kernels.py [--quick] [--top-stack-only | --optimizers-only]"""
+usage: python tools/bench_kernels.py [--quick] [--top-stack-only | --optimizers-only | --unified-only]"""
 import json
 import os
 import sys
@@ -35,8 +35,85 @@ def timeit(fn, iters=20, warm=5):
   return e0.elapsed_time(e1) / iters * 1e-3
 
 
+def graph_time(fn, iters=20):
+  """One call captured in a CUDA graph and replayed: device time.  (The Python binding of a 26-table gather costs more host
+  time than the kernel runs, so a plain Python loop measures the host, with run-to-run differences of 25 %.)"""
+  fn(); torch.cuda.synchronize()
+  gr = torch.cuda.CUDAGraph()
+  with torch.cuda.graph(gr):
+    fn()
+  return timeit(gr.replay, iters=iters)
+
+
 out = {"hbm_peak_gbs": HBM}
 g = torch.Generator(device=dev); g.manual_seed(7)
+
+
+def unified_legs():
+  """K8 (UnifiedEmbedding) at the cfg5 shape: 26 int64 features x 2 chunks over UnifiedEmbeddingConfig(13M buckets,
+  dim 16, 4 tables) -- cfg5's parameter count (26 x 1M x 32) and its [65536, 832] activation.  Ids uniform in [0, 1M)
+  and Zipf(1.05).  Device times are CUDA-graph replays.  Algorithmic bytes of the forward: the 52 rows read and the
+  activation written, the ids read and the bucket ids written (the training forward); the hash-only and K1-gather legs
+  split that time into its hashing and its row traffic."""
+  import subprocess
+  import numpy as np
+  from recommenders_b200.layers.feature_multiplexing import UnifiedEmbedding, UnifiedEmbeddingConfig
+  B, F, V = (65536, 26, 1_000_000) if not quick else (8192, 26, 100_000)
+  buckets, dim = (13_000_000 if not quick else 1_000_000), 16
+  cfg = UnifiedEmbeddingConfig(buckets, dim, 4, "cfg5")
+  for k in range(F):
+    cfg.add_feature(f"f{k}", 2)
+  layer = UnifiedEmbedding(cfg)
+  rng = np.random.RandomState(7)
+  g7 = torch.Generator(device=dev); g7.manual_seed(7)
+  dists = {"uniform": [torch.randint(0, V, (B,), generator=g7, device=dev) for _ in range(F)],
+           "zipf": [torch.from_numpy(np.minimum(rng.zipf(1.05, size=B) - 1, V - 1)).to(dev) for _ in range(F)]}
+  width = 2 * F * dim
+  act = torch.empty((B, width), device=dev)
+  tables = [t.weight for t in layer._tables]
+  chunks = [(k, t, key, pos) for k, (_, ch) in enumerate(layer._plan) for t, key, pos in ch]
+  res = {}
+  for kind, ids in dists.items():
+    inputs = [ops.LookupInput(x) for x in ids]
+    bins = [torch.empty(B, dtype=torch.int64, device=dev) for _ in chunks]
+    slots = [ops.LookupSlot(k, tables[t], key, act, pos * dim, b) for (k, t, key, pos), b in zip(chunks, bins)]
+    slots_inf = [s._replace(ids=None) for s in slots]
+    t_fwd = graph_time(lambda: ops.unified_lookup(inputs, slots))
+    t_inf = graph_time(lambda: ops.unified_lookup(inputs, slots_inf))
+    t_hash = graph_time(lambda: [ops.hash_bins(ids[k], buckets, key) for k, _, key, _ in chunks])
+    t_gather = graph_time(lambda: ops.gather([tables[t] for _, t, _, _ in chunks], bins, out=act,
+                                             col_offsets=[pos * dim for _, _, _, pos in chunks]))
+    grads = [torch.randn((B, width), generator=g7, device=dev)] * len(slots)
+    rows = [torch.empty((B, dim), device=dev) for _ in slots]
+    t_bwd = graph_time(lambda: ops.unified_lookup_bwd(inputs, slots, grads, rows))
+    n_slots = len(chunks)
+    by_fwd = B * n_slots * dim * 4 + B * width * 4 + B * F * 8 + B * n_slots * 8
+    by_gather = B * n_slots * dim * 4 + B * width * 4 + B * n_slots * 8
+    by_bwd = B * width * 4 + B * n_slots * dim * 4
+    res[kind] = {"fwd_seconds": t_fwd, "fwd_algorithmic_bytes": by_fwd, "fwd_GBps": by_fwd / t_fwd / 1e9,
+                 "fwd_frac_of_hbm": by_fwd / t_fwd / 1e9 / HBM, "fwd_no_bucket_ids_seconds": t_inf,
+                 "hash_only_seconds": t_hash, "k1_gather_same_rows_seconds": t_gather,
+                 "k1_gather_GBps": by_gather / t_gather / 1e9, "fwd_over_k1_gather": t_fwd / t_gather,
+                 "bwd_seconds": t_bwd, "bwd_GBps": by_bwd / t_bwd / 1e9}
+  # 26 string features end to end through the layer, host packing and the one upload included: host-bound
+  words = {f"f{k}": np.char.mod("%d", dists["uniform"][k].cpu().numpy()) for k in range(F)}
+  with torch.no_grad():
+    res["strings_end_to_end_seconds"] = timeit(lambda: layer(words), iters=5, warm=2)
+  try:
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                         text=True, timeout=30).stdout.strip().splitlines()[0]
+  except Exception as e:  # the card name from torch is still reported
+    smi = repr(e)
+  res["device"] = torch.cuda.get_device_name(dev)
+  res["nvidia_smi_name_power_limit"] = smi
+  res["shape"] = f"{F} int64 features x 2 chunks, 4 tables {buckets}x{dim}, batch {B}"
+  out["cfg5_unified_embedding"] = res
+
+
+if "--unified-only" in sys.argv:
+  unified_legs()
+  print(json.dumps(out))
+  sys.exit(0)
 
 
 def optimizer_legs():
@@ -132,16 +209,6 @@ state = {"i": 0}
 
 def gather5():
   ops.gather(tables, ids_sets[state["i"] % 4], out=act); state["i"] += 1
-
-
-def graph_time(fn, iters=20):
-  """One call captured in a CUDA graph and replayed: device time.  (The Python binding of a 26-table gather costs more host
-  time than the kernel runs, so a plain Python loop measures the host, with run-to-run differences of 25 %.)"""
-  fn(); torch.cuda.synchronize()
-  gr = torch.cuda.CUDAGraph()
-  with torch.cuda.graph(gr):
-    fn()
-  return timeit(gr.replay, iters=iters)
 
 
 t = sum(graph_time(lambda ids=ids: ops.gather(tables, ids, out=act)) for ids in ids_sets) / len(ids_sets)
