@@ -498,6 +498,52 @@ int tfrs_unified_lookup_bwd_f32(const tfrs_ue_feature* features, int n_features,
                                 void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K9  tree-AH approximate retrieval: the algorithm of ScaNN (layers/factorized_top_k.py:613-796) under the rules of
+ * DESIGN.md §2 -- a k-means tree of L leaves over the rows, 4-bit product codes of every row's residual (blocks of dpb
+ * dims, 16 centers each), and a search that scores the rows of the probed leaves with int8 lookup tables.
+ * d <= 256, 1 <= dpb <= 8, B = ceil(d / dpb) blocks, W = ceil(B / 8) code words per row, N < 2^24 rows.
+ *
+ * Index build (the host runs the Lloyd iterations):
+ *   tfrs_tree_ah_assign_f32: leaf[i] = top-1 of the canonical dot [x_i, 1] . [c_l, -0.5f * |c_l|^2] (squared L2, ties to
+ *     the lower l), through tfrs_topk_scan_f32 in chunks of 65536 rows.
+ *   tfrs_tree_ah_group: order[] = positions 0..n-1 grouped by leaf in ascending leaf order, positions ascending inside a
+ *     leaf; offsets[l] .. offsets[l+1] is leaf l's range (offsets has L + 1 entries).
+ *   tfrs_tree_ah_update_centroids_f32: every non-empty leaf's centroid = the float64 sum of its members' rows x[order[..]]
+ *     taken sequentially in that order, divided once by the count, rounded to fp32.  Empty leaves keep theirs.
+ *   Codebooks are fp32 [B][16][dpb] (the last block's unused dims are 0); residual r = x - c_leaf(x) (one fp32 subtraction).
+ *   tfrs_tree_ah_init_codebooks_f32: center j of every block = the residual of position pos[j] (pos: 16 int64).
+ *   tfrs_tree_ah_encode: codes of positions p < n (row = rows ? rows[p] : p; leaf indexed by row): per block the top-1 of
+ *     [r_b, 1] . [cb_j, -0.5f |cb_j|^2]; packed 8 per uint32 (block 8w+e in bits 4e..4e+3), W words per position.
+ *   tfrs_tree_ah_update_codebooks_f32: codebook update from the codes of positions 0..n-1, the same ordered float64 mean.
+ * Search: per query, probe the top P leaves by canonical dot(q, c_l) (ties to the lower leaf); LUT T[b][j] = canonical
+ *   dot of block b of q with center j, s = max|T| / 127 (0 if max|T| = 0), T8 = (int8) rint(T / s); the approximate
+ *   score of a row of probed leaf l is  dot(q, c_l) + s * (float) sum_b T8[b][code_b]  (two rounded fp32 ops).  The top
+ *   k' rows by that score are kept; with `rows` (fp32 [N, d], original row order) they are rescored with the canonical
+ *   dot and the top k of those returned, otherwise k' == k and the approximate scores are returned.  Order = (score desc,
+ *   row asc).  Positions with no row (the probed leaves hold fewer) get (NaN, 0).  out_*: [Q, k]; out_idx = row ids.
+ *   P <= min(L, 2048), k <= k' <= 2048.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_tree_ah_assign_workspace_bytes(int64_t n, int d, int L);
+int tfrs_tree_ah_assign_f32(const float* x, int64_t n, int d, const float* centers, int L, int64_t* leaf, void* ws,
+                            size_t ws_bytes, void* stream);
+size_t tfrs_tree_ah_group_workspace_bytes(int64_t n);
+int tfrs_tree_ah_group(const int64_t* leaf, int64_t n, int L, int32_t* offsets, int32_t* order, void* ws, size_t ws_bytes,
+                       void* stream);
+int tfrs_tree_ah_update_centroids_f32(const float* x, int d, const int32_t* order, const int32_t* offsets, int L,
+                                      float* centroids, void* stream);
+int tfrs_tree_ah_init_codebooks_f32(const float* x, int d, const int64_t* pos, const int64_t* leaf, const float* centroids,
+                                    int dpb, float* codebooks, void* stream);
+int tfrs_tree_ah_encode(const float* x, int d, const int32_t* rows, int64_t n, const int64_t* leaf, const float* centroids,
+                        const float* codebooks, int dpb, uint32_t* codes, void* stream);
+int tfrs_tree_ah_update_codebooks_f32(const float* x, int d, int64_t n, const int64_t* leaf, const float* centroids,
+                                      const uint32_t* codes, int dpb, float* codebooks, void* stream);
+size_t tfrs_tree_ah_search_workspace_bytes(int64_t Q, int d, int L, int P, int dpb, int k, int kp, int reorder, int64_t N);
+int tfrs_tree_ah_search_f32(const float* q, int64_t Q, int d, const float* centroids, int L, const int32_t* leaf_offsets,
+                            const float* codebooks, int dpb, const uint32_t* codes, const int32_t* order, int64_t N,
+                            const float* rows, int P, int k, int kp, float* out_scores, int64_t* out_idx, void* ws,
+                            size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DLRM DotInteraction (layers/feature_interaction/dot_interaction.py:53-104; SURVEY 8f-4): feats [B,F,d] ->
  * pairwise dots e_i.e_j of every sample; output = lower triangle in (i,j) row-major order without
  * (self_interaction=0) or with the diagonal, [B, out_dim], or the full [B,F*F] matrix with the excluded part

@@ -107,6 +107,17 @@ _SIGNATURES = {
     "tfrs_hash_bins": (c_i, [c_p, c_p, c_i, c_l, c_p, c_l, c_p, c_p]),
     "tfrs_unified_lookup_fwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
     "tfrs_unified_lookup_bwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
+    "tfrs_tree_ah_assign_workspace_bytes": (c_sz, [c_l, c_i, c_i]),
+    "tfrs_tree_ah_assign_f32": (c_i, [c_p, c_l, c_i, c_p, c_i, c_p, c_p, c_sz, c_p]),
+    "tfrs_tree_ah_group_workspace_bytes": (c_sz, [c_l]),
+    "tfrs_tree_ah_group": (c_i, [c_p, c_l, c_i, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_tree_ah_update_centroids_f32": (c_i, [c_p, c_i, c_p, c_p, c_i, c_p, c_p]),
+    "tfrs_tree_ah_init_codebooks_f32": (c_i, [c_p, c_i, c_p, c_p, c_p, c_i, c_p, c_p]),
+    "tfrs_tree_ah_encode": (c_i, [c_p, c_i, c_p, c_l, c_p, c_p, c_p, c_i, c_p, c_p]),
+    "tfrs_tree_ah_update_codebooks_f32": (c_i, [c_p, c_i, c_l, c_p, c_p, c_p, c_i, c_p, c_p]),
+    "tfrs_tree_ah_search_workspace_bytes": (c_sz, [c_l, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_l]),
+    "tfrs_tree_ah_search_f32": (c_i, [c_p, c_l, c_i, c_p, c_i, c_p, c_p, c_i, c_p, c_p, c_l, c_p, c_i, c_i, c_i, c_p, c_p,
+                                      c_p, c_sz, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

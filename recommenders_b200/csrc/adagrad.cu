@@ -305,6 +305,12 @@ int ag_group(const void* ids, int ids_dtype, long long n, long long rows, void* 
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }
+  return ag_sort(ids, ids_dtype, n, rows, ws, st);
+}
+
+int ag_sort(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st) {
+  const long long P = ag_pow2(n > 2 ? n : 2);
+  unsigned long long* keys = (unsigned long long*)ws;
   unsigned kb = (unsigned)ceil_div(P, 256);
   if (ids_dtype == TFRS_I32) ag_build_keys<int32_t><<<kb, 256, 0, st>>>((const int32_t*)ids, n, rows, P, keys);
   else ag_build_keys<int64_t><<<kb, 256, 0, st>>>((const int64_t*)ids, n, rows, P, keys);

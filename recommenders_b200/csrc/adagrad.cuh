@@ -23,6 +23,9 @@ struct AgGroups {
 size_t ag_group_workspace_bytes(long long n);
 // ws must hold ag_group_workspace_bytes(n) bytes; n >= 1, ids_dtype TFRS_I32 / TFRS_I64
 int ag_group(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st, AgGroups* out);
+// The bitonic branch of ag_group on its own: the first n keys at ws come out in ascending (id, position) order, i.e. the
+// groups in ascending id order as well (tree_ah.cu's leaf-major layout needs that global order).
+int ag_sort(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st);
 
 // One warp per run of equal ids (the warp of the run's first slot; the others exit).  Duplicates are summed in order of
 // occurrence -- the keys are sorted by (id, position) -- with the gradient rows of 8 members in flight per step, so a hot

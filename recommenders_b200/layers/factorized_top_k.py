@@ -1,9 +1,10 @@
 """Top-K retrieval layers: the H100 mirror of tensorflow_recommenders/layers/factorized_top_k.py.
 
 Same classes, constructor arguments, method names and error behaviour as the reference
-(`TopK` :140-333, `Streaming` :336-512, `BruteForce` :515-610, `ScaNN` stub :613-796); tensors are CUDA
-`torch.Tensor`s and the arithmetic runs in libtfrs_b200.so (exact fp32 scan or wgmma screening +
-exact rescoring).  Results follow tf.math.top_k's contract: scores descending, ties -> lower index.
+(`TopK` :140-333, `Streaming` :336-512, `BruteForce` :515-610, `ScaNN` stub :613-796), plus `TreeAH`, ScaNN's
+algorithm under its own name; tensors are CUDA `torch.Tensor`s and the arithmetic runs in libtfrs_b200.so (exact fp32
+scan or wgmma screening + exact rescoring; tree-AH scoring for `TreeAH`).  Results follow tf.math.top_k's contract:
+scores descending, ties -> lower index.
 """
 from __future__ import annotations
 
@@ -534,3 +535,109 @@ class ScaNN(TopK):
 
   def is_exact(self) -> bool:  # pragma: no cover
     return False
+
+
+class TreeAH(TopK):
+  """Tree-AH approximate retrieval: the algorithm of the reference's ScaNN layer (factorized_top_k.py:613-796) on K9.
+
+  Takes ScaNN's constructor arguments and defaults, so `ScaNN(` -> `TreeAH(` moves code over.  `index` trains a k-means
+  tree of `num_leaves` leaves and 4-bit codebooks of the residuals (`dimensions_per_block` dims per code); `call` scores
+  the rows of the best `num_leaves_to_search` leaves with int8 lookup tables and, when `num_reordering_candidates` is
+  set, rescores that many survivors with the exact fp32 dot.  Every rule is pinned in DESIGN.md §2; parity with the
+  scann package itself is not.  `parallelize_batch_searches` is accepted and has no effect: batches always run as one
+  call on the GPU."""
+
+  def __init__(self, query_model: Optional[torch.nn.Module] = None, k: int = 10, distance_measure: Text = "dot_product",
+               num_leaves: int = 100, num_leaves_to_search: int = 10, training_iterations: int = 12,
+               dimensions_per_block: int = 2, num_reordering_candidates: Optional[int] = None,
+               parallelize_batch_searches: bool = True, name: Optional[Text] = None):
+    super().__init__(k=k, name=name)
+    if distance_measure == "squared_l2":
+      raise NotImplementedError("TreeAH supports distance_measure='dot_product' only.")
+    if distance_measure != "dot_product":
+      raise ValueError(f"Unknown distance_measure {distance_measure!r}; expected 'dot_product'.")
+    for arg, v in (("k", k), ("num_leaves", num_leaves), ("num_leaves_to_search", num_leaves_to_search),
+                   ("num_reordering_candidates", num_reordering_candidates)):
+      if v is not None and v <= 0:
+        raise ValueError(f"{arg} must be positive, got {v}.")
+    if training_iterations < 0:
+      raise ValueError(f"training_iterations must be non-negative, got {training_iterations}.")
+    if not 1 <= dimensions_per_block <= 8:
+      raise ValueError(f"dimensions_per_block must be in 1..8, got {dimensions_per_block}.")
+    for arg, v in (("k", k), ("num_leaves_to_search", num_leaves_to_search),
+                   ("num_reordering_candidates", num_reordering_candidates)):
+      if v is not None and v > ops.TREE_AH_MAX_K:
+        raise ValueError(f"{arg} must be at most {ops.TREE_AH_MAX_K}, got {v}.")
+    self.query_model = query_model
+    self._num_leaves = num_leaves
+    self._num_leaves_to_search = num_leaves_to_search
+    self._training_iterations = training_iterations
+    self._dpb = dimensions_per_block
+    self._num_reordering_candidates = num_reordering_candidates
+    self._parallelize_batch_searches = parallelize_batch_searches
+    self._index = None       # ops.tree_ah_build's tensors
+    self._rows = None        # fp32 rows, kept only for reordering
+    self._identifiers = None
+
+  def index(self, candidates: Tensor, identifiers: Optional[Identifiers] = None) -> "TreeAH":
+    if candidates.dim() != 2:
+      raise ValueError(f"The candidates tensor must be 2D (got {tuple(candidates.shape)}).")
+    if identifiers is not None and candidates.shape[0] != identifiers.shape[0]:
+      raise ValueError("The candidates and identifiers tensors must have the same number of"
+                       f" rows (got {candidates.shape[0]} candidates rows and"
+                       f" {identifiers.shape[0]} identifier rows). ")
+    n, d = candidates.shape
+    if not 1 <= d <= 256:
+      raise ValueError(f"TreeAH needs 1 <= d <= 256, got d={d}.")
+    if not 1 <= n < ops.TREE_AH_MAX_ROWS:
+      raise ValueError(f"TreeAH needs 1 <= N < 2^24 candidates, got {n}.")
+    cands = ops.f32c(candidates, "candidates").detach()
+    self._index = ops.tree_ah_build(cands, self._num_leaves, self._training_iterations, self._dpb)
+    self._rows = cands.clone() if self._num_reordering_candidates is not None else None
+    self._identifiers = identifiers
+    self._reset_tf_function_cache()
+    return self
+
+  def call(self, queries, k: Optional[int] = None):
+    k = k if k is not None else self._k
+    if self._index is None:
+      raise ValueError("The `index` method must be called first to create the retrieval index.")
+    if self.query_model is not None:
+      queries = self.query_model(queries)
+    if not isinstance(queries, torch.Tensor):
+      raise ValueError(f"Queries must be a tensor, got {type(queries)}.")
+    if queries.dim() not in (1, 2):
+      raise ValueError(f"Queries must be of rank 2 or 1, got {queries.dim()}.")
+    if not 1 <= k <= ops.TREE_AH_MAX_K:
+      raise ValueError(f"k must be in 1..{ops.TREE_AH_MAX_K}, got {k}.")
+    q = queries.unsqueeze(0) if queries.dim() == 1 else queries
+    k_pre = max(self._num_reordering_candidates or k, k)
+    # every size (d, dimensions per block, L, N) is taken from the index tensors, which ops checks against the queries
+    scores, idx = ops.tree_ah_search(q, self._index, self._rows, self._num_leaves_to_search, k, k_pre)
+    if queries.dim() == 1:
+      scores, idx = scores[0], idx[0]
+    if self._identifiers is None:
+      return scores, idx.to(torch.int32)
+    return scores, _gather_identifiers(self._identifiers, idx)
+
+  def is_exact(self) -> bool:
+    return False
+
+  # -- checkpointing: the trained index is model state (the reference serializes its searcher into the module, :728-730)
+  def get_extra_state(self):
+    ids = self._identifiers
+    return {"index": None if self._index is None else {n: t.cpu() for n, t in self._index.items()},
+            "rows": None if self._rows is None else self._rows.cpu(),
+            "identifiers": ids.cpu() if isinstance(ids, torch.Tensor) else ids}
+
+  def set_extra_state(self, state):
+    if state and state.get("index") is not None:
+      if (state.get("rows") is not None) != (self._num_reordering_candidates is not None):
+        raise ValueError("The saved TreeAH index was built " + ("with" if state.get("rows") is not None else "without") +
+                         " reordering rows; construct the layer with the same num_reordering_candidates setting "
+                         "(None or not None) to restore it.")
+      dev = torch.device("cuda", torch.cuda.current_device())
+      self._index = {n: t.to(dev) for n, t in state["index"].items()}
+      self._rows = None if state.get("rows") is None else state["rows"].to(dev)
+      ids = state.get("identifiers")
+      self._identifiers = ids.to(dev) if isinstance(ids, torch.Tensor) else ids

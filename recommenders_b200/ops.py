@@ -372,6 +372,123 @@ def topk_merge_sorted(scores: torch.Tensor, idx: torch.Tensor, k: int) -> Tuple[
   return out_s, out_i
 
 
+# ------------------------------------------------------------------------------------------------
+# K9 tree-AH: index build and search (DESIGN.md §2 pins every rule)
+# ------------------------------------------------------------------------------------------------
+TREE_AH_MAX_TRAIN = 100000
+TREE_AH_CODEBOOK_ITERATIONS = 10
+TREE_AH_MAX_ROWS = 1 << 24
+TREE_AH_MAX_K = 2048         # probes, k and k' per query
+
+
+def tree_ah_assign(x: torch.Tensor, centers: torch.Tensor) -> torch.Tensor:
+  """Nearest center by squared L2 (top-1 of [x, 1] . [c, -0.5|c|^2], ties -> lower center) -> int64 [n]."""
+  n, d = x.shape
+  L = centers.shape[0]
+  leaf = torch.empty((n,), dtype=torch.int64, device=x.device)
+  ws = workspace(lib().tfrs_tree_ah_assign_workspace_bytes(n, d, L), x.device, "tree_ah")
+  check(lib().tfrs_tree_ah_assign_f32(ptr(x), n, d, ptr(centers), L, ptr(leaf), ptr(ws), ws.numel(), stream()), "tree_ah_assign")
+  return leaf
+
+
+def tree_ah_group(leaf: torch.Tensor, L: int) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Positions grouped by leaf (ascending leaf, then position) -> (order int32 [n], offsets int32 [L+1])."""
+  n = leaf.shape[0]
+  order = torch.empty((n,), dtype=torch.int32, device=leaf.device)
+  offsets = torch.empty((L + 1,), dtype=torch.int32, device=leaf.device)
+  ws = workspace(lib().tfrs_tree_ah_group_workspace_bytes(n), leaf.device, "tree_ah")
+  check(lib().tfrs_tree_ah_group(ptr(leaf), n, L, ptr(offsets), ptr(order), ptr(ws), ws.numel(), stream()), "tree_ah_group")
+  return order, offsets
+
+
+def tree_ah_encode(x: torch.Tensor, rows: Optional[torch.Tensor], leaf: torch.Tensor, centroids: torch.Tensor,
+                   codebooks: torch.Tensor, dpb: int) -> torch.Tensor:
+  """Packed 4-bit residual codes (int32 words [n, W]) of positions p (row = rows[p], or p)."""
+  d = x.shape[1]
+  n = rows.shape[0] if rows is not None else x.shape[0]
+  W = (-(-d // dpb) + 7) // 8
+  codes = torch.empty((n, W), dtype=torch.int32, device=x.device)
+  check(lib().tfrs_tree_ah_encode(ptr(x), d, ptr(rows), n, ptr(leaf), ptr(centroids), ptr(codebooks), dpb, ptr(codes),
+                                  stream()), "tree_ah_encode")
+  return codes
+
+
+def tree_ah_build(candidates: torch.Tensor, num_leaves: int, training_iterations: int, dpb: int) -> dict:
+  """Trains the tree and the codebooks and encodes every row (DESIGN.md §2, index build).  Returns the index tensors:
+  centroids [L, d], leaf_offsets int32 [L+1], order int32 [N] (row ids, leaf-major), codebooks [B, 16, dpb] and
+  codes int32 [N, W] in `order`."""
+  import numpy as np
+  x = f32c(candidates, "candidates")
+  N, d = x.shape
+  dev = x.device
+  n_train = min(N, TREE_AH_MAX_TRAIN)
+  L = min(num_leaves, n_train)
+  B = -(-d // dpb)
+  perm = np.random.default_rng(0).permutation(N)
+  train_rows = np.sort(perm[:n_train])   # ascending row order: the order of every float64 sum
+  xt = gather([x], [torch.from_numpy(train_rows).to(dev)])
+  cent = gather([x], [torch.from_numpy(perm[:L]).to(dev)])
+  for _ in range(training_iterations):
+    order_t, off_t = tree_ah_group(tree_ah_assign(xt, cent), L)
+    check(lib().tfrs_tree_ah_update_centroids_f32(ptr(xt), d, ptr(order_t), ptr(off_t), L, ptr(cent), stream()),
+          "tree_ah_update_centroids")
+  leaf_all = tree_ah_assign(x, cent)
+  order, offsets = tree_ah_group(leaf_all, L)
+  leaf_t = tree_ah_assign(xt, cent)
+  pos = torch.from_numpy(np.searchsorted(train_rows, perm[np.arange(16) % n_train]).astype(np.int64)).to(dev)
+  cb = torch.empty((B, 16, dpb), dtype=torch.float32, device=dev)
+  check(lib().tfrs_tree_ah_init_codebooks_f32(ptr(xt), d, ptr(pos), ptr(leaf_t), ptr(cent), dpb, ptr(cb), stream()),
+        "tree_ah_init_codebooks")
+  for _ in range(TREE_AH_CODEBOOK_ITERATIONS):
+    codes_t = tree_ah_encode(xt, None, leaf_t, cent, cb, dpb)
+    check(lib().tfrs_tree_ah_update_codebooks_f32(ptr(xt), d, n_train, ptr(leaf_t), ptr(cent), ptr(codes_t), dpb, ptr(cb),
+                                                  stream()), "tree_ah_update_codebooks")
+  codes = tree_ah_encode(x, order, leaf_all, cent, cb, dpb)
+  return {"centroids": cent, "leaf_offsets": offsets, "order": order, "codebooks": cb, "codes": codes}
+
+
+def tree_ah_search(q: torch.Tensor, index: dict, rows: Optional[torch.Tensor], num_probes: int, k: int,
+                   k_pre: int) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Probe, AH-score and pre-select k_pre rows per query, then rescore them exactly when `rows` is given -> top k
+  ([Q, k] f32 scores, [Q, k] int64 row ids; (NaN, 0) where the probed leaves hold fewer than k rows).  The sizes
+  (d, dimensions per block, L, N) come from the index tensors themselves, which are checked against each other and
+  against the queries: the kernels read every buffer with them."""
+  q = f32c(q, "queries")
+  if q.dim() != 2:
+    raise ValueError(f"tree_ah_search: queries must be [Q, d], got {tuple(q.shape)}")
+  Q, d = q.shape
+  cent, off, order = index["centroids"], index["leaf_offsets"], index["order"]
+  cb, codes = index["codebooks"], index["codes"]
+  for name, t, dt in (("centroids", cent, torch.float32), ("leaf_offsets", off, torch.int32), ("order", order, torch.int32),
+                      ("codebooks", cb, torch.float32), ("codes", codes, torch.int32)):
+    require_cuda(t, name)
+    if t.dtype != dt or not t.is_contiguous() or t.device != q.device:
+      raise ValueError(f"tree_ah_search: index tensor {name} must be a contiguous {dt} tensor on {q.device}")
+  if cent.dim() != 2 or cent.shape[1] != d:
+    raise ValueError(f"tree_ah_search: queries have d={d} but the index was built for d={cent.shape[1]}")
+  L, N = cent.shape[0], order.shape[0]
+  dpb = cb.shape[2] if cb.dim() == 3 else 0
+  B = -(-d // dpb) if dpb > 0 else 0
+  if (dpb < 1 or tuple(cb.shape) != (B, 16, dpb) or tuple(off.shape) != (L + 1,) or order.dim() != 1 or
+      tuple(codes.shape) != (N, (B + 7) // 8)):
+    raise ValueError("tree_ah_search: inconsistent index tensors "
+                     f"(centroids {tuple(cent.shape)}, leaf_offsets {tuple(off.shape)}, order {tuple(order.shape)}, "
+                     f"codebooks {tuple(cb.shape)}, codes {tuple(codes.shape)})")
+  if rows is not None:
+    rows = f32c(rows, "rows")
+    if tuple(rows.shape) != (N, d) or rows.device != q.device:
+      raise ValueError(f"tree_ah_search: reordering rows must be [{N}, {d}] on {q.device}, got {tuple(rows.shape)}")
+  P = min(num_probes, L)
+  out_s = torch.empty((Q, k), dtype=torch.float32, device=q.device)
+  out_i = torch.empty((Q, k), dtype=torch.int64, device=q.device)
+  wsb = lib().tfrs_tree_ah_search_workspace_bytes(Q, d, L, P, dpb, k, k_pre, 1 if rows is not None else 0, N)
+  ws = workspace(wsb, q.device, "tree_ah")
+  check(lib().tfrs_tree_ah_search_f32(ptr(q), Q, d, ptr(cent), L, ptr(off), ptr(cb), dpb, ptr(codes), ptr(order), N,
+                                      ptr(rows), P, k, k_pre, ptr(out_s), ptr(out_i), ptr(ws), ws.numel(), stream()),
+        "tree_ah_search")
+  return out_s, out_i
+
+
 def topk_sharded(comm, q: torch.Tensor, corpus_local: torch.Tensor, index_buf: Optional[torch.Tensor], k: int,
                  index_offset: int) -> Tuple[torch.Tensor, torch.Tensor]:
   """The row-sharded BruteForce call through the C ABI: local scan -> one NCCL all-gather -> merge, on every rank."""
