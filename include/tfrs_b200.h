@@ -128,11 +128,11 @@ int tfrs_count_above_f32(const float* scores, int64_t ld, int k, const float* po
 int tfrs_topk_hits_accumulate(const int32_t* count, const float* positive_scores, const float* sample_weight, int64_t Q,
                               const int32_t* ks, int n_ks, double* acc, void* stream);
 
-/* Test/debug introspection of tfrs_topk_tc_f32's workspace: out8 = {count offset, fallback-flag offset,
- * threshold offset, survivor-list offset, parts, cap_part, padded Q, cut offset} (byte offsets from the
- * 16-byte-aligned workspace base).  Lets the tests assert that the exact fallback was NOT what produced a
- * result. */
-int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out8);
+/* Test/debug introspection of tfrs_topk_tc_f32's workspace: out10 = {count offset, fallback-flag offset,
+ * threshold offset, survivor-list offset, parts, cap_part, padded Q, cut offset, bins of the sampled pass,
+ * row-exponent offset} (byte offsets from the 16-byte-aligned workspace base).  Lets the tests assert which rows
+ * took the exact fallback and which selection / threshold branch a call ran. */
+int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out10);
 
 /* Optional per-stage device timing of tfrs_topk_tc_f32 (CUDA events on the launch stream; used by
  * bench.py for the roofline figure).  tfrs_profile_read synchronises the device and returns the summed

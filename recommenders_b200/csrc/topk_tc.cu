@@ -440,6 +440,18 @@ __device__ __forceinline__ unsigned int f2key(float f) {
 __device__ __forceinline__ float key2f(unsigned int k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
+// Rank key of an exactly scored candidate (local index < 2^31):
+//   key(score, -0 folded onto +0) << 32 | (2^31 - 1 - index) << 1 | (score is -0.0f)
+// The 64-bit order is (score desc, index asc), with -0 tied to +0 as in the exact path.  The low bit never decides an
+// order (indices are unique); it carries the sign of a zero score, so the output keeps the chain's own bits.
+__device__ __forceinline__ unsigned long long rank_key(float s, unsigned int idx) {
+  const unsigned int lo = (0xFFFFFFFEu - 2u * idx) | (__float_as_uint(s) == 0x80000000u ? 1u : 0u);
+  return ((unsigned long long)f2key(s + 0.0f) << 32) | lo;
+}
+__device__ __forceinline__ float rank_key_score(unsigned long long e) {   // the low bit is only ever set on a zero key
+  return __uint_as_float(__float_as_uint(key2f((unsigned int)(e >> 32))) | ((unsigned int)e << 31));
+}
+__device__ __forceinline__ unsigned int rank_key_index(unsigned long long e) { return 0x7FFFFFFFu - ((unsigned int)e >> 1); }
 __device__ __forceinline__ int warp_incl_scan(int v, int lane) {
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
@@ -533,7 +545,7 @@ __device__ __forceinline__ float exact_score(const float* __restrict__ qs, const
   } else {
     for (int kk = 0; kk < d; ++kk) acc = fmaf(qs[kk], __ldg(c + kk), acc);
   }
-  return acc + 0.0f;  // -0 -> +0: the key order must agree with the float order
+  return acc;  // the chain's own bits, -0.0f included (rank_key folds -0 onto +0 for the order)
 }
 
 // two independent chains at once (same arithmetic per chain as exact_score)
@@ -554,21 +566,21 @@ __device__ __forceinline__ void exact_score2(const float* __restrict__ qs, const
         a0 = fmaf(q3, u0[u].w, a0); a1 = fmaf(q3, u1[u].w, a1);
       }
     }
-    s0 = a0 + 0.0f; s1 = a1 + 0.0f;
+    s0 = a0; s1 = a1;
   } else {
     s0 = exact_score(qs, c0, d); s1 = exact_score(qs, c1, d);
   }
 }
 
-// _exclude (layers/factorized_top_k.py:83-115) on a query's kf best candidates, sorted in `srt` as
-// (key(score) << 32 | ~local index): identifiers in `exclusions[row]` get score - 1e5, the k_out best ADJUSTED scores
-// win (ties -> lower position), the ORIGINAL scores and indices are written.  One warp; akey = kf words of scratch.
+// _exclude (layers/factorized_top_k.py:83-115) on a query's kf best candidates, sorted in `srt` as rank_key(score,
+// local index): identifiers in `exclusions[row]` get score - 1e5, the k_out best ADJUSTED scores win (ties -> lower
+// position), the ORIGINAL scores and indices are written.  One warp; akey = kf words of scratch.
 __device__ __forceinline__ void exclude_rerank(const unsigned long long* srt, int kf, unsigned long long* akey, long long row,
                                                const FinParams& p, int lane) {
   for (int t = lane; t < kf; t += 32) {
     const unsigned long long e = srt[t];
     const float s = key2f((unsigned int)(e >> 32));
-    const long long gi = (long long)(0xFFFFFFFFu - (unsigned int)e) + p.index_offset;
+    const long long gi = (long long)rank_key_index(e) + p.index_offset;
     const long long ident = p.identifiers ? __ldg(p.identifiers + gi) : gi;
     bool isin = false;
     for (int x = 0; x < p.n_excl; ++x) isin |= (__ldg(p.exclusions + row * p.n_excl + x) == ident);
@@ -582,8 +594,8 @@ __device__ __forceinline__ void exclude_rerank(const unsigned long long* srt, in
     for (int j = 0; j < kf; ++j) rank += (akey[j] > mine) ? 1 : 0;
     if (rank < p.k_out) {
       const unsigned long long e = srt[t];
-      p.out_s[row * p.k_out + rank] = key2f((unsigned int)(e >> 32));
-      p.out_i[row * p.k_out + rank] = (long long)(0xFFFFFFFFu - (unsigned int)e) + p.index_offset;
+      p.out_s[row * p.k_out + rank] = rank_key_score(e);
+      p.out_i[row * p.k_out + rank] = (long long)rank_key_index(e) + p.index_offset;
     }
   }
 }
@@ -854,17 +866,13 @@ tc_rescore_kernel(const FinParams p) {
           }
           acc = __shfl_sync(0xffffffffu, acc, (threadIdx.x & 24) | step);   // hand the accumulator to the next lane of the group
         }
-        if (live && sub == 0) {
-          const unsigned int idx = band[t];
-          sk[t] = ((unsigned long long)f2key(acc + 0.0f) << 32) | (unsigned long long)(0xFFFFFFFFu - idx);
-        }
+        if (live && sub == 0) sk[t] = rank_key(acc, band[t]);
       }
     }
   } else {
     for (int t = tid; t < m; t += RS_BLOCK) {
       const unsigned int idx = band[t];
-      const float s = exact_score(qs, p.corpus + (long long)idx * p.d, p.d);
-      sk[t] = ((unsigned long long)f2key(s) << 32) | (unsigned long long)(0xFFFFFFFFu - idx);
+      sk[t] = rank_key(exact_score(qs, p.corpus + (long long)idx * p.d, p.d), idx);
     }
   }
   __syncthreads();
@@ -877,8 +885,8 @@ tc_rescore_kernel(const FinParams p) {
     for (int j = 0; j < m; ++j) rank += (sk[j] > mine) ? 1 : 0;
     if (rank < p.k) {
       if (MODE == FIN_TOPK) {
-        p.out_s[row * p.k + rank] = key2f((unsigned int)(mine >> 32));
-        p.out_i[row * p.k + rank] = (long long)(0xFFFFFFFFu - (unsigned int)mine) + p.index_offset;
+        p.out_s[row * p.k + rank] = rank_key_score(mine);
+        p.out_i[row * p.k + rank] = (long long)rank_key_index(mine) + p.index_offset;
       } else {
         srt[rank] = mine;
       }
@@ -901,8 +909,7 @@ tc_exclude_fallback_kernel(const FinParams p, const float* __restrict__ tmp_s, c
   unsigned long long* srt = reinterpret_cast<unsigned long long*>(fsm) + (size_t)warp * 2 * p.k;
   unsigned long long* akey = srt + p.k;
   for (int t = lane; t < p.k; t += 32)
-    srt[t] = ((unsigned long long)f2key(tmp_s[row * p.k + t] + 0.0f) << 32) |
-             (unsigned long long)(0xFFFFFFFFu - (unsigned int)(tmp_i[row * p.k + t] - p.index_offset));
+    srt[t] = rank_key(tmp_s[row * p.k + t], (unsigned int)(tmp_i[row * p.k + t] - p.index_offset));
   __syncwarp();
   exclude_rerank(srt, p.k, akey, row, p, lane);
 }
@@ -919,7 +926,7 @@ struct FallbackProvider {
     const float* c = corpus + t * d;
     float acc = 0.f;
     for (int kk = 0; kk < d; ++kk) acc = fmaf(qs[kk], __ldg(c + kk), acc);
-    s = acc + 0.0f; i = index_offset + t;
+    s = acc; i = index_offset + t;   // the chain's own bits: row_topk_kernel compares floats (-0 == +0)
   }
 };
 
@@ -1274,12 +1281,13 @@ extern "C" int tfrs_topk_tc_count_f32(const float* q, int64_t Q, const float* co
 
 // Debug/test introspection: where the per-query survivor counts / fallback flags of the last call live
 // inside the caller's workspace (byte offsets from the 16-byte-aligned workspace base).
-extern "C" int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out8) {
-  TFRS_CHECK_ARG(out8, "topk_tc_layout: NULL pointer");
+extern "C" int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out10) {
+  TFRS_CHECK_ARG(out10, "topk_tc_layout: NULL pointer");
   Plan pl;
   if (!make_plan(Q, N, d, k, pl)) { set_error("topk_tc_layout: unsupported shape"); return TFRS_ERR_UNSUPPORTED; }
-  out8[0] = (int64_t)pl.o_count; out8[1] = (int64_t)pl.o_ovf; out8[2] = (int64_t)pl.o_thr; out8[3] = (int64_t)pl.o_cand;
-  out8[4] = pl.parts_full * 2; out8[5] = pl.cap_part; out8[6] = pl.Qp; out8[7] = (int64_t)pl.o_cut;
+  out10[0] = (int64_t)pl.o_count; out10[1] = (int64_t)pl.o_ovf; out10[2] = (int64_t)pl.o_thr; out10[3] = (int64_t)pl.o_cand;
+  out10[4] = pl.parts_full * 2; out10[5] = pl.cap_part; out10[6] = pl.Qp; out10[7] = (int64_t)pl.o_cut;
+  out10[8] = pl.n_bins; out10[9] = (int64_t)pl.o_qexp;
   return TFRS_OK;
 }
 

@@ -528,9 +528,9 @@ def tc_last_call_stats(Q: int, N: int, d: int, k: int, device=None) -> dict:
   """Survivor / fallback statistics of the most recent topk_tc call with this shape (reads the cached
   workspace; synchronises).  Used by tests to prove the tensor-core path -- not the exact fallback --
   produced the result."""
-  out = (ctypes.c_int64 * 8)()
+  out = (ctypes.c_int64 * 10)()
   check(lib().tfrs_topk_tc_layout(Q, N, d, k, out), "topk_tc_layout")
-  o_count, o_ovf, o_thr, o_cand, parts, cap, Qp, o_cut = [int(x) for x in out]
+  o_count, o_ovf, o_thr, o_cand, parts, cap, Qp, o_cut = [int(x) for x in out[:8]]
   dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
   ws = workspace(0, dev, "tc")
   base = (-ws.data_ptr()) % 16

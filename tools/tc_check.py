@@ -32,8 +32,8 @@ print("filter TFLOP/s: %.1f   q/s: %.0f" % (2.0 * Q * N * d / (ms[2] / calls * 1
 if os.environ.get("TC_DEBUG"):
   import ctypes
   from recommenders_b200 import _ffi
-  out = (ctypes.c_int64 * 8)(); _ffi.lib().tfrs_topk_tc_layout(Q, N, d, k, out)
-  o_count, o_ovf, o_thr, o_cand, parts, cap, Qp, o_cut = [int(x) for x in out]
+  out = (ctypes.c_int64 * 10)(); _ffi.lib().tfrs_topk_tc_layout(Q, N, d, k, out)
+  o_count, o_ovf, o_thr, o_cand, parts, cap, Qp, o_cut = [int(x) for x in out[:8]]
   ws = _ffi.workspace(0, dev, "tc"); base = (-ws.data_ptr()) % 16
   thr = ws[base + o_thr: base + o_thr + Q * 4].view(torch.float32)
   cut = ws[base + o_cut: base + o_cut + Q * 4].view(torch.float32)
