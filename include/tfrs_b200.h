@@ -344,7 +344,8 @@ int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* W, const fl
 /* K5 on the tensor cores (forward): the same cross formula as tfrs_cross_fwd_f32, computed as one wgmma GEMM on
  * exactly-rescaled fp16 hi/lo splits of x and W (3 MMAs per K step, fp32 accumulation in registers; ~2^-21 relative
  * error, inside the 1e-5 bar) with the formula fused in the epilogue.  W [D,D] ([in,out]) is taken as stored; `ws`
- * holds the per-call images of x and W.
+ * holds the per-call images of x and W, and for D > 1024 the chunk partials of the reduction (summed in fixed order,
+ * then the formula is applied).
  * For a STACK of cross layers (the reference chains `x = cross(x0, x)`): `out_amax_bits` (nullable, one uint32 on the
  * device) receives max |out| as float bits, accumulated by the epilogue; passing it as `x_amax_bits` (nullable) of the
  * next layer replaces that layer's pass over x for the power-of-two rescale statistic (identical bits, identical result). */
@@ -364,7 +365,7 @@ int tfrs_cross_tc_bwd_f32(const float* x0, const float* x, const float* W, const
 /* General fp32-parity GEMM on the tensor cores (the same exact-rescale + fp16 hi/lo split scheme, ~2^-21 relative error):
  *   C[M,N] = opA(A) . opB(B),  opA(m,k) = transA ? A[k*lda+m] : A[m*lda+k],  opB(k,n) = transB ? B[n*ldb+k] : B[k*ldb+n].
  * Reductions longer than 1024 are accumulated in chunks of 1024 with a fixed-order sum of the partials (deterministic).
- * Serves the projections of the low-rank Cross below and large `_compute_score`-style products. */
+ * Needs ldc >= N, lda >= (transA ? M : K) and ldb >= (transB ? K : N).  Serves the projections of the low-rank Cross below and large `_compute_score`-style products. */
 size_t tfrs_gemm_tc_workspace_bytes(int64_t M, int64_t N, int64_t K);
 int tfrs_gemm_tc_f32(int transA, int transB, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, const float* B,
                      int64_t ldb, float* C, int64_t ldc, void* ws, size_t ws_bytes, void* stream);

@@ -48,6 +48,14 @@ __host__ __device__ __forceinline__ bool better(float sa, long long ia, float sb
   return (sa > sb) || (sa == sb && ia < ib);
 }
 
+// |v| for the rescale statistic max |element|, 0 for Inf and NaN: one non-finite element makes only its own row or column
+// of a split-fp16 product non-finite, instead of leaving the whole operand unscaled.  Every producer of that statistic
+// (tc_split.cuh cx_amax_kernel, the CROSS epilogue's out_amax, cross.cu cross_bwd_elem) uses it, so they agree bit for bit.
+__device__ __forceinline__ float finite_abs(float v) {
+  const float a = fabsf(v);
+  return a < INFINITY ? a : 0.f;
+}
+
 int sm_count();  // SMs of the CURRENT device (cached per device)
 
 // 256-thread blocks for a grid-stride loop over n elements: one element per thread, at most 16 blocks per SM

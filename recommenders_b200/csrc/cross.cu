@@ -32,8 +32,8 @@ struct EpiCrossDx {
   }
 };
 
-// gp = g * x0 (dense [B,D]); dx0 = g * prod; optionally max |gp| (bits of a non-negative float, one atomic per CTA) for
-// the tensor-core path's power-of-two rescale.
+// gp = g * x0 (dense [B,D]); dx0 = g * prod; optionally max |gp| over the finite elements (bits of a non-negative float,
+// one atomic per CTA) for the tensor-core path's power-of-two rescale.
 __global__ void __launch_bounds__(256)
 cross_bwd_elem(const float* __restrict__ x0, const float* __restrict__ prod, const float* __restrict__ g,
                long long B, int D, long long ld, float* __restrict__ gp, float* __restrict__ dx0,
@@ -46,7 +46,7 @@ cross_bwd_elem(const float* __restrict__ x0, const float* __restrict__ prod, con
     float gv = g[o];
     const float v = gv * x0[o];
     gp[e] = v;
-    amax = fmaxf(amax, fabsf(v));
+    amax = fmaxf(amax, finite_abs(v));
     if (dx0) dx0[o] = gv * prod[o];
   }
   if (gp_amax_bits) {
@@ -144,7 +144,7 @@ extern "C" int tfrs_cross_bwd_f32(const float* x0, const float* x, const float* 
 
 // ---- K5 / K5b on the tensor cores: one split-fp16 GEMM forward, two backward; same contract and outputs as the exact path
 extern "C" size_t tfrs_cross_tc_workspace_bytes(int64_t B, int D) {
-  return tc::gemm_tc_workspace(B, D, D, tc::GEMM_EPI_CROSS);
+  return tc::gemm_tc_workspace(B, D, D);
 }
 
 extern "C" int tfrs_cross_tc_fwd_f32(const float* x0, const float* x, const float* W, const float* bias, int64_t B, int D, int64_t ld,
@@ -162,7 +162,7 @@ extern "C" int tfrs_cross_tc_fwd_f32(const float* x0, const float* x, const floa
 // gp | colsum partials | max |gp| | one GEMM workspace shared by the dx and dW calls
 extern "C" size_t tfrs_cross_tc_bwd_workspace_bytes(int64_t B, int D) {
   if (B <= 0 || D <= 0) return 0;
-  const size_t dx_ws = tc::gemm_tc_workspace(B, D, D, tc::GEMM_EPI_DX), dw_ws = tc::gemm_tc_workspace(D, D, B);
+  const size_t dx_ws = tc::gemm_tc_workspace(B, D, D), dw_ws = tc::gemm_tc_workspace(D, D, B);
   return align_up((size_t)B * D * 4, 1024) + align_up((size_t)CROSS_COL_SPLITS * D * 4, 1024) + 1024 + (dx_ws > dw_ws ? dx_ws : dw_ws);
 }
 
@@ -206,6 +206,8 @@ extern "C" int tfrs_gemm_tc_f32(int transA, int transB, int64_t M, int64_t N, in
                                 int64_t ldb, float* C, int64_t ldc, void* ws, size_t ws_bytes, void* stream) {
   TFRS_CHECK_ARG(A && B && C, "gemm_tc: NULL pointer");
   TFRS_CHECK_ARG(M > 0 && N > 0 && K > 0 && ldc >= N, "gemm_tc: bad shape");
+  TFRS_CHECK_ARG(lda >= (transA ? M : K) && ldb >= (transB ? K : N), "gemm_tc: lda=%lld / ldb=%lld below the row length",
+                 (long long)lda, (long long)ldb);
   const tc::GemmOperand a{A, lda, transA != 0};
   const tc::GemmOperand b{B, ldb, transB == 0};   // image rows = n, reduction index k: B[k*ldb + n] is the "transposed" read
   const tc::GemmEpilogue ep{tc::GEMM_EPI_PLAIN, nullptr, 0, nullptr, 0, nullptr, 0.f, nullptr};

@@ -11,10 +11,12 @@
 // K slab a bulk-TMA stage brings 2x(hi,lo) A blocks + (hi,lo) B blocks (96 KB, 2 stages); each of 4 consumer warpgroups
 // owns 64 rows and issues 12 wgmma m64n128k16 per slab into its register accumulators, then applies the epilogue on its
 // fragment.  The warpgroups run independently, so one's MMAs overlap another's epilogue; warp 16 drives the TMA ring.
-// Long reductions with a PLAIN or DENSE epilogue (K > 1024: the batch of a weight gradient) are cut into chunks of 16
+// Long reductions (K > 1024: the batch of a weight gradient, a Cross layer wider than 1024) are cut into chunks of 16
 // K slabs (the tensor core's fp32 adder truncates; long chains drift); every chunk stores a partial [M,N] (mode DW) and
-// a fixed-order fp32 reduction sums them -- deterministic, no atomics.  Items of one chunk run concurrently, so their
+// a fixed-order fp32 reduction sums them and applies the epilogue -- deterministic, no atomics.  Items of one chunk run concurrently, so their
 // image slabs are read from HBM once and shared through L2.
+// Each operand's exponent puts its largest FINITE |element| in [2^13, 2^14) (finite_abs); the epilogue undoes both
+// exponents exactly, also when 2^-(exp_a + exp_b) is not a normal float.
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -89,8 +91,13 @@ split_gemm_kernel(const SgParams p) {
   // warpgroup c: rows [64 c, 64 c + 64) of the 256-row block = half (c & 1) of A block c / 2
   const int c = wg;
   const uint32_t a_off = (uint32_t)((c >> 1) * 32768 + (c & 1) * 8192);
-  const float unscale = ldexpf(1.0f, -(p.ast->exp + p.bst->exp));
-  float amax_out = 0.f;       // CROSS: max |out| over this thread's elements
+  // the product is acc * 2^-S, S = exp_a + exp_b.  When 2^-S is not a normal float (S outside [-127, 126]: tiny or huge
+  // operands whose product is still an fp32 number) that factor would round to 0 or Inf, so unscale = 0 marks the case: the
+  // accumulator is scaled by ldexpf and the epilogue multiplies by 1.  Uniform across the CTA; where 2^-S is normal the bits
+  // are those of acc * 2^-S.
+  const int S = p.ast->exp + p.bst->exp;
+  const float unscale = S >= -127 && S <= 126 ? ldexpf(1.0f, -S) : 0.f;
+  float amax_out = 0.f;       // CROSS: max |out| over this thread's finite elements
   int stage = 0; uint32_t phase = 0;
   for (long long t = blockIdx.x; t < n_items; t += gridDim.x) {
     int kc = 0; long long rem = t;
@@ -118,6 +125,13 @@ split_gemm_kernel(const SgParams p) {
       if (lane == 0) mbar_arrive(&empty[stage]);
       if (++stage == SG_STAGES) { stage = 0; phase ^= 1; }
     }
+    float u = unscale;
+    if (u == 0.f) {
+      const int s = p.ast->exp + p.bst->exp;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = ldexpf(acc[i], -s);
+      u = 1.f;
+    }
     // epilogue on the fragment: lane pairs of adjacent columns, rows r and r + 8 of the warp's 16
     const long long row_base = mb * 256 + c * 64 + warp * 16;
     const int n_base = nt * 128, n_cols = (int)p.N;
@@ -127,24 +141,24 @@ split_gemm_kernel(const SgParams p) {
       const int col = n_base + frag_col(i, lane);
       if (rr >= p.M || col >= n_cols) continue;
       if (MODE == SG_DW) {
-        p.out[(long long)kc * p.M * p.N + rr * p.N + col] = acc[i] * unscale;
+        p.out[(long long)kc * p.M * p.N + rr * p.N + col] = acc[i] * u;
       } else if (MODE == SG_PLAIN) {
-        p.out[rr * p.ld_out + col] = acc[i] * unscale;
+        p.out[rr * p.ld_out + col] = acc[i] * u;
       } else if (MODE == SG_CROSS) {   // out = x0 * (acc + bias + diag * x) + x   (dcn.py:176-186)
         const long long o = rr * p.ld_out + col;
         const float xv = __ldg(p.e1 + o), x0v = __ldg(p.e0 + o);
-        float pv = fmaf(acc[i], unscale, p.bias ? __ldg(p.bias + col) : 0.f);
+        float pv = fmaf(acc[i], u, p.bias ? __ldg(p.bias + col) : 0.f);
         pv = fmaf(p.diag, xv, pv);
         if (p.prod) p.prod[o] = pv;
         const float ov = fmaf(x0v, pv, xv);
         p.out[o] = ov;
-        amax_out = fmaxf(amax_out, fabsf(ov));
+        amax_out = fmaxf(amax_out, finite_abs(ov));
       } else if (MODE >= SG_DENSE) {    // DENSE: y = act(acc + bias)   (Keras Dense: MatMul, BiasAdd, activation)
-        const float z = fmaf(acc[i], unscale, p.bias ? __ldg(p.bias + col) : 0.f);
+        const float z = fmaf(acc[i], u, p.bias ? __ldg(p.bias + col) : 0.f);
         if (MODE == SG_DENSE + TFRS_ACT_SIGMOID && p.prod) p.prod[rr * p.ld_out + col] = z;
         p.out[rr * p.ld_out + col] = dense_act(MODE - SG_DENSE, z);
       } else {                          // DX: dx = acc + diag * gp + g
-        float v = fmaf(acc[i], unscale, __ldg(p.e1 + rr * p.ld1 + col));
+        float v = fmaf(acc[i], u, __ldg(p.e1 + rr * p.ld1 + col));
         if (p.diag != 0.f) v = fmaf(p.diag, __ldg(p.e0 + rr * p.ld0 + col), v);
         p.out[rr * p.ld_out + col] = v;
       }
@@ -181,10 +195,9 @@ static int sg_launch(int mode, const SgParams& p, cudaStream_t st) {
 
 // ---- the driver: operand images, then one launch (plus the partials' reduction when chunked) ------------------------------
 struct GtPlan { int n_mb, n_nt, kb, n_kc; size_t o_st, o_aimg, o_bimg, o_partial, total; };
-static void gt_plan(long long M, long long N, long long K, int mode, GtPlan& pl) {
+static void gt_plan(long long M, long long N, long long K, GtPlan& pl) {
   pl.n_mb = (int)ceil_div(M, 256); pl.n_nt = (int)ceil_div(N, 128); pl.kb = (int)ceil_div(K, 64);
-  const bool chunked = mode == GEMM_EPI_PLAIN || mode == GEMM_EPI_DENSE;
-  pl.n_kc = chunked ? (int)ceil_div(pl.kb, DW_CHUNK_SLABS) : 1;
+  pl.n_kc = (int)ceil_div(pl.kb, DW_CHUNK_SLABS);
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += align_up(bytes, 1024); return r; };
   pl.o_st = take(2048);
@@ -193,9 +206,9 @@ static void gt_plan(long long M, long long N, long long K, int mode, GtPlan& pl)
   pl.o_partial = take(pl.n_kc > 1 ? (size_t)pl.n_kc * M * N * 4 : 0);
   pl.total = o;
 }
-size_t gemm_tc_workspace(long long M, long long N, long long K, int mode) {
+size_t gemm_tc_workspace(long long M, long long N, long long K) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
-  GtPlan pl; gt_plan(M, N, K, mode, pl);
+  GtPlan pl; gt_plan(M, N, K, pl);
   return pl.total;
 }
 
@@ -213,9 +226,45 @@ sg_reduce_chunks_dense_kernel(const float* __restrict__ partial, long long M, lo
   out[o] = dense_act(act, zv);
 }
 
+// The fixed-order sum of the chunk partials (as reduce_parts), then the CROSS or DX epilogue of split_gemm_kernel on the sum
+// (the partials are already unscaled):  CROSS: pv = sum + bias[n] + diag * x; prod = pv; out = x0 * pv + x; out_amax = max
+// finite |out| (one atomic per warp: the bits of a cx_amax_kernel pass over out).  DX: out = sum + g + diag * gp.
+__global__ void __launch_bounds__(256)
+sg_reduce_chunks_cross_dx_kernel(const float* __restrict__ partial, long long M, long long N, int chunks, bool cross,
+                                 const float* __restrict__ e0, long long ld0, const float* __restrict__ e1, long long ld1,
+                                 const float* __restrict__ bias, float diag, float* __restrict__ prod, float* __restrict__ out,
+                                 long long ld, unsigned int* __restrict__ out_amax) {
+  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
+  float amax = 0.f;
+  if (e < M * N) {
+    float a = partial[e];
+    for (int z = 1; z < chunks; ++z) a += partial[(long long)z * M * N + e];
+    const long long m = e / N, n = e % N;
+    if (cross) {   // ld0 == ld1 == ld
+      const long long o = m * ld + n;
+      const float xv = e1[o];
+      float pv = a + (bias ? bias[n] : 0.f);
+      pv = fmaf(diag, xv, pv);
+      if (prod) prod[o] = pv;
+      const float ov = fmaf(e0[o], pv, xv);
+      out[o] = ov;
+      amax = finite_abs(ov);
+    } else {
+      float v = a + e1[m * ld1 + n];
+      if (diag != 0.f) v = fmaf(diag, e0[m * ld0 + n], v);
+      out[m * ld + n] = v;
+    }
+  }
+  if (cross && out_amax) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    if ((threadIdx.x & 31) == 0 && amax > 0.f) atomicMax(out_amax, __float_as_uint(amax));
+  }
+}
+
 int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long N, long long K, const GemmEpilogue& ep,
             float* out, long long ld_out, void* ws, size_t ws_bytes, cudaStream_t st) {
-  GtPlan pl; gt_plan(M, N, K, ep.mode, pl);
+  GtPlan pl; gt_plan(M, N, K, pl);
   if (!ws || ws_bytes < pl.total) { set_error("gemm_tc: workspace too small"); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
   TFRS_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "gemm_tc: workspace must be 16-byte aligned");
   TFRS_CHECK_ARG(N < (1ll << 31) && M < (1ll << 31), "gemm_tc: M / N too large");
@@ -231,21 +280,24 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
   p.aimg = w8 + pl.o_aimg; p.bimg = w8 + pl.o_bimg; p.ast = ast; p.bst = bst;
   p.kb_total = pl.kb; p.n_mb = pl.n_mb; p.n_nt = pl.n_nt; p.n_kc = pl.n_kc; p.M = M; p.N = N;
   p.e0 = ep.e0; p.ld0 = ep.ld0; p.e1 = ep.e1; p.ld1 = ep.ld1; p.bias = ep.bias; p.diag = ep.diag; p.prod = ep.prod;
-  if (pl.n_kc > 1) {   // long reduction (the batch): chunked accumulation chains, fixed-order sum of the partials
+  if (ep.mode == GEMM_EPI_CROSS && ep.out_amax) TFRS_CUDA(cudaMemsetAsync(ep.out_amax, 0, sizeof(unsigned int), st));
+  if (pl.n_kc > 1) {   // long reduction: chunked accumulation chains, fixed-order sum of the partials, then the epilogue
     p.out = (float*)(w8 + pl.o_partial); p.ld_out = N;
     rc = sg_launch(SG_DW, p, st);
     if (rc) return rc;
-    if (ep.mode != GEMM_EPI_DENSE) return reduce_parts(p.out, M, N, pl.n_kc, out, ld_out, st);
-    // bias + activation applied to the reduced sum
-    sg_reduce_chunks_dense_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.bias, ep.act, out, ep.prod,
-                                                                                   ld_out);
+    if (ep.mode == GEMM_EPI_PLAIN) return reduce_parts(p.out, M, N, pl.n_kc, out, ld_out, st);
+    const unsigned grid = (unsigned)ceil_div(M * N, 256);
+    if (ep.mode == GEMM_EPI_DENSE)   // bias + activation applied to the reduced sum
+      sg_reduce_chunks_dense_kernel<<<grid, 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.bias, ep.act, out, ep.prod, ld_out);
+    else
+      sg_reduce_chunks_cross_dx_kernel<<<grid, 256, 0, st>>>(p.out, M, N, pl.n_kc, ep.mode == GEMM_EPI_CROSS, ep.e0, ep.ld0, ep.e1,
+                                                             ep.ld1, ep.bias, ep.diag, ep.prod, out, ld_out, ep.out_amax);
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }
   p.out = out; p.ld_out = ld_out;
   if (ep.mode == GEMM_EPI_DENSE) return sg_launch(SG_DENSE + ep.act, p, st);
   if (ep.mode == GEMM_EPI_CROSS) {
-    if (ep.out_amax) TFRS_CUDA(cudaMemsetAsync(ep.out_amax, 0, sizeof(unsigned int), st));
     p.out_amax = ep.out_amax;
     return sg_launch(SG_CROSS, p, st);
   }

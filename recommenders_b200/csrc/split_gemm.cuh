@@ -13,11 +13,12 @@ enum { GEMM_EPI_PLAIN = 0, GEMM_EPI_DX = 1, GEMM_EPI_CROSS = 2, GEMM_EPI_DENSE =
 // PLAIN: C = acc.   DX: C = acc + diag * e0 + e1.   CROSS: pv = acc + bias + diag * e1; prod = pv; C = e0 * pv + e1
 // (ld0 == ld1 == ld_out); out_amax (nullable, device) receives max |C| as float bits.
 // DENSE: z = acc + bias; C = act(z) (act = TFRS_ACT_*); prod = z when act is sigmoid (nullable).
-// PLAIN and DENSE accumulate K > 1024 in chunks of 1024 summed in fixed order; DX and CROSS run one chain over any K.
+// Every mode accumulates K > 1024 in chunks of 1024 (the tensor core's fp32 adder truncates, so one long chain drifts: a
+// full-rank Cross at D = 4096 missed the 1e-5 bar), summed in fixed order before the epilogue; K <= 1024 is one launch.
 struct GemmEpilogue { int mode; const float* e0; long long ld0; const float* e1; long long ld1; const float* bias; float diag; float* prod;
                       int act; unsigned int* out_amax = nullptr; };
-// workspace of one gemm_tc call with epilogue `mode` (the default, PLAIN, is an upper bound for every mode)
-size_t gemm_tc_workspace(long long M, long long N, long long K, int mode = GEMM_EPI_PLAIN);
+// workspace of one gemm_tc call (the same for every epilogue)
+size_t gemm_tc_workspace(long long M, long long N, long long K);
 int gemm_tc(const GemmOperand& A, const GemmOperand& B, long long M, long long N, long long K, const GemmEpilogue& ep,
             float* out, long long ld_out, void* ws, size_t ws_bytes, cudaStream_t st);
 

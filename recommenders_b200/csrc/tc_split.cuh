@@ -14,7 +14,9 @@ constexpr int CX_TARGET_EXP = 14;
 
 struct CxStats { unsigned int amax_bits; int exp; int pad0, pad1; };
 
-// max |element| of a [rows, D] matrix with row stride ld (one warp per row: coalesced, no index division)
+// max |element| over the FINITE elements of a [rows, D] matrix with row stride ld (one warp per row: coalesced, no index
+// division).  Inf and NaN are left out (finite_abs): the rescale then fits the finite data, and a non-finite element spoils
+// only the products of its own row or column (its hi is Inf or NaN, its lo NaN), as it would in fp32.
 static __global__ void __launch_bounds__(256)
 cx_amax_kernel(const float* __restrict__ src, long long rows, int D, long long ld, CxStats* __restrict__ st) {
   const int lane = threadIdx.x & 31;
@@ -23,7 +25,7 @@ cx_amax_kernel(const float* __restrict__ src, long long rows, int D, long long l
   float a = 0.f;
   for (long long r = warp; r < rows; r += nwarps) {
     const float* p = src + r * ld;
-    for (int c = lane; c < D; c += 32) a = fmaxf(a, fabsf(p[c]));
+    for (int c = lane; c < D; c += 32) a = fmaxf(a, finite_abs(p[c]));
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
