@@ -195,6 +195,19 @@ tc_qprep_kernel(const float* __restrict__ q, long long Q, long long Qp, int d, i
 // ------------------------------------------------------------------------------------------------
 enum { MODE_SAMPLE = 0, MODE_FILTER = 1 };
 
+// A/B ablations of the FILTER pass, timed by tools/filter_probe.py.  They exist only in the debug libraries that
+// `python -m recommenders_b200.build --debug-switches VARIANT` writes; the product library is always FILTER_FULL.
+// A call with an ablated pass stops after it and leaves its outputs unwritten: only the stage times
+// (tfrs_profile_read) mean anything.
+//   FILTER_NO_EMIT      hit test and octet mask computed, nothing stored
+//   FILTER_NO_EPILOGUE  the accumulators XOR-folded into one live word (ptxas deletes MMAs whose results are never read)
+enum { FILTER_FULL = 0, FILTER_NO_EMIT = 1, FILTER_NO_EPILOGUE = 2 };
+#if defined(TFRS_DEBUG_SWITCHES) && defined(TFRS_FILTER_ABLATION)
+constexpr int FILTER_ABLATION = TFRS_FILTER_ABLATION;
+#else
+constexpr int FILTER_ABLATION = FILTER_FULL;
+#endif
+
 struct ScanParams {
   const unsigned char* qimg;    // query tile image  [2*nqb tiles][KB][16 KB]
   const unsigned char* cimg;    // corpus tile image [n_tiles][KB][16 KB]
@@ -272,6 +285,10 @@ tc_scan_kernel(const ScanParams p) {
   }
   const unsigned int cap = (unsigned int)p.cap_part;
   unsigned int cnt[4] = {0u, 0u, 0u, 0u}, ovf = 0u;      // segment s = (row rr, column half h) = 2 rr + h
+  unsigned int sink = 0u;                                // what an ablated FILTER epilogue keeps live
+  long long seg_base[2];                                 // first record of segment (row rr, half 0); half 1 follows it
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) seg_base[rr] = ((row_a + 8 * rr) * p.parts + part) * 2 * (long long)cap;
   float binm[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
   int in_group = 0, bin_out = 0;
 
@@ -326,8 +343,14 @@ tc_scan_kernel(const ScanParams p) {
     } else {
       // Common path: a max tree over each row's 16 scores, one compare per row and one warp vote.  A warp of 16 rows meets
       // a survivor in about one half tile in two.  Only then each lane marks the octets (row rr, column group j) where one
-      // of its two scores passes, one warp-wide OR leaves the octets any lane hit, and those take a ballot, which makes the
-      // decision quad-uniform; each lane of a surviving octet stores its two scores, the quad leader the octet's first index.
+      // of its two scores passes.  An octet belongs to one row and its 8 columns to the 4 lanes of one quad, so an OR over
+      // the quad (two shuffles) makes the decision quad-uniform, with no warp-wide vote: each lane of a surviving octet
+      // stores its two scores, the quad leader the octet's first index, in ascending column order within the segment.
+      if (FILTER_ABLATION == FILTER_NO_EPILOGUE) {   // all 32 registers read: with one, ptxas serializes the wgmma (C7511)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) sink ^= __float_as_uint(acc[i]);
+        return;
+      }
       float pm[2][8];
       bool pass = false;
 #pragma unroll
@@ -344,24 +367,33 @@ tc_scan_kernel(const ScanParams p) {
         for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
           for (int j = 0; j < 8; ++j) mine |= (pm[rr][j] >= thr[rr]) ? (1u << (8 * rr + j)) : 0u;
-        const unsigned int hit = __reduce_or_sync(0xffffffffu, mine);
+        if (FILTER_ABLATION == FILTER_NO_EMIT) { sink |= mine; return; }
+        mine |= __shfl_xor_sync(0xffffffffu, mine, 1);
+        mine |= __shfl_xor_sync(0xffffffffu, mine, 2);
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
-          const long long seg_row = ((row_a + 8 * rr) * p.parts + part) * 2 + H;
+          const int s = 2 * rr + H;   // compile-time: cnt[] stays in registers
+          unsigned int m8 = (mine >> (8 * rr)) & 0xFFu;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (!((hit >> (8 * rr + j)) & 1u)) continue;   // warp-uniform
-            const unsigned int vote = __ballot_sync(0xffffffffu, (mine >> (8 * rr + j)) & 1u);
-            if ((vote >> (lane & ~3)) & 0xFu) {
-              const int s = 2 * rr + H;
-              if (cnt[s] < cap) {
-                const long long seg = seg_row * p.cap_part + cnt[s];
-                reinterpret_cast<float2*>(p.cand_s + seg * 8)[lane & 3] = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
-                if (quad_leader) p.cand_i[seg] = (unsigned int)(col0 + 64 * H + 8 * j);
-                ++cnt[s];
-              } else {
-                ovf |= 1u << s;
-              }
+          for (int t = 0; t < 8; ++t) {   // the set octets of this row in ascending order (quad-uniform trip count)
+            if (!m8) break;
+            const int j = __ffs(m8) - 1;
+            m8 &= m8 - 1u;
+            // the lane's score pair of octet j, selected by the bits of j (a runtime index would put acc in local memory)
+            float a[8], b[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) { a[u] = acc[4 * u + 2 * rr]; b[u] = acc[4 * u + 2 * rr + 1]; }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) { a[u] = (j & 1) ? a[2 * u + 1] : a[2 * u]; b[u] = (j & 1) ? b[2 * u + 1] : b[2 * u]; }
+#pragma unroll
+            for (int u = 0; u < 2; ++u) { a[u] = (j & 2) ? a[2 * u + 1] : a[2 * u]; b[u] = (j & 2) ? b[2 * u + 1] : b[2 * u]; }
+            if (cnt[s] < cap) {
+              const long long seg = seg_base[rr] + (H ? cap : 0u) + cnt[s];
+              reinterpret_cast<float2*>(p.cand_s + seg * 8)[lane & 3] = make_float2((j & 4) ? a[1] : a[0], (j & 4) ? b[1] : b[0]);
+              if (quad_leader) p.cand_i[seg] = (unsigned int)(col0 + 64 * H + 8 * j);
+              ++cnt[s];
+            } else {
+              ovf |= 1u << s;
             }
           }
         }
@@ -425,7 +457,8 @@ tc_scan_kernel(const ScanParams p) {
   } else if (quad_leader) {
 #pragma unroll
     for (int s = 0; s < 4; ++s)
-      p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] = ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
+      p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] =
+          FILTER_ABLATION != FILTER_FULL ? sink : ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
   }
 }
 
@@ -1152,6 +1185,7 @@ static int run_call(const Call& c) {
   rc = launch_scan_mode(pl, sp, st, MODE_FILTER);
   if (rc) return rc;
   prof_mark(st, 3);
+  if (FILTER_ABLATION != FILTER_FULL) { prof_mark(st, 4); return TFRS_OK; }   // no records: the outputs are not written
   // (3) exact re-scoring + final order (a warp per query); (4) exact fallback for the rows that asked for it
   FinParams fp{};
   fp.q = c.q; fp.corpus = c.corpus; fp.d = c.d; fp.k = c.k; fp.index_offset = c.index_offset; fp.N = c.N; fp.Q = c.Q;
