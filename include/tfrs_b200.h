@@ -327,6 +327,28 @@ int tfrs_clippy_adagrad_dense_f32(float* const* vars, const float* const* grads,
                                   void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K10  Adam with tf-keras's legacy rules (optimizer_v2/adam.py).  The caller computes, per step,
+ *   alpha = lr * sqrt(1 - beta2^t) / (1 - beta1^t)   (t = the optimizer's iterations + 1)
+ * and the kernels use omb1 = 1 - beta1 and omb2 = 1 - beta2 in fp32.  Every step one IEEE fp32 operation:
+ *   dense (_resource_apply_dense):  m' = m + (g - m)*omb1 ;  v' = v + (g*g - v)*omb2 ;
+ *                                   var' = var - (m'*alpha) / (sqrt(v') + eps)
+ *   sparse (_resource_apply_sparse), g = the row's gradient with duplicate ids summed in order of occurrence (as K4):
+ *     touched rows:  m' = m*beta1 + g*omb1 ;  v' = v*beta2 + (g*g)*omb2
+ *     other rows:    m' = m*beta1 ;  v' = v*beta2          (lazy != 0: other rows keep var, m and v bit for bit)
+ *     every updated row:  var' = var - (alpha*m') / (sqrt(v') + eps)
+ * Sparse: one table per call, the contract of tfrs_sparse_adagrad_f32 (I32/I64 ids, out-of-range ids skipped,
+ * n < 2^24, d <= 1024, rows < 2^40); n == 0 is allowed (with lazy == 0 every row still decays).  Deterministic.
+ * Dense: every variable of one optimizer in one call; vars / grads / ms / vs / numels are HOST arrays of nvars device
+ * pointers and element counts.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_sparse_adam_workspace_bytes(int64_t n, int64_t rows);
+int tfrs_sparse_adam_f32(float* table, float* m, float* v, int64_t rows, int d, const void* ids, int ids_dtype,
+                         int64_t n, const float* grad_rows, float alpha, float beta1, float beta2, float eps,
+                         int lazy, void* ws, size_t ws_bytes, void* stream);
+int tfrs_adam_dense_f32(float* const* vars, const float* const* grads, float* const* ms, float* const* vs,
+                        const int64_t* numels, int nvars, float alpha, float beta1, float beta2, float eps, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K5  DCN-v2 cross layer (layers/feature_interaction/dcn.py:176-186, full-rank, no preactivation):
  *   out = x0 * (x . W + bias + diag_scale * x) + x ,  W [D,D] in Keras [in,out] layout.
  * x0, x, out have row stride ld (>= D).  `prod` (nullable) receives x.W + bias + diag_scale*x for

@@ -6,8 +6,8 @@
 //     sums each run's duplicate rows in order of occurrence, saves the summed row in the workspace (slot = the run's first
 //     sorted position) and folds the run's per-element ratios into the factor; pass B updates every run head's row from
 //     the saved sum.  Pass A only reads the table and accumulator, pass B does every write.
-//   dense (all dense variables of one optimizer): descriptors by value in the kernel parameters (up to CD_MAX variables
-//     per launch), blocks of CD_CHUNK elements of one variable; one init, one pass A and one pass B launch per batch.
+//   dense (all dense variables of one optimizer): the multi-tensor launches of multi_tensor.cuh (descriptors by value in
+//     the kernel parameters, up to CD_MAX variables per launch); one init, one pass A and one pass B launch per batch.
 // The factor is an atomicMin on the bit pattern of a non-negative float: a minimum is order-independent, so the result is
 // bitwise reproducible.  NaN ratios do not lower it (fminf).  Every arithmetic step is a single IEEE fp32 op (no FMA
 // contraction), stated identically by the fp32 restatement the tests use (tests/, clippy_oracle).
@@ -15,6 +15,7 @@
 //                    pass B  3*u*d*4 (summed rows, var, acc) + 2*u*d*4 (var, acc written).
 //            dense:  pass A  3*N*4 ; pass B  3*N*4 + 2*N*4, N = elements of all variables.
 #include "adagrad.cuh"
+#include "multi_tensor.cuh"
 
 namespace tfrs {
 
@@ -95,47 +96,34 @@ cl_sparse_apply(const unsigned long long* __restrict__ keys, long long n, const 
 // ---- dense -----------------------------------------------------------------------------------------------------------
 // 32 B per descriptor + 4 B of block offset: 896 variables and the scalars stay under the 32764 bytes of kernel
 // parameters that CUDA 12.1+ allows on sm_90.
-constexpr int CD_MAX = 896, CD_THREADS = 256, CD_PER_THREAD = 4, CD_CHUNK = CD_THREADS * CD_PER_THREAD;
+constexpr int CD_MAX = 896;
 struct CdVar { float* var; const float* grad; float* acc; long long numel; };
-struct CdBatch {
-  CdVar v[CD_MAX];
-  unsigned int block0[CD_MAX + 1];   // first block of each variable; block0[nvars] = grid size
-  int nvars;
-};
+using CdBatch = MtBatch<CdVar, CD_MAX>;
 static_assert(sizeof(CdBatch) + sizeof(ClippyArgs) + 2 * sizeof(void*) <= 32764, "kernel parameters over the sm_90 limit");
 
-__device__ __forceinline__ int cd_find(const CdBatch& b) {   // the variable of this block: last v with block0[v] <= blockIdx.x
-  int lo = 0, hi = b.nvars - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (b.block0[mid] <= blockIdx.x) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
-__global__ void __launch_bounds__(CD_THREADS)
+__global__ void __launch_bounds__(MT_THREADS)
 cl_dense_factor(const __grid_constant__ CdBatch b, const ClippyArgs k, float* __restrict__ factors) {
-  const int v = cd_find(b);
+  const int v = mt_find(b);
   const CdVar& x = b.v[v];
-  const long long e0 = (long long)(blockIdx.x - b.block0[v]) * CD_CHUNK + threadIdx.x;
+  const long long e0 = mt_first(b, v);
   float m = 1.f;
 #pragma unroll
-  for (int u = 0; u < CD_PER_THREAD; ++u) {
-    const long long e = e0 + u * CD_THREADS;
+  for (int u = 0; u < MT_PER_THREAD; ++u) {
+    const long long e = e0 + u * MT_THREADS;
     if (e < x.numel) m = fminf(m, cl_ratio(x.grad[e], x.var[e], x.acc[e], k));
   }
   cl_fold_min(m, factors + v);
 }
 
-__global__ void __launch_bounds__(CD_THREADS)
+__global__ void __launch_bounds__(MT_THREADS)
 cl_dense_apply(const __grid_constant__ CdBatch b, const ClippyArgs k, const float* __restrict__ factors) {
-  const int v = cd_find(b);
+  const int v = mt_find(b);
   const CdVar& x = b.v[v];
   const float scale = factors[v];
-  const long long e0 = (long long)(blockIdx.x - b.block0[v]) * CD_CHUNK + threadIdx.x;
+  const long long e0 = mt_first(b, v);
 #pragma unroll
-  for (int u = 0; u < CD_PER_THREAD; ++u) {
-    const long long e = e0 + u * CD_THREADS;
+  for (int u = 0; u < MT_PER_THREAD; ++u) {
+    const long long e = e0 + u * MT_THREADS;
     if (e < x.numel) {
       float val = x.var[e], a = x.acc[e];
       cl_apply(x.grad[e], val, a, k, scale);
@@ -221,29 +209,14 @@ extern "C" int tfrs_clippy_adagrad_dense_f32(float* const* vars, const float* co
   float* factors = clipping_factors_out ? clipping_factors_out : (float*)ws;
   cl_fill_one<<<(unsigned)ceil_div(nvars, 256), 256, 0, st>>>(factors, nvars);
   TFRS_LAUNCH_CHECK();
-  static thread_local CdBatch b;   // 32 KB: off the stack
-  for (int v0 = 0; v0 < nvars;) {
-    // one batch: up to CD_MAX variables and at most 2^31 - 1 blocks
-    b.nvars = 0;
-    long long blocks = 0;
-    int v = v0;
-    for (; v < nvars && b.nvars < CD_MAX; ++v) {
-      const long long nb = ceil_div(numels[v], CD_CHUNK);
-      if (b.nvars > 0 && blocks + nb > 0x7FFFFFFFll) break;
-      TFRS_CHECK_ARG(nb <= 0x7FFFFFFFll, "clippy_adagrad_dense: variable %d too large", v);
-      b.v[b.nvars] = CdVar{vars[v], grads[v], accums[v], numels[v]};
-      b.block0[b.nvars] = (unsigned int)blocks;
-      blocks += nb;
-      ++b.nvars;
-    }
-    b.block0[b.nvars] = (unsigned int)blocks;
-    if (blocks > 0) {
-      cl_dense_factor<<<(unsigned)blocks, CD_THREADS, 0, st>>>(b, k, factors + v0);
-      TFRS_LAUNCH_CHECK();
-      cl_dense_apply<<<(unsigned)blocks, CD_THREADS, 0, st>>>(b, k, factors + v0);
-      TFRS_LAUNCH_CHECK();
-    }
-    v0 = v;
-  }
-  return TFRS_OK;
+  return mt_for_each_batch<CdVar, CD_MAX>(
+      nvars, numels, "clippy_adagrad_dense",
+      [&](int v) { return CdVar{vars[v], grads[v], accums[v], numels[v]}; },
+      [&](const CdBatch& b, unsigned blocks, int v0) {
+        cl_dense_factor<<<blocks, MT_THREADS, 0, st>>>(b, k, factors + v0);
+        TFRS_LAUNCH_CHECK();
+        cl_dense_apply<<<blocks, MT_THREADS, 0, st>>>(b, k, factors + v0);
+        TFRS_LAUNCH_CHECK();
+        return TFRS_OK;
+      });
 }

@@ -6,6 +6,7 @@ autograd tape.  No CPU fallback.
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import NamedTuple, Optional, Sequence, Tuple
 
 import torch
@@ -976,6 +977,65 @@ def clippy_adagrad_dense_(variables: Sequence[torch.Tensor], grads: Sequence[tor
       c_f(accumulator_relative_threshold), c_f(absolute_threshold),
       _clippy_flags(clip_accumulator_update, use_standard_accumulator_update), ptr(clipping_factors), ptr(ws), ws.numel(),
       stream()), "clippy_adagrad_dense")
+
+
+# ------------------------------------------------------------------------------------------------
+# K10 Adam
+# ------------------------------------------------------------------------------------------------
+def adam_alpha(learning_rate: float, beta_1: float, beta_2: float, t: int) -> float:
+  """The step size of Adam's step t (1-based): lr * sqrt(1 - beta_2^t) / (1 - beta_1^t), evaluated in float64 from the
+  fp32-rounded hyperparameters and rounded once to fp32."""
+  lr, b1, b2 = (c_f(x).value for x in (learning_rate, beta_1, beta_2))
+  return c_f(lr * math.sqrt(1.0 - b2 ** t) / (1.0 - b1 ** t)).value
+
+
+def sparse_adam_(table: torch.Tensor, m: torch.Tensor, v: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor,
+                 alpha: float, beta_1: float, beta_2: float, epsilon: float, lazy: bool = False) -> None:
+  """Adam step of one embedding table whose gradient rows `grad_rows` belong to the rows `ids` (duplicates summed in order
+  of occurrence, out-of-range ids skipped).  `alpha` is the step size of `adam_alpha`.  Not lazy: every row of the table
+  and of its slots `m` / `v` is updated (the untouched ones decay); lazy: only the touched rows."""
+  _f32_inplace(table, "table"); _f32_inplace(m, "m"); _f32_inplace(v, "v")
+  ids = require_cuda(ids, "ids").contiguous().view(-1)
+  g = f32c(grad_rows, "grad_rows")
+  if table.dim() != 2:
+    raise ValueError(f"sparse_adam_: table must be 2-D, got {tuple(table.shape)}")
+  n = ids.numel(); rows, d = table.shape
+  for name, s in (("m", m), ("v", v)):
+    if s.shape != table.shape or s.device != table.device:
+      raise ValueError(f"sparse_adam_: {name} must be {tuple(table.shape)} on {table.device}, got {tuple(s.shape)} on {s.device}")
+  if g.shape != (n, d):
+    raise ValueError(f"sparse_adam_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
+  if ids.device != table.device or g.device != table.device:
+    raise ValueError("sparse_adam_: ids and grad_rows must live on the table's device")
+  ws = workspace(lib().tfrs_sparse_adam_workspace_bytes(n, rows), table.device, "adam")
+  check(lib().tfrs_sparse_adam_f32(
+      ptr(table), ptr(m), ptr(v), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(alpha), c_f(beta_1),
+      c_f(beta_2), c_f(epsilon), int(bool(lazy)), ptr(ws), ws.numel(), stream()), "sparse_adam")
+
+
+def adam_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], ms: Sequence[torch.Tensor],
+                vs: Sequence[torch.Tensor], alpha: float, beta_1: float, beta_2: float, epsilon: float) -> None:
+  """Adam step of a list of dense variables and their slots `ms` / `vs` in one multi-tensor call; `alpha` is the step
+  size of `adam_alpha`."""
+  nv = len(variables)
+  if len(grads) != nv or len(ms) != nv or len(vs) != nv:
+    raise ValueError("adam_dense_: variables, grads, ms and vs must have the same length")
+  if nv == 0:
+    return
+  dev = variables[0].device
+  gs = []
+  for i, (x, g, m, v) in enumerate(zip(variables, grads, ms, vs)):
+    _f32_inplace(x, f"variables[{i}]"); _f32_inplace(m, f"ms[{i}]"); _f32_inplace(v, f"vs[{i}]")
+    g = f32c(g, f"grads[{i}]")
+    if any(t.device != dev for t in (x, g, m, v)):
+      raise ValueError("adam_dense_: every tensor must live on one device")
+    if g.shape != x.shape or m.shape != x.shape or v.shape != x.shape:
+      raise ValueError(f"adam_dense_: grads[{i}] / ms[{i}] / vs[{i}] must have the shape {tuple(x.shape)}")
+    gs.append(g)
+  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
+  numels = (ctypes.c_int64 * nv)(*[x.numel() for x in variables])
+  check(lib().tfrs_adam_dense_f32(arr(variables), arr(gs), arr(ms), arr(vs), numels, nv, c_f(alpha), c_f(beta_1),
+                                  c_f(beta_2), c_f(epsilon), stream()), "adam_dense")
 
 
 # ------------------------------------------------------------------------------------------------

@@ -3,10 +3,12 @@ passes to `model.compile`, README.md:84: `tf.keras.optimizers.Adagrad(0.5)`).
 
 Keras defaults: initial_accumulator_value=0.1, epsilon=1e-7.  `eps_inside_sqrt=True` is the Keras-3 /
 tf-keras `optimizers.Adagrad` rule  var -= lr*g/sqrt(acc+eps); False is the legacy
-`optimizers.legacy.Adagrad` rule  var -= lr*g/(sqrt(acc)+eps)  (SURVEY.md A10 -- third-party, unpinned)."""
+`optimizers.legacy.Adagrad` rule  var -= lr*g/(sqrt(acc)+eps)  (SURVEY.md A10 -- third-party, unpinned).
+
+Adam: tf-keras's legacy `optimizers.legacy.Adam` rules on the K10 kernels (DESIGN.md A15)."""
 from __future__ import annotations
 
-from typing import Iterable, List, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -47,18 +49,15 @@ def clear_grads(tables: Sequence[Embedding], dense: Sequence[torch.Tensor]) -> N
     t._anchor.grad = None
 
 
-class _AccumulatorOptimizer:
-  """Variable discovery and per-variable accumulator slots shared by Adagrad and ClippyAdagrad."""
+class _SlotOptimizer:
+  """Variable discovery and per-variable slots shared by Adagrad, ClippyAdagrad and Adam."""
 
-  _ACC_ATTR = "_tfrs_adagrad_acc"
-
-  def __init__(self, initial_accumulator_value: float):
-    self.initial_accumulator_value = initial_accumulator_value
+  def __init__(self):
     self.iterations = 0
     self._module = None
     self._dense: List[torch.nn.Parameter] = []
     self._tables: List[Embedding] = []
-    self._acc = {}
+    self._slots = {}
 
   def bind(self, module: torch.nn.Module):
     """Attach to a model.  The variable lists are re-read on every step (`_refresh`), like the reference's
@@ -74,14 +73,15 @@ class _AccumulatorOptimizer:
     self._tables = embedding_tables(self._module)
     self._dense = dense_variables(self._module)
 
-  def _accum(self, owner, like: torch.Tensor) -> torch.Tensor:
-    """Accumulator slot of a variable, stored ON its owner object (an Embedding module or a Parameter) so it
-    lives and dies with it -- an id()-keyed dict would hand a recycled id the previous owner's state."""
-    a = getattr(owner, self._ACC_ATTR, None)
+  def _slot(self, owner, attr: str, like: torch.Tensor, value: float) -> torch.Tensor:
+    """The slot `attr` of a variable, filled with `value` when created, stored ON its owner object (an Embedding module
+    or a Parameter) so it lives and dies with it -- an id()-keyed dict would hand a recycled id the previous owner's
+    state."""
+    a = getattr(owner, attr, None)
     if a is None or a.shape != like.shape or a.device != like.device:
-      a = torch.full_like(like, self.initial_accumulator_value)
-      setattr(owner, self._ACC_ATTR, a)
-      self._acc[id(owner)] = a
+      a = torch.full_like(like, value)
+      setattr(owner, attr, a)
+      self._slots[(id(owner), attr)] = a
     return a
 
   def zero_grad(self):
@@ -107,11 +107,24 @@ class _AccumulatorOptimizer:
     raise NotImplementedError
 
   def variables(self) -> List[torch.Tensor]:
-    """The optimizer's state: one accumulator per variable it has updated."""
-    return list(self._acc.values())
+    """The optimizer's state: its slots of every variable it has updated."""
+    return list(self._slots.values())
+
+
+class _AccumulatorOptimizer(_SlotOptimizer):
+  """One accumulator slot per variable (Adagrad and ClippyAdagrad)."""
+
+  _ACC_ATTR = "_tfrs_adagrad_acc"
+
+  def __init__(self, initial_accumulator_value: float):
+    super().__init__()
+    self.initial_accumulator_value = initial_accumulator_value
+
+  def _accum(self, owner, like: torch.Tensor) -> torch.Tensor:
+    return self._slot(owner, self._ACC_ATTR, like, self.initial_accumulator_value)
 
   def state_dict(self):
-    return {"acc": {k: v.clone() for k, v in self._acc.items()}}
+    return {"acc": {k: v.clone() for (k, _), v in self._slots.items()}}
 
 
 class Adagrad(_AccumulatorOptimizer):
@@ -140,3 +153,53 @@ class Adagrad(_AccumulatorOptimizer):
       a.addcmul_(g, g)
       den = (a + self.epsilon).sqrt_() if self.eps_inside_sqrt else a.sqrt().add_(self.epsilon)
       p.addcdiv_(g, den, value=-self.learning_rate)
+
+
+class Adam(_SlotOptimizer):
+  """Adam with tf-keras's legacy rules (`tf.keras.optimizers.legacy.Adam`, optimizer_v2/adam.py; DESIGN.md section 2).
+  Dense variables take the dense rule.  An embedding table takes the sparse rule: every step decays `m` and `v` over
+  the whole table and moves every row whose `m` is nonzero, touched or not, like tf-keras's `_resource_apply_sparse` on
+  CPU / GPU.  With `lazy_embeddings=True` only the rows of the step's ids are updated and the other rows keep their
+  variable, `m` and `v` bit for bit, as TPU embedding engines do by default; for a large table that is the cheap choice.
+
+  The slots `m` and `v` start at zero.  `amsgrad=True` raises NotImplementedError."""
+
+  _M_ATTR = "_tfrs_adam_m"
+  _V_ATTR = "_tfrs_adam_v"
+
+  def __init__(self, learning_rate: float = 0.001, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7,
+               amsgrad: bool = False, lazy_embeddings: bool = False, name: str = "Adam"):
+    if amsgrad:
+      raise NotImplementedError("Adam: amsgrad=True is not supported")
+    super().__init__()
+    self.learning_rate = learning_rate
+    self.beta_1 = beta_1
+    self.beta_2 = beta_2
+    self.epsilon = epsilon
+    self.amsgrad = amsgrad
+    self.lazy_embeddings = lazy_embeddings
+    self.name = name
+
+  def _apply(self, tables, dense):
+    alpha = ops.adam_alpha(self.learning_rate, self.beta_1, self.beta_2, self.iterations + 1)
+    rule = dict(alpha=alpha, beta_1=self.beta_1, beta_2=self.beta_2, epsilon=self.epsilon)
+    for t in tables:
+      grads = t.pop_sparse_grads()
+      if not grads:
+        continue
+      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)   # one variable: the IndexedSlices of all its lookups
+      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
+      ops.sparse_adam_(t.weight, self._slot(t, self._M_ATTR, t.weight, 0.0), self._slot(t, self._V_ATTR, t.weight, 0.0),
+                       ids, rows, lazy=self.lazy_embeddings, **rule)
+    params = [p for p in dense if p.grad is not None]
+    if params:
+      ops.adam_dense_(params, [p.grad for p in params], [self._slot(p, self._M_ATTR, p, 0.0) for p in params],
+                      [self._slot(p, self._V_ATTR, p, 0.0) for p in params], **rule)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "learning_rate": self.learning_rate, "beta_1": self.beta_1, "beta_2": self.beta_2,
+            "epsilon": self.epsilon, "amsgrad": self.amsgrad, "lazy_embeddings": self.lazy_embeddings}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]) -> "Adam":
+    return cls(**config)
