@@ -141,14 +141,10 @@ int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out10);
 int tfrs_profile_enable(int on);
 int tfrs_profile_read(float* stage_ms, int* calls);
 
-/* K2m  merge n_lists per-shard/per-chunk [Q, k_in] lists (list-major: [n_lists, Q, k_in]) into the
- * best k_out = min(k_out, n_lists*k_in) per query (Streaming reduce :440-472; shard merge after the
- * all-gather).  Order = (score desc, index asc). */
-int tfrs_topk_merge(const float* scores, const int64_t* idx, int n_lists, int64_t Q, int k_in, int k_out,
-                    float* out_scores, int64_t* out_idx, void* stream);
-
-/* Same merge for lists that sit `list_stride_*` elements apart (e.g. the receive buffer of the single
- * all-gather, where every rank's block is [scores | indices]). */
+/* K2m  merge n_lists per-shard/per-chunk [Q, k_in] lists into the best k_out = min(k_out, n_lists*k_in) per query
+ * (Streaming reduce :440-472; shard merge after the all-gather).  Order = (score desc, index asc).  The lists sit
+ * `list_stride_*` elements apart: Q*k_in for a list-major [n_lists, Q, k_in] array, more in the receive buffer of the
+ * single all-gather, where every rank's block is [scores | indices]. */
 int tfrs_topk_merge_strided(const float* scores, const int64_t* idx, int64_t list_stride_scores,
                             int64_t list_stride_idx, int n_lists, int64_t Q, int k_in, int k_out,
                             float* out_scores, int64_t* out_idx, void* stream);

@@ -45,7 +45,6 @@ _SIGNATURES = {
     "tfrs_dot_interaction_bwd_f32": (c_i, [c_p, c_p, c_l, c_i, c_i, c_i, c_i, c_p, c_p]),
     "tfrs_profile_enable": (c_i, [c_i]),
     "tfrs_profile_read": (c_i, [c_p, c_p]),
-    "tfrs_topk_merge": (c_i, [c_p, c_p, c_i, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_topk_merge_strided": (c_i, [c_p, c_p, c_l, c_l, c_i, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_topk_merge_sorted_strided": (c_i, [c_p, c_p, c_l, c_l, c_i, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_comm_unique_id": (c_i, [c_p]),

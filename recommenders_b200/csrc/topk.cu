@@ -3,7 +3,7 @@
 //   tfrs_topk_scan_f32 : layers/factorized_top_k.py:603-605 (BruteForce.call) and :424-472
 //                        (Streaming's per-chunk top_k + running merge), chunk by chunk:
 //                        scores chunk = exact SGEMM (sgemm.cuh) -> per-row select (rowselect.cuh).
-//   tfrs_topk_merge    : Streaming.reduce (:440-472) / the shard merge after the all-gather.
+//   tfrs_topk_merge_strided : Streaming.reduce (:440-472) / the shard merge after the all-gather.
 #include "rowselect.cuh"
 #include "sgemm.cuh"
 
@@ -123,18 +123,6 @@ extern "C" int tfrs_topk_scan_f32(const float* q, int64_t Q, const float* corpus
     buf ^= 1;
   }
   return TFRS_OK;
-}
-
-extern "C" int tfrs_topk_merge(const float* scores, const int64_t* idx, int n_lists, int64_t Q, int k_in,
-                               int k_out, float* out_scores, int64_t* out_idx, void* stream) {
-  TFRS_CHECK_ARG(n_lists > 0 && Q >= 0 && k_in > 0 && k_out > 0, "topk_merge: bad shape");
-  TFRS_CHECK_ARG(k_out <= 2048, "topk_merge: k_out=%d > 2048", k_out);
-  if (Q == 0) return TFRS_OK;
-  TFRS_CHECK_ARG(scores && idx && out_scores && out_idx, "topk_merge: NULL pointer");
-  long long tot = (long long)n_lists * k_in;
-  int ko = (int)(k_out < tot ? k_out : tot);
-  MergeProvider prov{scores, (const long long*)idx, n_lists, Q, k_in, Q * k_in, Q * k_in};
-  return launch_row_topk(prov, Q, ko, out_scores, (long long*)out_idx, k_out, (cudaStream_t)stream);
 }
 
 extern "C" int tfrs_topk_merge_strided(const float* scores, const int64_t* idx, int64_t list_stride_scores,

@@ -190,6 +190,11 @@ class TopK(torch.nn.Module, abc.ABC):
     x, y = self(queries=queries, k=adjusted_k)
     return _exclude(x, y, exclude=exclusions, k=k)
 
+  def in_top_k_count(self, queries: Tensor, positive_scores: Tensor, k: int) -> Optional[Tensor]:
+    """min(k, #{candidates scoring strictly above positive_scores[q]}) per query (int32 [Q]) when the layer can count
+    without retrieving a top-k list; None when it cannot, and the caller counts on `self(queries, k=k)` instead."""
+    return None
+
   @abc.abstractmethod
   def is_exact(self) -> bool:
     raise NotImplementedError()
@@ -296,20 +301,6 @@ class Streaming(TopK):
     raise NotImplementedError("The streaming top k class only accepts datasets. "
                               "Please call `index_from_dataset` instead.")
 
-  def _scan_chunk(self, queries: Tensor, emb: Tensor, k: int, counter: int, state):
-    """state + top-k of one chunk -> new state."""
-    rows, d = int(emb.shape[0]), int(emb.shape[1])
-    if (self.use_tensor_cores and rows >= ops.TC_MIN_N and d <= 128 and state[0].shape[1] in (0, k) and
-        ops.tc_supported(queries.shape[0], rows, d, k)):
-      image = ops.index_build(emb, reuse_slot="stream_index")
-      s, i = ops.topk_tc(queries, emb, image, k, index_offset=counter)
-      if state[0].shape[1] == 0:
-        return s, i
-      return ops.topk_merge_sorted(torch.stack([state[0], s]), torch.stack([state[1], i]), k)
-    # the exact scan kernel takes the carried state and numbers the rows with the running counter
-    # (enumerate_rows, :474-485)
-    return ops.topk_scan(queries, emb, k, index_offset=counter, state=state)
-
   def _run(self, queries, k: int):
     """-> (scores [Q,k'], running row indices [Q,k'] i64, identifier chunks or None)."""
     if self._candidates is None:
@@ -337,7 +328,10 @@ class Streaming(TopK):
         emb = st.stage([p if p.is_cuda else p.to(torch.float32) for p in pending])
       else:
         emb = pending[0] if len(pending) == 1 else torch.cat(pending, 0)
-      state = self._scan_chunk(queries, ops.f32c(emb, "candidates"), k, counter, state)
+      # state + top-k of the chunk, its rows numbered with the running counter (enumerate_rows, :474-485); the chunk's
+      # tensor-core image is built in a per-stream scratch slot
+      state = ops.topk(queries, ops.f32c(emb, "candidates"), k, image="stream_index" if self.use_tensor_cores else None,
+                       index_offset=counter, state=state)
       if staged:
         self._stager.release()
       counter += int(emb.shape[0])
@@ -446,20 +440,29 @@ class BruteForce(TopK):
       self._tc_index = ops.index_build(cands)
 
   def _tc_ok(self, Q: int, k: int) -> bool:
-    return self._tc_index is not None and ops.tc_supported(Q, self._candidates.shape[0], self._candidates.shape[1], k)
+    return self._tc_index is not None and ops.uses_tc_scan(Q, self._candidates.shape[0], self._candidates.shape[1], k)
 
   def _local_topk(self, queries: Tensor, k: int, offset: int, out=None):
-    if self._tc_ok(queries.shape[0], k):
-      return ops.topk_tc(queries, self._candidates, self._tc_index, k, index_offset=offset, out=out)
     n, d = self._candidates.shape
-    if self.use_tensor_cores and n >= ops.TC_MIN_N and not BruteForce._warned_slow_path:
+    if (self.use_tensor_cores and n >= ops.TC_MIN_N and not BruteForce._warned_slow_path and
+        not self._tc_ok(queries.shape[0], k)):
       # same results, ~20x slower: say so once instead of silently leaving the tensor-core path
       BruteForce._warned_slow_path = True
       import warnings
       warnings.warn(f"BruteForce: a {n} x {d} corpus with k={k} is outside the tensor-core scan's range (d <= 128, k <= "
                     f"{ops.TC_MAX_K}, corpus >= ~256*k rows); running the exact CUDA-core scan instead (same results, "
                     "roughly 20x slower).", RuntimeWarning, stacklevel=3)
-    return ops.topk_scan(queries, self._candidates, k, index_offset=offset, out=out)
+    return ops.topk(queries, self._candidates, k, image=self._tc_index, index_offset=offset, out=out)
+
+  def in_top_k_count(self, queries: Tensor, positive_scores: Tensor, k: int) -> Optional[Tensor]:
+    """Counted inside the tensor-core scan (`tfrs_topk_tc_count_f32`) when the index is unsharded and has no query
+    model, so `queries` are already the embeddings the corpus is scored against."""
+    if self._candidates is None or self._shard is not None or self.query_model is not None:
+      return None
+    k = min(k, self._candidates.shape[0])
+    if not self._tc_ok(queries.shape[0], k):
+      return None
+    return ops.topk_tc_count(queries, self._candidates, self._tc_index, k, positive_scores)
 
   def call(self, queries, k: Optional[int] = None):
     k = k if k is not None else self._k

@@ -114,8 +114,8 @@ class FactorizedTopK(Factorized):
   """Top-K categorical accuracy across the candidates surfaced by a retrieval layer (:52-194).
 
   Score branch (no `true_candidate_ids`): in_top_k(target = the positive) only needs  c_q = #{candidates scoring
-  strictly above the positive}, clipped at max(ks).  With a tensor-core `BruteForce` index that count comes straight
-  out of the scan (`tfrs_topk_tc_count_f32`: no top-K list, no sort); otherwise it is counted on the retrieved list.
+  strictly above the positive}, clipped at max(ks).  When the layer can count inside its scan (`TopK.in_top_k_count`,
+  e.g. a tensor-core `BruteForce` index: no top-K list, no sort) it does; otherwise it is counted on the retrieved list.
   Either way ONE kernel folds  w_q * [c_q < k]  for every k into a device accumulator -- update_state never
   synchronises with the host."""
 
@@ -173,12 +173,8 @@ class FactorizedTopK(Factorized):
       # positive score with the same canonical chain as the retrieved scores (:133-134)
       positive_scores = ops.rowwise_dot(query_embeddings, true_candidate_embeddings)
       layer = self._candidates
-      fused = (isinstance(layer, ftk.BruteForce) and layer._shard is None and layer.query_model is None and
-               layer._candidates is not None and layer._tc_ok(query_embeddings.shape[0], min(kmax, layer._candidates.shape[0])))
-      if fused:    # count inside the scan: no top-K list at all
-        count = ops.topk_tc_count(query_embeddings, layer._candidates, layer._tc_index, min(kmax, layer._candidates.shape[0]),
-                                  positive_scores)
-      else:
+      count = layer.in_top_k_count(query_embeddings, positive_scores, kmax)
+      if count is None:
         top_k_predictions, _ = layer(query_embeddings, k=kmax)
         count = ops.count_above(top_k_predictions, positive_scores)
       ops.hits_accumulate(count, positive_scores, w, self._ks, acc)

@@ -251,6 +251,15 @@ def index_build(corpus: torch.Tensor, reuse_slot: Optional[str] = None) -> torch
   return buf
 
 
+def _tc_query_chunks(q: torch.Tensor, N: int, k_ws: int):
+  """(lo, hi, workspace) for each run of at most TC_MAX_Q_PER_CALL queries: the tensor-core workspace (bin maxima and
+  survivor records) grows with Q, so larger batches run chunk by chunk, each workspace sized for k_ws per query."""
+  Q, d = q.shape
+  for lo in range(0, Q, TC_MAX_Q_PER_CALL):
+    hi = min(Q, lo + TC_MAX_Q_PER_CALL)
+    yield lo, hi, workspace(lib().tfrs_topk_tc_workspace_bytes(hi - lo, N, d, k_ws), q.device, "tc")
+
+
 def topk_tc(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor, k: int, index_offset: int = 0,
             out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
   """wgmma screening + exact rescoring; bit-identical to topk_scan."""
@@ -261,18 +270,40 @@ def topk_tc(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor, k: i
     out_i = torch.empty((Q, k), dtype=torch.int64, device=q.device)
   else:
     out_s, out_i = out
-  if Q == 0:
-    return out_s, out_i
-  if Q > TC_MAX_Q_PER_CALL:  # bound the workspace (bin maxima + survivor records scale with Q): query chunks
-    for lo in range(0, Q, TC_MAX_Q_PER_CALL):
-      hi = min(Q, lo + TC_MAX_Q_PER_CALL)
-      topk_tc(q[lo:hi], corpus, index_buf, k, index_offset, out=(out_s[lo:hi], out_i[lo:hi]))
-    return out_s, out_i
-  wsb = lib().tfrs_topk_tc_workspace_bytes(Q, N, d, k)
-  ws = workspace(wsb, q.device, "tc")
-  check(lib().tfrs_topk_tc_f32(ptr(q), Q, ptr(corpus), ptr(index_buf), N, d, k, index_offset, ptr(out_s),
-                               ptr(out_i), ptr(ws), ws.numel(), stream()), "topk_tc")
+  for lo, hi, ws in _tc_query_chunks(q, N, k):
+    check(lib().tfrs_topk_tc_f32(ptr(q[lo:hi]), hi - lo, ptr(corpus), ptr(index_buf), N, d, k, index_offset, ptr(out_s[lo:hi]),
+                                 ptr(out_i[lo:hi]), ptr(ws), ws.numel(), stream()), "topk_tc")
   return out_s, out_i
+
+
+def tc_supported(Q: int, N: int, d: int, k: int) -> bool:
+  """True when (Q, N, d, k) is inside the tensor-core kernels' range (d <= 128, k <= TC_MAX_K, N >= ~256*k)."""
+  return lib().tfrs_topk_tc_workspace_bytes(Q, N, d, k) > 0
+
+
+def uses_tc_scan(Q: int, N: int, d: int, k: int) -> bool:
+  """True when a top-k of Q queries over an N x d corpus takes the tensor-core scan.  TC_MIN_N is this module's policy,
+  not the kernels': smaller corpora take the exact scan even inside the kernels' range."""
+  return N >= TC_MIN_N and tc_supported(Q, N, d, k)
+
+
+def topk(q: torch.Tensor, corpus: torch.Tensor, k: int, image=None, index_offset: int = 0,
+         state: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+         out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Exact top-k of the corpus rows, numbered from index_offset, merged with the carried `state` ([Q, w] scores and
+  indices): scores descending, ties -> lower index.  `image` is the corpus's tensor-core image (index_build), the name
+  of a scratch slot to build it in, or None.  With an image, uses_tc_scan(Q, N, d, k) and a state of width 0 or k,
+  the tensor-core scan runs (a k-wide state is merged in by the sorted-list merge); otherwise topk_scan does."""
+  N, d = corpus.shape
+  st_k = 0 if state is None else state[0].shape[1]
+  if image is None or st_k not in (0, k) or not uses_tc_scan(q.shape[0], N, d, k):
+    return topk_scan(q, corpus, k, index_offset=index_offset, state=state, out=out)
+  if isinstance(image, str):
+    image = index_build(corpus, reuse_slot=image)
+  s, i = topk_tc(q, corpus, image, k, index_offset=index_offset, out=out)
+  if st_k == 0:
+    return s, i
+  return topk_merge(torch.stack([state[0], s]), torch.stack([state[1], i]), k, sorted_lists=True)
 
 
 def _i64(t, name: str, device) -> torch.Tensor:
@@ -293,12 +324,7 @@ def topk_tc_exclude(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tens
   ids = None if identifiers is None else _i64(identifiers, "identifiers", q.device)
   out_s = torch.empty((Q, k), dtype=torch.float32, device=q.device)
   out_i = torch.empty((Q, k), dtype=torch.int64, device=q.device)
-  if Q == 0:
-    return out_s, out_i
-  for lo in range(0, Q, TC_MAX_Q_PER_CALL):
-    hi = min(Q, lo + TC_MAX_Q_PER_CALL)
-    wsb = lib().tfrs_topk_tc_workspace_bytes(hi - lo, N, d, k + E)
-    ws = workspace(wsb, q.device, "tc")
+  for lo, hi, ws in _tc_query_chunks(q, N, k + E):
     check(lib().tfrs_topk_tc_exclude_f32(ptr(q[lo:hi]), hi - lo, ptr(corpus), ptr(index_buf), N, d, k, index_offset, ptr(ids),
                                          ptr(ex[lo:hi]), E, ptr(out_s[lo:hi]), ptr(out_i[lo:hi]), ptr(ws), ws.numel(), stream()),
           "topk_tc_exclude")
@@ -313,10 +339,7 @@ def topk_tc_count(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor
   pos = f32c(positive_scores, "positive_scores").view(-1)
   Q, d = q.shape; N = corpus.shape[0]
   out = torch.empty((Q,), dtype=torch.int32, device=q.device)
-  for lo in range(0, Q, TC_MAX_Q_PER_CALL):
-    hi = min(Q, lo + TC_MAX_Q_PER_CALL)
-    wsb = lib().tfrs_topk_tc_workspace_bytes(hi - lo, N, d, k)
-    ws = workspace(wsb, q.device, "tc")
+  for lo, hi, ws in _tc_query_chunks(q, N, k):
     check(lib().tfrs_topk_tc_count_f32(ptr(q[lo:hi]), hi - lo, ptr(corpus), ptr(index_buf), N, d, k, ptr(pos[lo:hi]),
                                        ptr(out[lo:hi]), ptr(ws), ws.numel(), stream()), "topk_tc_count")
   return out
@@ -361,15 +384,16 @@ def hits_accumulate(count: torch.Tensor, positive_scores: torch.Tensor, sample_w
                                         len(ks), ptr(acc), stream()), "hits_accumulate")
 
 
-def topk_merge_sorted(scores: torch.Tensor, idx: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
-  """Merge [L,Q,k_in] lists that are each sorted (score desc, index asc): rank by binary search, no sort."""
+def topk_merge(scores: torch.Tensor, idx: torch.Tensor, k: int, sorted_lists: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Merge [L,Q,k_in] lists into the best min(k, L*k_in) per query (score desc, index asc).  `sorted_lists`: every list
+  is already in that order (what the scans emit), so the merge ranks by binary search instead of sorting."""
   scores = f32c(scores, "scores"); idx = require_cuda(idx, "idx").to(torch.int64).contiguous()
   L, Q, k_in = scores.shape
   k_out = min(k, L * k_in)
   out_s = torch.empty((Q, k_out), dtype=torch.float32, device=scores.device)
   out_i = torch.empty((Q, k_out), dtype=torch.int64, device=scores.device)
-  check(lib().tfrs_topk_merge_sorted_strided(ptr(scores), ptr(idx), Q * k_in, Q * k_in, L, Q, k_in, k_out, ptr(out_s), ptr(out_i),
-                                             stream()), "topk_merge_sorted")
+  fn = lib().tfrs_topk_merge_sorted_strided if sorted_lists else lib().tfrs_topk_merge_strided
+  check(fn(ptr(scores), ptr(idx), Q * k_in, Q * k_in, L, Q, k_in, k_out, ptr(out_s), ptr(out_i), stream()), "topk_merge")
   return out_s, out_i
 
 
@@ -520,11 +544,6 @@ def topk_merge_packed(gathered: torch.Tensor, n_lists: int, Q: int, k_in: int, k
   return out_s, out_i
 
 
-def tc_supported(Q: int, N: int, d: int, k: int) -> bool:
-  """True when (Q, N, d, k) is inside the tensor-core path (otherwise callers use topk_scan)."""
-  return lib().tfrs_topk_tc_workspace_bytes(Q, N, d, k) > 0
-
-
 def tc_last_call_stats(Q: int, N: int, d: int, k: int, device=None) -> dict:
   """Survivor / fallback statistics of the most recent topk_tc call with this shape (reads the cached
   workspace; synchronises).  Used by tests to prove the tensor-core path -- not the exact fallback --
@@ -553,17 +572,6 @@ def profile_read():
   ms = (ctypes.c_float * 4)(); calls = ctypes.c_int(0)
   check(lib().tfrs_profile_read(ms, ctypes.byref(calls)), "profile_read")
   return [float(x) for x in ms], int(calls.value)
-
-
-def topk_merge(scores: torch.Tensor, idx: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
-  """Merge [L,Q,k_in] lists into the best min(k, L*k_in) per query."""
-  scores = f32c(scores, "scores"); idx = require_cuda(idx, "idx").to(torch.int64).contiguous()
-  L, Q, k_in = scores.shape
-  k_out = min(k, L * k_in)
-  out_s = torch.empty((Q, k_out), dtype=torch.float32, device=scores.device)
-  out_i = torch.empty((Q, k_out), dtype=torch.int64, device=scores.device)
-  check(lib().tfrs_topk_merge(ptr(scores), ptr(idx), L, Q, k_in, k_out, ptr(out_s), ptr(out_i), stream()), "topk_merge")
-  return out_s, out_i
 
 
 # ------------------------------------------------------------------------------------------------
@@ -840,7 +848,7 @@ class _HardNegativeSoftmax(torch.autograd.Function):
   @staticmethod
   def forward(ctx, q, c, num_hard_negatives, sample_weight, inv_temperature):
     q = f32c(q, "query_embeddings"); c = f32c(c, "candidate_embeddings")
-    B, d = q.shape; C = c.shape[0]
+    B = q.shape[0]; C = c.shape[0]
     if not inv_temperature > 0:
       raise NotImplementedError("hard_negative_softmax_loss needs a positive temperature")
     k1 = min(int(num_hard_negatives) + 1, C)
@@ -848,10 +856,7 @@ class _HardNegativeSoftmax(torch.autograd.Function):
     if w is not None and w.numel() != B:
       raise ValueError(f"sample_weight must have one entry per query (got {w.numel()}, expected {B})")
     qd, cd = q.detach(), c.detach()
-    if C >= TC_MIN_N and d <= 128 and tc_supported(B, C, d, k1):
-      top_s, top_i = topk_tc(qd, cd, index_build(cd, reuse_slot="hardneg_index"), k1)
-    else:
-      top_s, top_i = topk_scan(qd, cd, k1)
+    top_s, top_i = topk(qd, cd, k1, image="hardneg_index")
     pos = rowwise_dot(qd, cd[:B])
     loss = torch.empty((1,), dtype=torch.float32, device=q.device)
     coef = torch.empty((B, k1 + 2), dtype=torch.float32, device=q.device)

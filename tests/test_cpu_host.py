@@ -31,7 +31,7 @@ def test_library_builds_and_exports_exactly_the_declared_symbols():
     assert hasattr(lib, name), f"{name} declared in include/tfrs_b200.h but not exported"
   assert set(declared) == set(_ffi.EXPORTS), set(declared) ^ set(_ffi.EXPORTS)
   for gone in ("tfrs_inbatch_softmax_tc_ex_workspace_bytes", "tfrs_inbatch_softmax_tc_fwd_ex",
-               "tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes", "tfrs_inbatch_softmax_tc_bwd_ex"):
+               "tfrs_inbatch_softmax_tc_bwd_ex_workspace_bytes", "tfrs_inbatch_softmax_tc_bwd_ex", "tfrs_topk_merge"):
     assert not hasattr(lib, gone), f"{gone} is still exported"
   # no-compute calls are safe without a GPU
   l = _ffi.lib()

@@ -223,7 +223,7 @@ def test_cfg4_shape_d128_two_shards(ops):
     lo, hi = tfrs.layers.factorized_top_k.shard_bounds(N, r, 2)
     img = ops.index_build(c[lo:hi])
     parts.append(ops.topk_tc(q, c[lo:hi], img, k, index_offset=lo))
-  ms, mi = ops.topk_merge_sorted(torch.stack([p[0] for p in parts]), torch.stack([p[1] for p in parts]), k)
+  ms, mi = ops.topk_merge(torch.stack([p[0] for p in parts]), torch.stack([p[1] for p in parts]), k, sorted_lists=True)
   assert torch.equal(mi, i) and torch.equal(ms, s)
 
 
