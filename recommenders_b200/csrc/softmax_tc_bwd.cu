@@ -209,14 +209,21 @@ softmax_tc_bwd_kernel(const SoftmaxBwdParams p) {
     const long long row = row_a + 8 * rr;
     if (row >= p.n_x_rows) continue;
     // transposed: G carried w^ = w 2^wexp per column; otherwise G carried 2^14 and the row weight is applied here
-    const float fs = TRANSPOSED ? ldexpf(gl * p.inv_t, -(p.wst->exp + p.yst->exp))
-                                : ldexpf(gl * p.inv_t * w_r[rr], -(p.wst->exp + 14 + p.yst->exp));
+    const float f = TRANSPOSED ? gl * p.inv_t : gl * p.inv_t * w_r[rr];
+    const int fe = TRANSPOSED ? -(p.wst->exp + p.yst->exp) : -(p.wst->exp + 14 + p.yst->exp);
+    const float fs = ldexpf(f, fe);
+    // a tiny operand or grad_loss can push the factor out of the normal range (dq near 2^-110 needs 2^-138) while the
+    // gradient itself is normal: then it is applied as two normal factors, f 2^(fe - e2) and 2^e2, so that only the
+    // final product rounds there.  Where fs is normal the second factor is 1 and the bits are those of dacc * fs.
+    const bool fs_normal = fabsf(fs) >= 1.17549435e-38f && fabsf(fs) <= 3.40282347e38f;
+    const int e2 = fs_normal ? 0 : min(max(fe, -126), 127);
+    const float f1 = fs_normal ? fs : ldexpf(f, fe - e2), f2 = ldexpf(1.0f, e2);
     float* dst = p.out + (long long)part * p.part_stride + row * p.d;
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       if (((i >> 1) & 1) != rr) continue;
       const int col = frag_col(i, lane);
-      if (col < p.d) dst[col] = dacc[i] * fs;
+      if (col < p.d) dst[col] = dacc[i] * f1 * f2;
     }
   }
 }

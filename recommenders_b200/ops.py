@@ -703,10 +703,12 @@ class _InBatchSoftmax(torch.autograd.Function):
         raise ValueError(f"score_mask must be [{B},{C}], got {tuple(mask.shape)}")
       mask = (mask if mask.dtype == torch.bool else mask != 0).contiguous().view(torch.uint8)
     ext = ids is not None or mask is not None
-    if (cb is not None or ext) and not inbatch_softmax_bias_supported(B, C, d):
+    # the tensor-core kernels work in log2 units scaled by 1/T > 0; any other temperature takes the exact path
+    if (cb is not None or ext) and not (inv_temperature > 0 and inbatch_softmax_bias_supported(B, C, d)):
       raise NotImplementedError("inbatch_softmax_loss: candidate_bias / candidate_ids / score_mask need the tensor-core path "
-                                f"(B >= {SOFTMAX_TC_MIN_B}, d <= 64); got B={B}, d={d}")
-    used_tc = B >= SOFTMAX_TC_MIN_B and \
+                                f"(B >= {SOFTMAX_TC_MIN_B}, d <= 64, temperature > 0); got B={B}, d={d}, "
+                                f"1/temperature={inv_temperature}")
+    used_tc = inv_temperature > 0 and B >= SOFTMAX_TC_MIN_B and \
         lib().tfrs_inbatch_softmax_tc_workspace_bytes(B, C, d, int(ids is not None), int(mask is not None)) > 0
     if used_tc:  # tensor-core forward (hi/lo fp16 split, fp32 accumulate, online log-sum-exp epilogue)
       loss, lse = inbatch_softmax_tc(q, c, w, inv_temperature, cb, ids, mask)

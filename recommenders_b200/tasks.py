@@ -91,6 +91,7 @@ class Retrieval(torch.nn.Module, Task):
                   (self._temperature is None or self._temperature > 0) and
                   ops.hard_negative_supported(B_, C_, d_, self._num_hard_negatives))
     fused_opts = (fusable and self._num_hard_negatives is None and options and
+                  (self._temperature is None or self._temperature > 0) and
                   ops.inbatch_softmax_bias_supported(B_, C_, d_))
     plain = not three_d and self._loss is None and self._num_hard_negatives is None and not options
     # multi-head queries (maxsim, :172-176) with the default loss: the head maximum is folded inside the blocked loss kernels
