@@ -517,6 +517,64 @@ int tfrs_unified_lookup_bwd_f32(const tfrs_ue_feature* features, int n_features,
                                 void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K11  Weighted multi-hot bag pooling (layers/embedding/tpu_embedding_layer.py off TPU: safe_embedding_lookup_sparse per
+ * feature).  Every feature of a call in one launch (up to 128 features; longer calls take one launch per group of whole
+ * features).  A feature reads `table` [rows, dim] (row-major) with n ids `values` (kind TFRS_I32 / TFRS_I64) and optional
+ * fp32 `weights` [n] (NULL = 1), and writes output row r at out[r * ld + col_off ..]:
+ *  - row_splits != NULL, max_seq_len == 0 (pooled, n_bags rows): row b = (sum of w*e over the valid values of the bag
+ *    values[row_splits[b] .. row_splits[b+1]), in value order from +0.0f, each step one fp32 multiply and one add) / D;
+ *    D = 1 (SUM), sum w (MEAN), sqrtf(sum w*w) (SQRTN), summed sequentially in fp32; one IEEE division; an empty bag
+ *    gives zeros.  `denom` (fp32 [n_bags], nullable) receives D for MEAN / SQRTN; the backward reads it.
+ *  - row_splits != NULL, max_seq_len L > 0 (sequence, n_bags * L rows): row b*L + j = w_j * e_j for j < bag size, zeros
+ *    for the positions past the bag; values past L are cut.
+ *  - row_splits == NULL (dense, n rows): row i = e_i; weights must be NULL.
+ * Ids outside [0, rows) are dropped with their weight (zeros at their position, nothing added to a bag or to D).
+ * `ids` (int64 [n], nullable) receives the ids as int64: pointing the features of one table at consecutive ranges of one
+ * buffer gives that table's (ids, grad_rows) pair.  row_splits are non-decreasing from 0 to n, n_bags >= 1 unless n == 0.
+ * Backward: grad_rows (fp32 [n, dim]) row v = grad[r * ld + col_off ..] of the value's output row r (dense), times w
+ * (sequence; zeros past L), or g_b * w / D_b (pooled; g_b * w for SUM); zeros for dropped ids.  One launch per group.
+ * No alignment is required: dim, col_off, ld multiples of 4 with 16-byte aligned pointers take float4 pieces, anything
+ * else a scalar path with the same bits.  No float atomics.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct tfrs_bag_feature {
+  const float* table;
+  int64_t rows;
+  int32_t dim;
+  int32_t kind;                /* TFRS_I32 / TFRS_I64 */
+  const void* values;
+  int64_t n;
+  const int64_t* row_splits;   /* nullable: dense */
+  int64_t n_bags;
+  const float* weights;        /* nullable */
+  int32_t combiner;            /* TFRS_COMBINER_*, pooled features */
+  int32_t max_seq_len;         /* > 0: sequence feature */
+  float* out;                  /* forward */
+  int64_t ld;
+  int32_t col_off;
+  int32_t reserved;
+  int64_t* ids;                /* forward, nullable */
+  float* denom;                /* forward: written (nullable); backward: read (MEAN / SQRTN) */
+  const float* grad;           /* backward: gradient of out (same ld / col_off) */
+  float* grad_rows;            /* backward: [n, dim] */
+} tfrs_bag_feature;
+int tfrs_embedding_bag_fwd_f32(const tfrs_bag_feature* features, int n_features, void* stream);
+int tfrs_embedding_bag_bwd_f32(const tfrs_bag_feature* features, int n_features, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * SGD with tf-keras's legacy rules (optimizer_v2/gradient_descent.py, momentum 0), every step one IEEE fp32 operation:
+ *   dense:   var' = var - lr*g
+ *   sparse:  var[id] = var[id] - lr*g_i once per occurrence i of id, in order of occurrence (no deduplication)
+ * Sparse: one table per call; I32/I64 ids, out-of-range ids skipped, n < 2^24, rows < 2^40; ws holds
+ * tfrs_sparse_sgd_workspace_bytes(n) bytes.  Dense: vars / grads / numels are HOST arrays of nvars device pointers and
+ * element counts.  Deterministic, no atomics.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_sparse_sgd_workspace_bytes(int64_t n);
+int tfrs_sparse_sgd_f32(float* table, int64_t rows, int d, const void* ids, int ids_dtype, int64_t n,
+                        const float* grad_rows, float lr, void* ws, size_t ws_bytes, void* stream);
+int tfrs_sgd_dense_f32(float* const* vars, const float* const* grads, const int64_t* numels, int nvars, float lr,
+                       void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K9  tree-AH approximate retrieval: the algorithm of ScaNN (layers/factorized_top_k.py:613-796) under the rules of
  * DESIGN.md §2 -- a k-means tree of L leaves over the rows, 4-bit product codes of every row's residual (blocks of dpb
  * dims, 16 centers each), and a search that scores the rows of the probed leaves with int8 lookup tables.

@@ -109,6 +109,11 @@ _SIGNATURES = {
     "tfrs_hash_bins": (c_i, [c_p, c_p, c_i, c_l, c_p, c_l, c_p, c_p]),
     "tfrs_unified_lookup_fwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
     "tfrs_unified_lookup_bwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
+    "tfrs_embedding_bag_fwd_f32": (c_i, [c_p, c_i, c_p]),
+    "tfrs_embedding_bag_bwd_f32": (c_i, [c_p, c_i, c_p]),
+    "tfrs_sparse_sgd_workspace_bytes": (c_sz, [c_l]),
+    "tfrs_sparse_sgd_f32": (c_i, [c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_p, c_sz, c_p]),
+    "tfrs_sgd_dense_f32": (c_i, [c_p, c_p, c_p, c_i, c_f, c_p]),
     "tfrs_tree_ah_assign_workspace_bytes": (c_sz, [c_l, c_i, c_i]),
     "tfrs_tree_ah_assign_f32": (c_i, [c_p, c_l, c_i, c_p, c_i, c_p, c_p, c_sz, c_p]),
     "tfrs_tree_ah_group_workspace_bytes": (c_sz, [c_l]),

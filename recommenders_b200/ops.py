@@ -209,6 +209,141 @@ def unified_lookup_bwd(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot
 
 
 # ------------------------------------------------------------------------------------------------
+# K11 weighted multi-hot bag pooling (TPUEmbedding)
+# ------------------------------------------------------------------------------------------------
+class _BagFeature(ctypes.Structure):
+  _fields_ = [("table", ctypes.c_void_p), ("rows", ctypes.c_int64), ("dim", ctypes.c_int32), ("kind", ctypes.c_int32),
+              ("values", ctypes.c_void_p), ("n", ctypes.c_int64), ("row_splits", ctypes.c_void_p),
+              ("n_bags", ctypes.c_int64), ("weights", ctypes.c_void_p), ("combiner", ctypes.c_int32),
+              ("max_seq_len", ctypes.c_int32), ("out", ctypes.c_void_p), ("ld", ctypes.c_int64),
+              ("col_off", ctypes.c_int32), ("reserved", ctypes.c_int32), ("ids", ctypes.c_void_p),
+              ("denom", ctypes.c_void_p), ("grad", ctypes.c_void_p), ("grad_rows", ctypes.c_void_p)]
+
+
+class BagFeature(NamedTuple):
+  """One feature of an embedding_bag call.  `values`: CUDA int32 / int64 ids (flattened).  With `row_splits` (int64
+  [bags+1]) the values form bags: pooled with `combiner`, or, when `max_sequence_length` L > 0, laid out as L positions
+  per bag.  Without, every value is looked up on its own (dense).  `weights` (fp32, one per value) only with bags.
+  `out` is 2-D with one row per output row (bags, bags * L, or values); this feature's columns are
+  [col_off, col_off + dim).  `ids` (int64 [n]) receives the ids for the backward pair; `denom` (fp32 [bags]) receives
+  the mean / sqrtn denominators, which the backward needs."""
+  table: torch.Tensor
+  values: torch.Tensor
+  out: torch.Tensor
+  row_splits: Optional[torch.Tensor] = None
+  weights: Optional[torch.Tensor] = None
+  combiner: str = "mean"
+  max_sequence_length: int = 0
+  col_off: int = 0
+  ids: Optional[torch.Tensor] = None
+  denom: Optional[torch.Tensor] = None
+
+
+def bag_out_rows(f: BagFeature) -> int:
+  if f.row_splits is None:
+    return f.values.numel()
+  bags = f.row_splits.numel() - 1
+  return bags * f.max_sequence_length if f.max_sequence_length > 0 else bags
+
+
+def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor]):
+  """The C descriptors; `mats[k]` is the 2-D tensor feature k's columns live in (its output, or that output's gradient)."""
+  cs = (_BagFeature * len(features))()
+  for k, (f, m) in enumerate(zip(features, mats)):
+    d = cs[k]
+    require_cuda(f.table, "table")
+    if f.table.dtype != torch.float32 or not f.table.is_contiguous() or f.table.dim() != 2:
+      raise ValueError("embedding_bag: tables must be contiguous 2-D float32")
+    d.table, d.rows, d.dim = f.table.data_ptr(), f.table.shape[0], f.table.shape[1]
+    d.kind = _ffi.ids_dtype_code(require_cuda(f.values, "values"))
+    if not f.values.is_contiguous():
+      raise ValueError("embedding_bag: values must be contiguous")
+    d.values, d.n = f.values.data_ptr(), f.values.numel()
+    if f.row_splits is not None:
+      require_cuda(f.row_splits, "row_splits")
+      if f.row_splits.dtype != torch.int64 or f.row_splits.dim() != 1 or f.row_splits.numel() < 1:
+        raise TypeError("row_splits must be a non-empty 1-D int64 tensor")
+      d.row_splits, d.n_bags = f.row_splits.data_ptr(), f.row_splits.numel() - 1
+      d.combiner, d.max_seq_len = COMBINERS[f.combiner], int(f.max_sequence_length)
+    if f.weights is not None:
+      require_cuda(f.weights, "weights")
+      if f.weights.dtype != torch.float32 or not f.weights.is_contiguous() or f.weights.numel() != f.values.numel():
+        raise ValueError("embedding_bag: weights must be contiguous float32 with one entry per value")
+      d.weights = f.weights.data_ptr()
+    _check_2d(m, bag_out_rows(f), "each output / gradient")
+    d.ld, d.col_off = max(m.stride(0), m.shape[1]), f.col_off
+    if f.ids is not None:
+      require_cuda(f.ids, "ids")
+      if f.ids.dtype != torch.int64 or not f.ids.is_contiguous() or f.ids.numel() != f.values.numel():
+        raise ValueError("embedding_bag: ids must be contiguous int64 with one entry per value")
+      d.ids = f.ids.data_ptr()
+    if f.denom is not None:
+      if f.denom.dtype != torch.float32 or not f.denom.is_contiguous() or f.denom.numel() != d.n_bags:
+        raise ValueError("embedding_bag: denom must be contiguous float32 with one entry per bag")
+      d.denom = f.denom.data_ptr()
+  return cs
+
+
+def embedding_bag(features: Sequence[BagFeature]) -> None:
+  """Every lookup of one call (tfrs_embedding_bag_fwd_f32): pooled bags, sequence positions and dense values written
+  into each feature's `out`.  One launch for up to 128 features."""
+  cs = _bag_structs(features, [f.out for f in features])
+  for k, f in enumerate(features):
+    cs[k].out = f.out.data_ptr()
+  check(lib().tfrs_embedding_bag_fwd_f32(cs, len(features), stream()), "embedding_bag")
+
+
+def embedding_bag_bwd(features: Sequence[BagFeature], grads: Sequence[torch.Tensor],
+                      grad_rows: Sequence[torch.Tensor]) -> None:
+  """grad_rows[k] ([n, dim]) = the gradient of feature k's table rows, value by value, from grads[k] (the gradient of
+  its 2-D output; `out` itself is not read) and the forward's `denom`.  One launch for up to 128 features."""
+  if len(grads) != len(features) or len(grad_rows) != len(features):
+    raise ValueError("embedding_bag_bwd: one gradient and one grad_rows tensor per feature")
+  cs = _bag_structs(features, grads)
+  for k, (f, g, r) in enumerate(zip(features, grads, grad_rows)):
+    require_cuda(r, "grad_rows")
+    if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (f.values.numel(), cs[k].dim):
+      raise ValueError("embedding_bag_bwd: grad_rows must be contiguous float32 [n, dim]")
+    cs[k].grad, cs[k].grad_rows = g.data_ptr(), r.data_ptr()
+  check(lib().tfrs_embedding_bag_bwd_f32(cs, len(features), stream()), "embedding_bag_bwd")
+
+
+# ------------------------------------------------------------------------------------------------
+# SGD (tf-keras legacy rules, momentum 0)
+# ------------------------------------------------------------------------------------------------
+def sparse_sgd_(table: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor, lr: float) -> None:
+  """table[ids[i]] -= lr * grad_rows[i] for every i, duplicates applied one by one in order of occurrence."""
+  table = require_cuda(table, "table")
+  if table.dtype != torch.float32 or not table.is_contiguous() or table.dim() != 2:
+    raise ValueError("sparse_sgd: table must be contiguous 2-D float32")
+  ids = require_cuda(ids, "ids").reshape(-1).contiguous()
+  n, d = ids.numel(), table.shape[1]
+  grad_rows = f32c(grad_rows, "grad_rows").reshape(n, d)
+  if n == 0:
+    return
+  ws = workspace(lib().tfrs_sparse_sgd_workspace_bytes(n), table.device, "sgd")
+  check(lib().tfrs_sparse_sgd_f32(ptr(table), table.shape[0], d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(grad_rows),
+                                  float(lr), ptr(ws), ws.numel(), stream()), "sparse_sgd")
+
+
+def sgd_dense_(params: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], lr: float) -> None:
+  """p -= lr * g for every (p, g), in one multi-tensor launch per batch of variables."""
+  n = len(params)
+  if n == 0:
+    return
+  gs = []
+  for p, g in zip(params, grads):
+    require_cuda(p, "param")
+    if p.dtype != torch.float32 or not p.is_contiguous() or g.shape != p.shape:
+      raise ValueError("sgd_dense: parameters must be contiguous float32, gradients of the same shape")
+    gs.append(f32c(g, "grad"))
+  vp = (ctypes.c_void_p * n)(*[p.data_ptr() for p in params])
+  gp = (ctypes.c_void_p * n)(*[g.data_ptr() for g in gs])
+  ne = (ctypes.c_int64 * n)(*[p.numel() for p in params])
+  check(lib().tfrs_sgd_dense_f32(vp, gp, ne, n, float(lr), stream()), "sgd_dense")
+
+
+# ------------------------------------------------------------------------------------------------
 # K2 top-k
 # ------------------------------------------------------------------------------------------------
 def topk_scan(q: torch.Tensor, corpus: torch.Tensor, k: int, index_offset: int = 0,

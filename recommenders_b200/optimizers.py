@@ -203,3 +203,39 @@ class Adam(_SlotOptimizer):
   @classmethod
   def from_config(cls, config: Dict[str, Any]) -> "Adam":
     return cls(**config)
+
+
+class SGD(_SlotOptimizer):
+  """Plain SGD with tf-keras's legacy rules (`tf.keras.optimizers.legacy.SGD`, optimizer_v2/gradient_descent.py):
+  var -= lr * g.  An embedding table applies every occurrence of an id on its own, in order of occurrence, like the
+  reference's `resource_scatter_add` without deduplication (the order is unpinned against TF).  Dense variables take one
+  multi-tensor launch.  `momentum != 0` and `nesterov=True` raise NotImplementedError."""
+
+  def __init__(self, learning_rate: float = 0.01, momentum: float = 0.0, nesterov: bool = False, name: str = "SGD"):
+    if momentum != 0.0 or nesterov:
+      raise NotImplementedError("SGD: momentum and nesterov are not supported")
+    super().__init__()
+    self.learning_rate = learning_rate
+    self.momentum = momentum
+    self.nesterov = nesterov
+    self.name = name
+
+  def _apply(self, tables, dense):
+    for t in tables:
+      grads = t.pop_sparse_grads()
+      if not grads:
+        continue
+      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)
+      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
+      ops.sparse_sgd_(t.weight, ids, rows, self.learning_rate)
+    params = [p for p in dense if p.grad is not None]
+    if params:
+      with torch.no_grad():
+        ops.sgd_dense_([p.data for p in params], [p.grad for p in params], self.learning_rate)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "learning_rate": self.learning_rate, "momentum": self.momentum, "nesterov": self.nesterov}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]) -> "SGD":
+    return cls(**config)
