@@ -134,6 +134,12 @@ int tfrs_topk_hits_accumulate(const int32_t* count, const float* positive_scores
  * took the exact fallback and which selection / threshold branch a call ran. */
 int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out10);
 
+/* The same workspace's two-threshold state: out4 = {guaranteed-threshold offset (float [padded Q], the k-th bin bound
+ * thr_safe), retry-mark offset (uint32 [padded Q], 1 = the row missed at its raised filter threshold and was filtered
+ * again at thr_safe), bin rank K' of the filter threshold of a top-K / exclusion call, sample stride}.  The threshold
+ * at the tfrs_topk_tc_layout offset is the one whose records the workspace holds: thr_safe for a retried row. */
+int tfrs_topk_tc_retry_layout(int64_t Q, int64_t N, int d, int k, int64_t* out4);
+
 /* Optional per-stage device timing of tfrs_topk_tc_f32 (CUDA events on the launch stream; used by
  * bench.py for the roofline figure).  tfrs_profile_read synchronises the device and returns the summed
  * times in ms of stage 0 = query image, 1 = sampled pass + threshold, 2 = full filter pass (the

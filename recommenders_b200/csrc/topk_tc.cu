@@ -10,7 +10,9 @@
 //                (1) tc_scan<SAMPLE> : screening GEMM over every 4th corpus tile; each epilogue thread keeps the maximum
 //                    of a GROUP of tiles (a "bin") -> <= 1024 bins per query; tc_threshold (a warp per query, bins in
 //                    registers) takes the K-th largest bin maximum L_q: K distinct bins hold K distinct candidates
-//                    >= L_q, so L_q is a valid lower bound of the K-th best screening score
+//                    >= L_q, so L_q is a valid lower bound of the K-th best screening score; top-K and EXCLUDE calls
+//                    filter at the K'-th largest (filter_bin_rank, K' < K: a bound but for ~1e-9 of rows in random
+//                    order) and keep L_q for the rows that miss, which are filtered and selected again (retry)
 //                (2) tc_scan<FILTER> : screening GEMM over the whole corpus; epilogue compares the fp32
 //                    accumulators (in registers) with T_q = L_q - margin_q and appends the rare
 //                    survivors (octet records) to per-(query, part, half) lists -- nothing else leaves the SM
@@ -219,6 +221,9 @@ struct ScanParams {
   int group, bins_per_part;
   // FILTER
   const float* thr;               // [Qp]
+  // Retry launch (null on the first filter pass): [Qp] marks of the rows the select kernel sends back at their guaranteed
+  // threshold.  Only those rows rewrite their records and counts; a CTA whose 256 queries hold none exits at once.
+  const unsigned int* retry;
   unsigned int* count;            // [Qp, parts, 2]   records written by each (query, corpus part, half)
   // Survivor RECORDS: when any of 8 consecutive columns of a row passes the threshold, the whole octet is
   // appended (two 16-byte stores + the index of its first column); finalize drops the non-survivors.
@@ -247,6 +252,11 @@ tc_scan_kernel(const ScanParams p) {
   const int u_end = (int)((long long)(part + 1) * p.n_seq / p.parts);
   const int n_iter = u_end - u_begin;
   const bool issuer = threadIdx.x == 0;   // also drives the bulk-TMA ring
+  // rows this launch (re)writes: every row on the first filter pass, the marked ones on a retry
+  auto rescanned = [&](long long row) { return p.retry == nullptr || (row < p.Q && p.retry[row] != 0u); };
+  if (MODE == MODE_FILTER && p.retry != nullptr &&
+      !__syncthreads_or(threadIdx.x < QBLK && rescanned((long long)qb * QBLK + threadIdx.x)))
+    return;
 
   if (issuer) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
@@ -280,8 +290,9 @@ tc_scan_kernel(const ScanParams p) {
   const bool quad_leader = (lane & 3) == 0;
   float thr[2] = {INFINITY, INFINITY};
   if (MODE == MODE_FILTER) {
+    // a row a retry launch does not rescan gets a NaN threshold, which no score passes (not even +inf): its records stay
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) if (row_a + 8 * rr < p.Q) thr[rr] = p.thr[row_a + 8 * rr];
+    for (int rr = 0; rr < 2; ++rr) if (row_a + 8 * rr < p.Q) thr[rr] = rescanned(row_a + 8 * rr) ? p.thr[row_a + 8 * rr] : NAN;
   }
   const unsigned int cap = (unsigned int)p.cap_part;
   unsigned int cnt[4] = {0u, 0u, 0u, 0u}, ovf = 0u;      // segment s = (row rr, column half h) = 2 rr + h
@@ -457,8 +468,9 @@ tc_scan_kernel(const ScanParams p) {
   } else if (quad_leader) {
 #pragma unroll
     for (int s = 0; s < 4; ++s)
-      p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] =
-          FILTER_ABLATION != FILTER_FULL ? sink : ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
+      if (rescanned(row_a + 8 * (s >> 1)))
+        p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] =
+            FILTER_ABLATION != FILTER_FULL ? sink : ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
   }
 }
 
@@ -518,12 +530,14 @@ __device__ __forceinline__ unsigned int warp_kth_largest_smem(const unsigned int
   return prefix;
 }
 
-// (1b) K-th largest bin maximum of the sampled pass -> filter threshold T = L - margin.  One warp per query, the
-// query's <= 32*KPL bin maxima live in registers.
+// (1b) K-th largest bin maximum of the sampled pass -> guaranteed threshold thr_safe = L_K - margin, and the filter
+// threshold thr = L_K' - margin at the smaller bin rank k_filter (Plan::k_filter; == k where the threshold must stay a
+// guarantee).  One warp per query, the query's <= 32*KPL bin maxima live in registers.
 template <int KPL>
 __global__ void __launch_bounds__(256)
-tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, int k, const float* __restrict__ margin,
-                    float* __restrict__ thr, unsigned int* __restrict__ overflow, long long Q) {
+tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, int k, int k_filter, const float* __restrict__ margin,
+                    float* __restrict__ thr, float* __restrict__ thr_safe, unsigned int* __restrict__ overflow,
+                    unsigned int* __restrict__ retry, long long Q) {
   const int lane = threadIdx.x & 31;
   const long long row = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5;
   if (row >= Q) return;
@@ -531,8 +545,9 @@ tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, i
   unsigned int key[KPL];
 #pragma unroll
   for (int j = 0; j < KPL; ++j) { const int i = j * 32 + lane; key[j] = i < n_bins ? f2key(__ldg(src + i)) : 0u; }
-  const unsigned int kth = warp_kth_largest_regs<KPL>(key, k);
-  if (lane == 0) { thr[row] = key2f(kth) - margin[row]; overflow[row] = 0; }
+  const float safe = key2f(warp_kth_largest_regs<KPL>(key, k)) - margin[row];
+  const float filter = k_filter < k ? key2f(warp_kth_largest_regs<KPL>(key, k_filter)) - margin[row] : safe;
+  if (lane == 0) { thr[row] = filter; thr_safe[row] = safe; overflow[row] = 0; retry[row] = 0; }
 }
 
 // (3) finalize: one WARP per query, no block-wide barriers.
@@ -540,11 +555,13 @@ enum { FIN_TOPK = 0, FIN_EXCLUDE = 1, FIN_COUNT = 2 };
 constexpr int FW_WARPS = 4;                       // queries per CTA of the fallback re-rank kernel
 // Capacities per query come from the plan (they grow with k); a row that overflows them takes the exact fallback.
 // overflow[row]: 0 = done, 1 = exact fallback
+// retry[row]:    1 = the row's filter threshold was above thr_safe and missed; it was filtered again at thr_safe
 
 struct FinParams {
   const float* q; const float* corpus; int d; int k; long long index_offset; long long N; long long Q;
   const unsigned int* count; const float* cand_s; const unsigned int* cand_i; int segs; int cap_part;
-  const float* cut; const float* thr; unsigned int* overflow;
+  const float* cut; float* thr; const float* thr_safe; unsigned int* overflow;
+  unsigned int* retry; int retry_pass;           // retry_pass: the select launch after the retry filter pass (marked rows only)
   int cap_keys, cap_band;                        // survivors per query (keys in shared memory) / band entries re-scored exactly
   unsigned int* band_idx; int* band_n;           // [Qp, cap_band] local indices of the band, [Qp] their number
   int allow_short;                               // sharded scan with a GLOBAL threshold: a shard may hold fewer than k survivors
@@ -664,7 +681,7 @@ tc_select_kernel(const FinParams p) {
   extern __shared__ __align__(16) unsigned char fsm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * SEL_WARPS + warp;
-  if (row >= p.Q) return;
+  if (row >= p.Q || (p.retry_pass && p.retry[row] == 0u)) return;
   unsigned char* base = fsm + (size_t)warp * sel_warp_bytes(p.cap_keys, p.segs);
   unsigned int* keys = reinterpret_cast<unsigned int*>(base);                 // [cap_keys] screening keys
   unsigned short* loc = reinterpret_cast<unsigned short*>(keys + p.cap_keys);  // [cap_keys] (flat record index << 3 | column): total records < 8192
@@ -766,7 +783,19 @@ tc_select_kernel(const FinParams p) {
     }
     n += tot;
   }
-  if (n > p.cap_keys || (n < p.k && !p.allow_short)) { if (lane == 0) { p.overflow[row] = 1; p.band_n[row] = 0; } return; }
+  // A row whose filter threshold (bin rank k_filter) was above the guaranteed one and fails a check that a lower
+  // threshold can pass (n >= k, lim >= thr) is marked for the retry filter pass at thr_safe; any other miss, and any
+  // miss at thr_safe, takes the exact fallback.  Overflows (segments, records, survivor keys) grow as the threshold
+  // drops, so they go straight to the fallback.
+  auto miss = [&]() {
+    if (lane == 0) {
+      const float safe = p.thr_safe[row];
+      if (thr_row > safe) { p.retry[row] = 1; p.thr[row] = safe; } else p.overflow[row] = 1;
+      p.band_n[row] = 0;
+    }
+  };
+  if (n > p.cap_keys) { if (lane == 0) { p.overflow[row] = 1; p.band_n[row] = 0; } return; }
+  if (n < p.k && !p.allow_short) { miss(); return; }
   __syncwarp();
   if (n < p.k) {
     // Sharded scan, threshold agreed across the shards (see comm.cu): this shard holds fewer than k candidates above it.
@@ -808,7 +837,7 @@ tc_select_kernel(const FinParams p) {
   // lie above the filter threshold, otherwise survivors could be missing -> exact fallback.
   // (with a threshold agreed across shards the local band may reach below it: what is missing there cannot be in the
   //  GLOBAL top-k, and the local list is only an input of the cross-shard merge)
-  if (!p.allow_short && (!(lim >= thr_row) || !(lim > -INFINITY))) { if (lane == 0) { p.overflow[row] = 1; p.band_n[row] = 0; } return; }
+  if (!p.allow_short && (!(lim >= thr_row) || !(lim > -INFINITY))) { miss(); return; }
   // pass 2: only the band members (key >= key(lim)) go back to their record for the corpus index
   const unsigned int lim_key = f2key(lim + 0.0f);
   const unsigned int lt_mask = (1u << lane) - 1u;
@@ -1014,10 +1043,29 @@ static void prof_mark(cudaStream_t st, int stage) {
 struct Plan {
   int kb, stages; long long n_tiles; int nqb; long long Qp;
   int stride, n_sample, group, bins_per_part, n_bins, bins_ld, parts_sample, parts_full, cap_part, cap_keys, cap_band;
+  int k_filter;   // bin rank of the filter threshold of TOPK / EXCLUDE calls (filter_bin_rank)
   size_t smem;
   // workspace offsets
-  size_t o_qimg, o_margin, o_cut, o_thr, o_qexp, o_count, o_ovf, o_binmax, o_cand, o_tmp, o_band, o_bandn, total;
+  size_t o_qimg, o_margin, o_cut, o_thr, o_qexp, o_count, o_ovf, o_binmax, o_cand, o_tmp, o_band, o_bandn, o_thr_safe, o_retry,
+      total;
 };
+
+// The bin rank K' of the filter threshold: the smallest rank with P(Binomial(k - 1, 1/stride) >= K') <= 1e-9, capped at k.
+// L_K' (the K'-th largest bin maximum) is below tau, the k-th best screening score, unless K' of the k - 1 scores above
+// tau sit in sampled tiles, one per bin; for a row in random order each of them does so with probability 1/stride.  A
+// row that meets those odds anyway is caught by the select kernel's self-check and retried at L_k, which is always a
+// lower bound (DESIGN.md, K2).
+static int filter_bin_rank(int k, int stride) {
+  if (stride <= 1 || k <= 1) return k;   // every tile is sampled: only rank k is a bound
+  const int n = k - 1;
+  const double p = 1.0 / stride;
+  double tail = 0.0;   // P(X >= r), summed from the top
+  for (int r = n; r >= 1; --r) {
+    tail += exp(lgamma(n + 1.0) - lgamma(r + 1.0) - lgamma(n - r + 1.0) + r * log(p) + (n - r) * log1p(-p));
+    if (tail > 1e-9) return r + 1;
+  }
+  return 1;
+}
 
 static bool make_plan(long long Q, long long N, int d, int k, Plan& pl) {
   if (d <= 0 || d > 128 || Q <= 0 || N <= 0 || k <= 0) return false;   // d > 128: smem budget (A blocks + ring) not laid out
@@ -1035,6 +1083,7 @@ static bool make_plan(long long Q, long long N, int d, int k, Plan& pl) {
   { static int ov = getenv("TFRS_TC_SAMPLE_STRIDE") ? atoi(getenv("TFRS_TC_SAMPLE_STRIDE")) : 0; if (ov >= 1 && ov <= 16) pl.stride = ov; }
 #endif
   while (pl.stride > 1 && 2 * ceil_div(full_tiles, pl.stride) < 4ll * k) pl.stride >>= 1;
+  pl.k_filter = filter_bin_rank(k, pl.stride);
   pl.n_sample = (int)ceil_div(full_tiles, pl.stride);
   if (2ll * pl.n_sample < 4ll * k) return false;  // too few bins for a useful threshold -> caller uses the exact path
   const int sms = sm_count();
@@ -1081,6 +1130,8 @@ static bool make_plan(long long Q, long long N, int d, int k, Plan& pl) {
   pl.o_tmp = take((size_t)Q * k * 12);   // EXCLUDE: the exact fallback's [Q, k] lists before the re-ranking
   pl.o_band = take((size_t)pl.Qp * pl.cap_band * 4);
   pl.o_bandn = take((size_t)pl.Qp * 4);
+  pl.o_thr_safe = take((size_t)pl.Qp * 4);
+  pl.o_retry = take((size_t)pl.Qp * 4);
   pl.total = o;
   return true;
 }
@@ -1107,13 +1158,23 @@ static int launch_scan_mode(const Plan& pl, const ScanParams& sp, cudaStream_t s
   return launch_scans<2, 4>(pl, sp, st, mode);
 }
 
+// select; with `retry`, the filter pass and the select again for the rows the first select marked (launched
+// unconditionally: no host sync; CTAs and warps without a marked row exit at once); then the exact re-scoring
 template <int MODE>
-static int launch_finalize(FinParams fp, cudaStream_t st) {
+static int launch_finalize(FinParams fp, const Plan& pl, ScanParams sp, bool retry, cudaStream_t st) {
   auto ksel = tc_select_kernel<MODE>;
   auto krs = tc_rescore_kernel<MODE>;
   TFRS_DYN_SMEM(ksel, (int)(SEL_WARPS * sel_warp_bytes(4096, FIN_MAX_PARTS)));
   ksel<<<(unsigned)ceil_div(fp.Q, SEL_WARPS), SEL_WARPS * 32, SEL_WARPS * sel_warp_bytes(fp.cap_keys, fp.segs), st>>>(fp);
   TFRS_LAUNCH_CHECK();
+  if (retry) {
+    sp.retry = fp.retry;
+    const int rc = launch_scan_mode(pl, sp, st, MODE_FILTER);
+    if (rc) return rc;
+    fp.retry_pass = 1;
+    ksel<<<(unsigned)ceil_div(fp.Q, SEL_WARPS), SEL_WARPS * 32, SEL_WARPS * sel_warp_bytes(fp.cap_keys, fp.segs), st>>>(fp);
+    TFRS_LAUNCH_CHECK();
+  }
   const size_t rs_smem = (size_t)fp.cap_band * 8 + (size_t)((fp.d + 3) & ~3) * 4 + (MODE == FIN_EXCLUDE ? (size_t)fp.k * 16 : 0);
   TFRS_DYN_SMEM(krs, 64 * 1024);
   krs<<<(unsigned)fp.Q, RS_BLOCK, rs_smem, st>>>(fp);
@@ -1156,8 +1217,13 @@ static int run_call(const Call& c) {
   unsigned int* cand_i = (unsigned int*)(w + pl.o_cand + (size_t)pl.Qp * pl.parts_full * 2 * pl.cap_part * 32);
   float* tmp_s = (float*)(w + pl.o_tmp);
   long long* tmp_i = (long long*)(w + pl.o_tmp + align_up((size_t)c.Q * c.k * 4, 8));
+  float* thr_safe = (float*)(w + pl.o_thr_safe);
+  unsigned int* retry = (unsigned int*)(w + pl.o_retry);
   const IndexHeader* hdr = (const IndexHeader*)c.index_buf;
   const unsigned char* cimg = (const unsigned char*)c.index_buf + HEADER_BYTES;
+  // The raised filter threshold needs the select kernel's self-check behind it: COUNT has none (its count of definite
+  // candidates leans on L_k itself) and a sharded call turns it off (allow_short), so both keep the guaranteed bound.
+  const int k_filter = (c.mode == FIN_COUNT || c.hook) ? c.k : pl.k_filter;
 
   prof_mark(st, 0);
   // (0) per-row exponent, image and margins: one launch
@@ -1172,9 +1238,11 @@ static int run_call(const Call& c) {
   int rc = launch_scan_mode(pl, sp, st, MODE_SAMPLE);
   if (rc) return rc;
   if (pl.n_bins <= 512)
-    tc_threshold_kernel<16><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, margin, thr, ovf, c.Q);
+    tc_threshold_kernel<16><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, k_filter, margin,
+                                                                                 thr, thr_safe, ovf, retry, c.Q);
   else
-    tc_threshold_kernel<32><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, margin, thr, ovf, c.Q);
+    tc_threshold_kernel<32><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, k_filter, margin,
+                                                                                 thr, thr_safe, ovf, retry, c.Q);
   TFRS_LAUNCH_CHECK();
   if (c.hook) {
     rc = c.hook(c.hook_ctx, thr, margin, cut, qexp, &hdr->st.exp, c.Q, st);
@@ -1190,14 +1258,15 @@ static int run_call(const Call& c) {
   FinParams fp{};
   fp.q = c.q; fp.corpus = c.corpus; fp.d = c.d; fp.k = c.k; fp.index_offset = c.index_offset; fp.N = c.N; fp.Q = c.Q;
   fp.count = count; fp.cand_s = cand_s; fp.cand_i = cand_i; fp.segs = pl.parts_full * 2; fp.cap_part = pl.cap_part;
-  fp.cut = cut; fp.thr = thr; fp.overflow = ovf; fp.out_s = c.out_s; fp.out_i = c.out_i;
+  fp.cut = cut; fp.thr = thr; fp.thr_safe = thr_safe; fp.overflow = ovf; fp.retry = retry; fp.out_s = c.out_s; fp.out_i = c.out_i;
   fp.cap_keys = pl.cap_keys; fp.cap_band = pl.cap_band; fp.allow_short = c.allow_short;
   fp.band_idx = (unsigned int*)(w + pl.o_band); fp.band_n = (int*)(w + pl.o_bandn);
   fp.identifiers = c.identifiers; fp.exclusions = c.exclusions; fp.n_excl = c.n_excl; fp.k_out = c.k_out;
   fp.pos = c.pos; fp.qexp = qexp; fp.hdr = hdr; fp.out_count = c.out_count;
-  if (c.mode == FIN_TOPK) rc = launch_finalize<FIN_TOPK>(fp, st);
-  else if (c.mode == FIN_EXCLUDE) rc = launch_finalize<FIN_EXCLUDE>(fp, st);
-  else rc = launch_finalize<FIN_COUNT>(fp, st);
+  const bool may_retry = k_filter < c.k;
+  if (c.mode == FIN_TOPK) rc = launch_finalize<FIN_TOPK>(fp, pl, sp, may_retry, st);
+  else if (c.mode == FIN_EXCLUDE) rc = launch_finalize<FIN_EXCLUDE>(fp, pl, sp, may_retry, st);
+  else rc = launch_finalize<FIN_COUNT>(fp, pl, sp, false, st);
   if (rc) return rc;
   if (c.mode == FIN_COUNT) {
     tc_count_fallback_kernel<<<(unsigned)c.Q, 256, 0, st>>>(c.q, c.corpus, c.N, c.d, c.k, c.pos, ovf, c.out_count);
@@ -1322,6 +1391,16 @@ extern "C" int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* 
   out10[0] = (int64_t)pl.o_count; out10[1] = (int64_t)pl.o_ovf; out10[2] = (int64_t)pl.o_thr; out10[3] = (int64_t)pl.o_cand;
   out10[4] = pl.parts_full * 2; out10[5] = pl.cap_part; out10[6] = pl.Qp; out10[7] = (int64_t)pl.o_cut;
   out10[8] = pl.n_bins; out10[9] = (int64_t)pl.o_qexp;
+  return TFRS_OK;
+}
+
+// The same for the two-threshold filter: where thr_safe and the per-row retry marks live, the bin rank of the filter
+// threshold of a TOPK / EXCLUDE call and the sample stride it was derived from.
+extern "C" int tfrs_topk_tc_retry_layout(int64_t Q, int64_t N, int d, int k, int64_t* out4) {
+  TFRS_CHECK_ARG(out4, "topk_tc_retry_layout: NULL pointer");
+  Plan pl;
+  if (!make_plan(Q, N, d, k, pl)) { set_error("topk_tc_retry_layout: unsupported shape"); return TFRS_ERR_UNSUPPORTED; }
+  out4[0] = (int64_t)pl.o_thr_safe; out4[1] = (int64_t)pl.o_retry; out4[2] = pl.k_filter; out4[3] = pl.stride;
   return TFRS_OK;
 }
 
