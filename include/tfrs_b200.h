@@ -351,6 +351,29 @@ int tfrs_adam_dense_f32(float* const* vars, const float* const* grads, float* co
                         const int64_t* numels, int nvars, float alpha, float beta1, float beta2, float eps, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K12  FTRL-Proximal with tf-keras's legacy rules (optimizer_v2/ftrl.py; TF's ApplyFtrl / ApplyFtrlV2).  The caller
+ * folds beta into l2 once per call:  l2a = l2 + beta / (2*lr)  (fp32).  Power term:
+ *   P(x) = sqrt(x) when lr_power == -0.5, else the fp32 rounding of the fp64 pow(x, -lr_power).
+ * Every other step one IEEE fp32 operation, per element with g the gradient:
+ *   gs = l2_shrinkage > 0 ? g + (2*l2_shrinkage)*var : g ;  na = acc + g*g
+ *   lin' = lin + (gs - ((P(na) - P(acc)) / lr)*var) ;  y = P(na)/lr + 2*l2a
+ *   var' = |lin'| > l1 ? (copysign(l1, lin') - lin') / y : +0 ;  acc' = na
+ * TFRS_ERR_INVALID_ARG on a non-finite scalar, lr <= 0, lr_power > 0, or a negative l1, l2a or l2_shrinkage.
+ * Sparse (_resource_apply_sparse): one table per call, the contract of tfrs_sparse_adagrad_f32 (I32/I64 ids, duplicate
+ * ids summed in order of occurrence, out-of-range ids skipped, n < 2^24, d <= 1024, rows < 2^40); n == 0 is a no-op.
+ * Only the touched rows change: every other row keeps var, accum and linear bit for bit.  Deterministic.
+ * Dense: every variable of one optimizer in one call; vars / grads / accums / linears / numels are HOST arrays of nvars
+ * device pointers and element counts.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_sparse_ftrl_workspace_bytes(int64_t n);
+int tfrs_sparse_ftrl_f32(float* table, float* accum, float* linear, int64_t rows, int d, const void* ids, int ids_dtype,
+                         int64_t n, const float* grad_rows, float lr, float lr_power, float l1, float l2a,
+                         float l2_shrinkage, void* ws, size_t ws_bytes, void* stream);
+int tfrs_ftrl_dense_f32(float* const* vars, const float* const* grads, float* const* accums, float* const* linears,
+                        const int64_t* numels, int nvars, float lr, float lr_power, float l1, float l2a,
+                        float l2_shrinkage, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K5  DCN-v2 cross layer (layers/feature_interaction/dcn.py:176-186, full-rank, no preactivation):
  *   out = x0 * (x . W + bias + diag_scale * x) + x ,  W [D,D] in Keras [in,out] layout.
  * x0, x, out have row stride ld (>= D).  `prod` (nullable) receives x.W + bias + diag_scale*x for

@@ -84,6 +84,9 @@ _SIGNATURES = {
     "tfrs_sparse_adam_workspace_bytes": (c_sz, [c_l, c_l]),
     "tfrs_sparse_adam_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_f, c_f, c_f, c_i, c_p, c_sz, c_p]),
     "tfrs_adam_dense_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_f, c_f, c_f, c_f, c_p]),
+    "tfrs_sparse_ftrl_workspace_bytes": (c_sz, [c_l]),
+    "tfrs_sparse_ftrl_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_p, c_i, c_l, c_p, c_f, c_f, c_f, c_f, c_f, c_p, c_sz, c_p]),
+    "tfrs_ftrl_dense_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_f, c_f, c_f, c_f, c_f, c_p]),
     "tfrs_cross_fwd_f32":(c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p]),
     "tfrs_cross_tc_workspace_bytes": (c_sz, [c_l, c_i]),
     "tfrs_cross_tc_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_l, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),

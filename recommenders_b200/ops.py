@@ -1181,6 +1181,67 @@ def adam_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor]
 
 
 # ------------------------------------------------------------------------------------------------
+# K12 FTRL
+# ------------------------------------------------------------------------------------------------
+def ftrl_l2(l2: float, beta: float, lr: float) -> float:
+  """The l2 strength FTRL's kernels take: l2 + beta / (2*lr), evaluated in fp32 one operation at a time from the
+  fp32-rounded arguments, as tf-keras folds `beta` into l2 before calling the raw op."""
+  l2, beta, lr = (c_f(x).value for x in (l2, beta, lr))
+  return c_f(l2 + c_f(beta / c_f(2.0 * lr).value).value).value
+
+
+def sparse_ftrl_(table: torch.Tensor, accum: torch.Tensor, linear: torch.Tensor, ids: torch.Tensor,
+                 grad_rows: torch.Tensor, lr: float, lr_power: float, l1: float, l2a: float,
+                 l2_shrinkage: float) -> None:
+  """FTRL step of one embedding table whose gradient rows `grad_rows` belong to the rows `ids` (duplicates summed in order
+  of occurrence, out-of-range ids skipped).  `l2a` is the l2 strength of `ftrl_l2`.  Only the touched rows of the table
+  and of its slots `accum` / `linear` change."""
+  _f32_inplace(table, "table"); _f32_inplace(accum, "accum"); _f32_inplace(linear, "linear")
+  ids = require_cuda(ids, "ids").contiguous().view(-1)
+  g = f32c(grad_rows, "grad_rows")
+  if table.dim() != 2:
+    raise ValueError(f"sparse_ftrl_: table must be 2-D, got {tuple(table.shape)}")
+  n = ids.numel(); rows, d = table.shape
+  for name, s in (("accum", accum), ("linear", linear)):
+    if s.shape != table.shape or s.device != table.device:
+      raise ValueError(f"sparse_ftrl_: {name} must be {tuple(table.shape)} on {table.device}, got {tuple(s.shape)} on {s.device}")
+  if g.shape != (n, d):
+    raise ValueError(f"sparse_ftrl_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
+  if ids.device != table.device or g.device != table.device:
+    raise ValueError("sparse_ftrl_: ids and grad_rows must live on the table's device")
+  ws = workspace(lib().tfrs_sparse_ftrl_workspace_bytes(n), table.device, "ftrl")
+  check(lib().tfrs_sparse_ftrl_f32(
+      ptr(table), ptr(accum), ptr(linear), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(lr), c_f(lr_power),
+      c_f(l1), c_f(l2a), c_f(l2_shrinkage), ptr(ws), ws.numel(), stream()), "sparse_ftrl")
+
+
+def ftrl_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], accums: Sequence[torch.Tensor],
+                linears: Sequence[torch.Tensor], lr: float, lr_power: float, l1: float, l2a: float,
+                l2_shrinkage: float) -> None:
+  """FTRL step of a list of dense variables and their slots `accums` / `linears` in one multi-tensor call; `l2a` is the
+  l2 strength of `ftrl_l2`."""
+  nv = len(variables)
+  if len(grads) != nv or len(accums) != nv or len(linears) != nv:
+    raise ValueError("ftrl_dense_: variables, grads, accums and linears must have the same length")
+  if nv == 0:
+    return
+  dev = variables[0].device
+  gs = []
+  for i, (x, g, a, z) in enumerate(zip(variables, grads, accums, linears)):
+    _f32_inplace(x, f"variables[{i}]"); _f32_inplace(a, f"accums[{i}]"); _f32_inplace(z, f"linears[{i}]")
+    g = f32c(g, f"grads[{i}]")
+    if any(t.device != dev for t in (x, g, a, z)):
+      raise ValueError("ftrl_dense_: every tensor must live on one device")
+    if g.shape != x.shape or a.shape != x.shape or z.shape != x.shape:
+      raise ValueError(f"ftrl_dense_: grads[{i}] / accums[{i}] / linears[{i}] must have the shape {tuple(x.shape)}")
+    gs.append(g)
+  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
+  numels = (ctypes.c_int64 * nv)(*[x.numel() for x in variables])
+  check(lib().tfrs_ftrl_dense_f32(arr(variables), arr(gs), arr(accums), arr(linears), numels, nv, c_f(lr), c_f(lr_power),
+                                  c_f(l1), c_f(l2a), c_f(l2_shrinkage), stream()), "ftrl_dense")
+
+
+# ------------------------------------------------------------------------------------------------
 # K5 cross
 # ------------------------------------------------------------------------------------------------
 # Cross layers at least this large run their forward GEMM on the tensor cores (fp16 hi/lo split, fp32 accumulate).

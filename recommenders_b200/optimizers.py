@@ -5,7 +5,8 @@ Keras defaults: initial_accumulator_value=0.1, epsilon=1e-7.  `eps_inside_sqrt=T
 tf-keras `optimizers.Adagrad` rule  var -= lr*g/sqrt(acc+eps); False is the legacy
 `optimizers.legacy.Adagrad` rule  var -= lr*g/(sqrt(acc)+eps)  (SURVEY.md A10 -- third-party, unpinned).
 
-Adam: tf-keras's legacy `optimizers.legacy.Adam` rules on the K10 kernels (DESIGN.md A15)."""
+Adam: tf-keras's legacy `optimizers.legacy.Adam` rules on the K10 kernels (DESIGN.md A15).
+Ftrl: tf-keras's legacy `optimizers.legacy.Ftrl` rules on the K12 kernels (DESIGN.md A17)."""
 from __future__ import annotations
 
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
@@ -50,7 +51,7 @@ def clear_grads(tables: Sequence[Embedding], dense: Sequence[torch.Tensor]) -> N
 
 
 class _SlotOptimizer:
-  """Variable discovery and per-variable slots shared by Adagrad, ClippyAdagrad and Adam."""
+  """Variable discovery and per-variable slots shared by Adagrad, ClippyAdagrad, Adam, Ftrl and SGD."""
 
   def __init__(self):
     self.iterations = 0
@@ -202,6 +203,73 @@ class Adam(_SlotOptimizer):
 
   @classmethod
   def from_config(cls, config: Dict[str, Any]) -> "Adam":
+    return cls(**config)
+
+
+class Ftrl(_SlotOptimizer):
+  """FTRL-Proximal with tf-keras's legacy rules (`tf.keras.optimizers.legacy.Ftrl`, optimizer_v2/ftrl.py; DESIGN.md
+  section 2).  Dense variables and embedding tables take the same element rule; a table updates only the rows of the
+  step's ids (duplicates summed), and every other row keeps its variable, accumulator and linear slot bit for bit, as
+  tf-keras's `_resource_apply_sparse` does.  `beta` is folded into the l2 strength once per step (`ops.ftrl_l2`).
+
+  The accumulator starts at `initial_accumulator_value`, the linear slot at zero."""
+
+  _ACC_ATTR = "_tfrs_ftrl_acc"
+  _LIN_ATTR = "_tfrs_ftrl_linear"
+
+  def __init__(self, learning_rate: float = 0.001, learning_rate_power: float = -0.5,
+               initial_accumulator_value: float = 0.1, l1_regularization_strength: float = 0.0,
+               l2_regularization_strength: float = 0.0, name: str = "Ftrl",
+               l2_shrinkage_regularization_strength: float = 0.0, beta: float = 0.0):
+    if initial_accumulator_value < 0.0:
+      raise ValueError(f"`initial_accumulator_value` needs to be positive or zero, received: {initial_accumulator_value}")
+    if learning_rate_power > 0.0:
+      raise ValueError(f"`learning_rate_power` needs to be negative or zero, received: {learning_rate_power}")
+    for arg, value in (("l1_regularization_strength", l1_regularization_strength),
+                       ("l2_regularization_strength", l2_regularization_strength),
+                       ("l2_shrinkage_regularization_strength", l2_shrinkage_regularization_strength)):
+      if value < 0.0:
+        raise ValueError(f"`{arg}` needs to be positive or zero, received: {value}")
+    super().__init__()
+    self.learning_rate = learning_rate
+    self.learning_rate_power = learning_rate_power
+    self.initial_accumulator_value = initial_accumulator_value
+    self.l1_regularization_strength = l1_regularization_strength
+    self.l2_regularization_strength = l2_regularization_strength
+    self.name = name
+    self.l2_shrinkage_regularization_strength = l2_shrinkage_regularization_strength
+    self.beta = beta
+
+  def _slots_of(self, owner, like: torch.Tensor):
+    return (self._slot(owner, self._ACC_ATTR, like, self.initial_accumulator_value),
+            self._slot(owner, self._LIN_ATTR, like, 0.0))
+
+  def _apply(self, tables, dense):
+    rule = dict(lr=self.learning_rate, lr_power=self.learning_rate_power, l1=self.l1_regularization_strength,
+                l2a=ops.ftrl_l2(self.l2_regularization_strength, self.beta, self.learning_rate),
+                l2_shrinkage=self.l2_shrinkage_regularization_strength)
+    for t in tables:
+      grads = t.pop_sparse_grads()
+      if not grads:
+        continue
+      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)   # one variable: the IndexedSlices of all its lookups
+      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
+      ops.sparse_ftrl_(t.weight, *self._slots_of(t, t.weight), ids, rows, **rule)
+    params = [p for p in dense if p.grad is not None]
+    if params:
+      slots = [self._slots_of(p, p) for p in params]
+      ops.ftrl_dense_([p.data for p in params], [p.grad for p in params], [a for a, _ in slots], [z for _, z in slots],
+                      **rule)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "learning_rate": self.learning_rate, "learning_rate_power": self.learning_rate_power,
+            "initial_accumulator_value": self.initial_accumulator_value,
+            "l1_regularization_strength": self.l1_regularization_strength,
+            "l2_regularization_strength": self.l2_regularization_strength,
+            "l2_shrinkage_regularization_strength": self.l2_shrinkage_regularization_strength, "beta": self.beta}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]) -> "Ftrl":
     return cls(**config)
 
 
