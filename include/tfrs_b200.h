@@ -488,6 +488,39 @@ int tfrs_ranking_metrics_f32(const float* pred, const float* labels, const float
                                     float threshold, int num_thresholds, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K13  Listwise ranking losses and NDCG (TF-Ranking's ListMLELoss, PairwiseHingeLoss, SoftmaxLoss and NDCGMetric, as the
+ * reference's listwise_ranking tutorial uses them).  pred, labels [B, L] row-major, 1 <= L <= TFRS_LISTWISE_MAX_LIST;
+ * weights (nullable) [B], one per list.  An item with !(label >= 0) (negative or NaN) is padding: it takes no part in any
+ * loss, pair, rank or gain, and gets dl/ds = +0.  s = pred * inv_temperature (fp32); n = the valid items of a list,
+ * m = max of their s.  Per list, in fp64 unless stated:
+ *   LISTMLE         pi = valid items by label descending, ties by mix32(seed, call, b, i) ascending, then by i;
+ *                   e_k = exp(s_pi(k) - m), S_k = sum_{j >= k} e_j;  l = sum_k log S_k - (s_pi(k) - m);
+ *                   dl/ds_pi(k) = e_k * sum_{j <= k} 1/S_j - 1.
+ *                   mix32(seed, call, b, i) = f(f(f(f(seed) ^ call) ^ b) ^ i), f = murmur3's 32-bit finalizer.
+ *   PAIRWISE_HINGE  pairs (i, j) with y_i > y_j; fp32: r_i = sum_{j asc} max(0, 1 - (s_i - s_j)), l = (sum_{i asc} r_i) / #pairs
+ *                   (0 without a pair); dl/ds_k = (#active (i, k) - #active (k, j)) / #pairs, active: 1 - (s_i - s_j) > 0.
+ *   SOFTMAX         Y = sum y;  l = Y log sum_i exp(s_i - m) - sum_i y_i (s_i - m);  dl/ds_i = Y softmax_i - y_i (0 when Y = 0).
+ * The fp32 list loss l_b is the rounded fp64 value (hinge: the fp32 chain); per_list[b] = w_b * l_b (fp32) and
+ * dlds[b, i] = (float)(w_b * dl/ds_i).  loss = sum_b per_list[b] in fp64 (/ B for SUM_OVER_BATCH_SIZE), rounded once.
+ * NDCG at topn (<= 0: L), when `discount` (device fp32 [>= L], discount[r - 1] = 1 / log2(r + 1)) is given: gain =
+ * exp2f(y) - 1, ranks by pred descending (ties to the lower i), ideal ranks by label descending; DCG / IDCG are sequential
+ * fp32 sums in rank order over r < min(topn, n); ndcg[b] = DCG / IDCG, 0 when IDCG = 0.  ndcg_stats (float64 [2]) is WRITTEN
+ * with [sum_b w_b ndcg_b, sum_b w'_b], w'_b = w_b, or for a list with IDCG = 0 the mean w_b of the lists with IDCG > 0.
+ * loss_mode TFRS_LIST_LOSS_NONE computes NDCG alone.  The CTA records are folded in a fixed order by the last CTA: one kernel
+ * per call, no float atomics, bitwise reproducible.  Backward: dx = (c * dlds) * inv_temperature + 0, c = grad[b] (NONE),
+ * grad[0] (SUM) or grad[0] / B (SUM_OVER_BATCH_SIZE) in fp32.
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_LIST_LOSS_NONE = 0, TFRS_LIST_LOSS_LISTMLE = 1, TFRS_LIST_LOSS_PAIRWISE_HINGE = 2, TFRS_LIST_LOSS_SOFTMAX = 3 };
+#define TFRS_LISTWISE_MAX_LIST 1024
+size_t tfrs_listwise_workspace_bytes(int64_t B, int L);
+int tfrs_listwise_fwd_f32(const float* pred, const float* labels, const float* weights, int64_t B, int L, int loss_mode,
+                          int reduction, float inv_temperature, uint32_t seed, uint32_t call, float* per_list, float* loss,
+                          float* dlds, const float* discount, int topn, float* ndcg, double* ndcg_stats, void* ws,
+                          size_t ws_bytes, void* stream);
+int tfrs_listwise_bwd_f32(const float* dlds, int64_t B, int L, int reduction, float inv_temperature, const float* grad,
+                          float* dx, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K8  UnifiedEmbedding lookup (layers/feature_multiplexing/unified_embedding.py:186-215): every chunk of a feature is
  * tf-keras Hashing(num_bins = table rows, salt) followed by an embedding lookup in a table shared with other features.
  *   bin = SipHash-2-4(k0 = salt[0], k1 = salt[1], message) mod num_bins   (tf.strings.to_hash_bucket_strong)

@@ -22,6 +22,7 @@ c_i = ctypes.c_int
 c_l = ctypes.c_int64
 c_f = ctypes.c_float
 c_sz = ctypes.c_size_t
+c_u32 = ctypes.c_uint32
 
 _SIGNATURES = {
     "tfrs_version": (c_i, []),
@@ -110,6 +111,10 @@ _SIGNATURES = {
     "tfrs_ranking_loss_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p, c_f, c_i, c_p, c_sz, c_p]),
     "tfrs_ranking_loss_bwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_ranking_metrics_f32": (c_i, [c_p, c_p, c_p, c_l, c_p, c_f, c_i, c_p, c_sz, c_p]),
+    "tfrs_listwise_workspace_bytes": (c_sz, [c_l, c_i]),
+    "tfrs_listwise_fwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_i, c_f, c_u32, c_u32, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p,
+                                    c_sz, c_p]),
+    "tfrs_listwise_bwd_f32": (c_i, [c_p, c_l, c_i, c_i, c_f, c_p, c_p, c_p]),
     "tfrs_hash_bins": (c_i, [c_p, c_p, c_i, c_l, c_p, c_l, c_p, c_p]),
     "tfrs_unified_lookup_fwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),
     "tfrs_unified_lookup_bwd_f32": (c_i, [c_p, c_i, c_p, c_i, c_p]),

@@ -1,7 +1,8 @@
 """A minimal stand-in for the slice of `tf.data.Dataset` the reference's retrieval path uses
 (`from_tensor_slices`, `batch`, `zip`, `map`, iteration) so candidate corpora can be written the same
 way as in the reference (`tf.data.Dataset.from_tensor_slices(c).batch(128)`, README.md:71).
-Elements are CUDA torch tensors (embeddings / integer ids) or NumPy arrays (e.g. string identifiers)."""
+Elements are CUDA torch tensors (embeddings / integer ids) or NumPy arrays (e.g. string identifiers), or tuples or dicts of
+them."""
 from __future__ import annotations
 
 from typing import Callable, Iterable, Iterator, List, Sequence, Tuple, Union
@@ -9,18 +10,22 @@ from typing import Callable, Iterable, Iterator, List, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-Element = Union[torch.Tensor, np.ndarray, Tuple]
+Element = Union[torch.Tensor, np.ndarray, Tuple, dict]
 
 
 def _slice(x, lo, hi):
   if isinstance(x, tuple):
     return tuple(_slice(e, lo, hi) for e in x)
+  if isinstance(x, dict):
+    return {k: _slice(v, lo, hi) for k, v in x.items()}
   return x[lo:hi]
 
 
 def _len(x) -> int:
   if isinstance(x, tuple):
     return _len(x[0])
+  if isinstance(x, dict):
+    return _len(next(iter(x.values())))
   return int(x.shape[0])
 
 
@@ -36,6 +41,14 @@ class Dataset:
 
   @staticmethod
   def from_tensor_slices(tensors) -> "Dataset":
+    if isinstance(tensors, dict):
+      tensors = {k: v if isinstance(v, (torch.Tensor, np.ndarray)) else np.asarray(v) for k, v in tensors.items()}
+      if not tensors:
+        raise ValueError("from_tensor_slices needs at least one feature")
+      n = _len(tensors)
+      if any(_len(v) != n for v in tensors.values()):
+        raise ValueError(f"All features have to have the same batch dimension. Got { {k: _len(v) for k, v in tensors.items()} }.")
+      return _Slices(tensors)
     if isinstance(tensors, list):
       tensors = tuple(tensors)
     if isinstance(tensors, tuple):

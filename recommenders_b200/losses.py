@@ -1,5 +1,9 @@
-"""The tf.keras loss objects the ranking tutorials pass to `tasks.Ranking` (BinaryCrossentropy, MeanSquaredError), computed
-by the fused ranking-loss kernel.  Predictions and labels are [B] or [B, 1]: one example per row."""
+"""The loss objects the ranking tutorials pass to `tasks.Ranking`.
+
+The tf.keras pointwise losses (BinaryCrossentropy, MeanSquaredError) run in the fused ranking-loss kernel; predictions and
+labels are [B] or [B, 1], one example per row.  TF-Ranking's listwise losses (ListMLELoss, PairwiseHingeLoss, SoftmaxLoss)
+run in the fused per-list kernel K13; predictions and labels are [B, L] (or [B, L, 1]), one list per row, and an item with
+label < 0 is padding.  Their rules are in DESIGN.md §2 (A18)."""
 from __future__ import annotations
 
 from typing import Optional
@@ -81,3 +85,86 @@ class MeanSquaredError(Loss):
 
   def _inputs(self, y_pred):
     return y_pred, ops.LOSS_MSE
+
+
+class ListwiseLoss:
+  """Base of TF-Ranking's listwise Keras losses (`tfr.keras.losses`): `loss(y_true, y_pred, sample_weight=None)` on [B, L]
+  lists with one weight per list ([B] or [B, 1]) and the Keras reductions (AUTO = SUM_OVER_BATCH_SIZE: sum_b w_b l_b / B;
+  SUM; NONE: the weighted per-list losses [B]).  Scores are divided by `temperature` (one fp32 multiply by 1/T)."""
+
+  _mode = None
+
+  def __init__(self, reduction: str = Reduction.AUTO, name: Optional[str] = None, lambda_weight=None, temperature: float = 1.0,
+               ragged: bool = False):
+    if reduction not in _REDUCTIONS:
+      raise ValueError(f"Invalid Reduction Key: {reduction}. Expected keys are {tuple(_REDUCTIONS)}")
+    if lambda_weight is not None:
+      raise NotImplementedError(f"{type(self).__name__}: lambda_weight is not supported")
+    if ragged:
+      raise NotImplementedError(f"{type(self).__name__}: ragged inputs are not supported")
+    if not temperature > 0:
+      raise ValueError(f"temperature must be > 0, got {temperature}")
+    self.reduction = reduction
+    self.name = name
+    self.lambda_weight = lambda_weight
+    self.temperature = float(temperature)
+    self.ragged = ragged
+
+  def _key(self):
+    """(seed, call) of ListMLE's tie order; 0 for the other losses."""
+    return 0, 0
+
+  def _compute(self, y_true, y_pred, sample_weight=None, ndcg_stats=None, topn=None) -> torch.Tensor:
+    seed, call = self._key()
+    return ops.listwise_loss(y_pred, y_true, sample_weight, self._mode, _REDUCTIONS[self.reduction], self.temperature, seed, call,
+                             ndcg_stats, topn)
+
+  def __call__(self, y_true, y_pred, sample_weight=None) -> torch.Tensor:
+    return self._compute(y_true, y_pred, sample_weight)
+
+  def get_config(self):
+    return {"reduction": self.reduction, "name": self.name, "lambda_weight": self.lambda_weight, "temperature": self.temperature,
+            "ragged": self.ragged}
+
+
+class ListMLELoss(ListwiseLoss):
+  """tfr.keras.losses.ListMLELoss: the negative log-likelihood of the label-sorted permutation under the Plackett-Luce model,
+  l = sum_k log sum_{j >= k} exp(s_pi(j)) - s_pi(k).  Label ties are broken by a hash of (seed, call, list, item), `call` being
+  this object's call counter, so every call shuffles ties differently and reproducibly."""
+
+  _mode = ops.LIST_LOSS_LISTMLE
+
+  def __init__(self, reduction: str = Reduction.AUTO, name: str = "list_mle_loss", lambda_weight=None, temperature: float = 1.0,
+               ragged: bool = False, seed: Optional[int] = None):
+    super().__init__(reduction, name, lambda_weight, temperature, ragged)
+    self.seed = seed
+    self._calls = 0
+
+  def _key(self):
+    call = self._calls
+    self._calls += 1
+    return (0 if self.seed is None else int(self.seed)), call
+
+  def get_config(self):
+    return {**super().get_config(), "seed": self.seed}
+
+
+class PairwiseHingeLoss(ListwiseLoss):
+  """tfr.keras.losses.PairwiseHingeLoss: the mean over the list's pairs (y_i > y_j) of max(0, 1 - (s_i - s_j))."""
+
+  _mode = ops.LIST_LOSS_PAIRWISE_HINGE
+
+  def __init__(self, reduction: str = Reduction.AUTO, name: str = "pairwise_hinge_loss", lambda_weight=None,
+               temperature: float = 1.0, ragged: bool = False):
+    super().__init__(reduction, name, lambda_weight, temperature, ragged)
+
+
+class SoftmaxLoss(ListwiseLoss):
+  """tfr.keras.losses.SoftmaxLoss: the cross-entropy of softmax(s) against the labels normalised to sum 1, weighted by the
+  label sum: l = -sum_i y_i log_softmax(s)_i."""
+
+  _mode = ops.LIST_LOSS_SOFTMAX
+
+  def __init__(self, reduction: str = Reduction.AUTO, name: str = "softmax_loss", lambda_weight=None, temperature: float = 1.0,
+               ragged: bool = False):
+    super().__init__(reduction, name, lambda_weight, temperature, ragged)

@@ -337,6 +337,50 @@ class AUC(_RankingMetric):
     return float(np.sum((fpr[:-1] - fpr[1:]) * (tpr[:-1] + tpr[1:]) / 2.0))
 
 
+class NDCGMetric:
+  """tfr.keras.metrics.NDCGMetric on [B, L] lists: gain 2^y - 1, discount 1 / log2(rank + 1) truncated at `topn`, ranks by
+  prediction descending (ties to the lower item), items with label < 0 are padding; result() = sum w NDCG / sum w over every
+  update, one weight per list (a list without gain weighs the batch's mean weight).  The two sums are float64 on the device:
+  update_state runs K13's metric-only launch and never synchronises; result() reads them once.  `tasks.Ranking` with a
+  listwise loss feeds the metric from the loss launch (`_add`)."""
+
+  def __init__(self, name: str = "ndcg_metric", topn: Optional[int] = None, gain_fn=None, rank_discount_fn=None, dtype=None,
+               ragged: bool = False):
+    if gain_fn is not None or rank_discount_fn is not None:
+      raise NotImplementedError("NDCGMetric: custom gain_fn / rank_discount_fn are not supported")
+    if ragged:
+      raise NotImplementedError("NDCGMetric: ragged inputs are not supported")
+    if topn is not None and topn < 1:
+      raise ValueError(f"topn must be >= 1 or None, got {topn}")
+    self.name = name
+    self.topn = topn
+    self._acc = None
+    self._host = None
+
+  def reset_states(self) -> None:
+    if self._acc is not None:
+      self._acc.zero_()
+    self._host = None
+
+  reset_state = reset_states
+
+  def _add(self, stats: torch.Tensor) -> None:
+    if self._acc is None or self._acc.device != stats.device:
+      self._acc = torch.zeros_like(stats)
+    self._acc.add_(stats)
+    self._host = None
+
+  def update_state(self, y_true, y_pred, sample_weight=None) -> None:
+    self._add(ops.listwise_ndcg(y_pred.detach(), y_true, sample_weight, self.topn))
+
+  def result(self) -> float:
+    if self._acc is None:
+      return 0.0
+    if self._host is None:
+      self._host = self._acc.cpu().numpy()   # the one synchronisation
+    return _div_no_nan(float(self._host[0]), float(self._host[1]))
+
+
 def _flat_device(w, device) -> torch.Tensor:
   t = w if isinstance(w, torch.Tensor) else torch.as_tensor(np.asarray(w))
   return t.to(device=device, dtype=torch.float32).reshape(-1)

@@ -9,6 +9,7 @@ import ctypes
 import math
 from typing import NamedTuple, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _ffi
@@ -1588,6 +1589,123 @@ def ranking_metrics(pred: torch.Tensor, labels: torch.Tensor, sample_weight=None
   check(lib().tfrs_ranking_metrics_f32(ptr(p), ptr(y), ptr(w), B, ptr(stats), c_f(threshold), int(num_thresholds), ptr(ws), ws.numel(),
                                        stream()), "ranking_metrics")
   return stats
+
+
+# ------------------------------------------------------------------------------------------------
+# listwise losses + NDCG (K13, csrc/listwise.cu)
+# ------------------------------------------------------------------------------------------------
+LIST_LOSS_NONE, LIST_LOSS_LISTMLE, LIST_LOSS_PAIRWISE_HINGE, LIST_LOSS_SOFTMAX = 0, 1, 2, 3
+LISTWISE_MAX_LIST = 1024
+_discounts = {}
+
+
+def ndcg_discounts(device) -> torch.Tensor:
+  """discount[r - 1] = 1 / log2(r + 1) for r = 1 .. LISTWISE_MAX_LIST: computed in float64 on the host, rounded once to fp32."""
+  dev = torch.device(device)
+  key = dev.index if dev.index is not None else torch.cuda.current_device()
+  t = _discounts.get(key)
+  if t is None:
+    r = np.arange(1, LISTWISE_MAX_LIST + 1, dtype=np.float64)
+    t = torch.from_numpy((1.0 / np.log2(r + 1.0)).astype(np.float32)).to(dev)
+    _discounts[key] = t
+  return t
+
+
+def _list_tensor(t, name: str, device=None) -> torch.Tensor:
+  if not isinstance(t, torch.Tensor):
+    t = torch.as_tensor(np.asarray(t), dtype=torch.float32, device=device)
+  t = f32c(t, name)
+  if t.dim() == 3 and t.shape[-1] == 1:
+    t = t.squeeze(-1)
+  if t.dim() != 2:
+    raise ValueError(f"{name} must be [B, L] or [B, L, 1], got {tuple(t.shape)}")
+  return t.contiguous()
+
+
+def listwise_inputs(predictions, labels, sample_weight=None):
+  """(predictions [B, L], labels [B, L], per-list weights [B] or None) as contiguous fp32 device tensors."""
+  p = _list_tensor(predictions, "predictions")
+  y = _list_tensor(labels, "labels", p.device)
+  if y.shape != p.shape:
+    raise ValueError(f"labels and predictions must have the same shape ({tuple(y.shape)} vs {tuple(p.shape)})")
+  B, L = p.shape
+  if not 1 <= L <= LISTWISE_MAX_LIST:
+    raise ValueError(f"list length {L} is outside [1, {LISTWISE_MAX_LIST}]")
+  w = None
+  if sample_weight is not None:
+    w = sample_weight if isinstance(sample_weight, torch.Tensor) else torch.as_tensor(np.asarray(sample_weight), dtype=torch.float32)
+    w = w.to(device=p.device, dtype=torch.float32)
+    if w.dim() == 2 and w.shape[1] > 1:
+      raise NotImplementedError("listwise losses and NDCG take one weight per list ([B] or [B, 1]), not per-item weights")
+    if w.dim() > 2 or (w.numel() != B and w.numel() != 1):
+      raise ValueError(f"sample_weight must be [B] or [B, 1] (got {tuple(w.shape)}, B = {B})")
+    w = w.reshape(-1).expand(B).contiguous()
+  return p, y, w
+
+
+def _listwise_fwd(p, y, w, mode, reduction, inv_t, seed, call, dlds, ndcg_stats, topn, ndcg=None):
+  B, L = p.shape
+  per = torch.empty((B,), dtype=torch.float32, device=p.device) if mode != LIST_LOSS_NONE and reduction == REDUCTION_NONE else None
+  loss = torch.empty((1,), dtype=torch.float32, device=p.device) if mode != LIST_LOSS_NONE and reduction != REDUCTION_NONE else None
+  disc = ndcg_discounts(p.device) if (ndcg_stats is not None or ndcg is not None) else None
+  ws = workspace(lib().tfrs_listwise_workspace_bytes(B, L), p.device, "listwise")
+  check(lib().tfrs_listwise_fwd_f32(ptr(p), ptr(y), ptr(w), B, L, mode, reduction, c_f(inv_t), seed & 0xFFFFFFFF, call & 0xFFFFFFFF,
+                                    ptr(per), ptr(loss), ptr(dlds), ptr(disc), int(topn or 0), ptr(ndcg), ptr(ndcg_stats), ptr(ws),
+                                    ws.numel(), stream()), "listwise_fwd")
+  if mode == LIST_LOSS_NONE:
+    return None
+  return per if reduction == REDUCTION_NONE else loss.view(())
+
+
+class _ListwiseLoss(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, pred, p, y, w, mode, reduction, inv_t, seed, call, ndcg_stats, topn):
+    dlds = torch.empty_like(p) if ctx.needs_input_grad[0] else None
+    out = _listwise_fwd(p, y, w, mode, reduction, inv_t, seed, call, dlds, ndcg_stats, topn)
+    if dlds is not None:
+      ctx.save_for_backward(dlds)
+    ctx.reduction, ctx.inv_t, ctx.shape = reduction, inv_t, pred.shape
+    return out
+
+  @staticmethod
+  def backward(ctx, g):
+    dlds, = ctx.saved_tensors
+    B, L = dlds.shape
+    g = f32c(g, "grad").reshape(-1)
+    dx = torch.empty_like(dlds)
+    check(lib().tfrs_listwise_bwd_f32(ptr(dlds), B, L, ctx.reduction, c_f(ctx.inv_t), ptr(g), ptr(dx), stream()), "listwise_bwd")
+    return (dx.view(ctx.shape),) + (None,) * 10
+
+
+def listwise_loss(predictions: torch.Tensor, labels, sample_weight=None, mode: int = LIST_LOSS_SOFTMAX,
+                  reduction: int = REDUCTION_SUM_OVER_BATCH_SIZE, temperature: float = 1.0, seed: int = 0, call: int = 0,
+                  ndcg_stats: Optional[torch.Tensor] = None, topn: Optional[int] = None) -> torch.Tensor:
+  """A TF-Ranking listwise loss (K13) of [B, L] (or [B, L, 1]) predictions: the reduced loss (0-dim) or, for REDUCTION_NONE,
+  the weighted per-list losses [B].  `ndcg_stats` (float64 [2], nullable) receives [sum w ndcg, sum w] at `topn` from the same
+  launch.  Differentiable in `predictions`; the backward is one scaling launch."""
+  if mode == LIST_LOSS_NONE:
+    raise ValueError("listwise_loss needs a loss mode")
+  if not temperature > 0 or not np.isfinite(temperature):
+    raise ValueError(f"temperature must be finite and > 0, got {temperature}")
+  p, y, w = listwise_inputs(predictions, labels, sample_weight)
+  inv_t = float(np.float32(1.0 / float(temperature)))
+  return _ListwiseLoss.apply(predictions, p, y, w, int(mode), int(reduction), inv_t, int(seed), int(call), ndcg_stats, topn)
+
+
+def ndcg_stats_buffer(device) -> torch.Tensor:
+  return torch.empty((2,), dtype=torch.float64, device=device)
+
+
+@torch.no_grad()
+def listwise_ndcg(predictions: torch.Tensor, labels, sample_weight=None, topn: Optional[int] = None, per_list: bool = False):
+  """The NDCG statistics [sum w ndcg, sum w] of one batch (float64 device tensor) from K13's metric-only launch; with
+  per_list=True also every list's NDCG [B] (fp32)."""
+  p, y, w = listwise_inputs(predictions, labels, sample_weight)
+  stats = ndcg_stats_buffer(p.device)
+  nd = torch.empty((p.shape[0],), dtype=torch.float32, device=p.device) if per_list else None
+  _listwise_fwd(p, y, w, LIST_LOSS_NONE, REDUCTION_SUM, 1.0, 0, 0, None, stats, topn, nd)
+  return (stats, nd) if per_list else stats
 
 
 def launch_count() -> int:

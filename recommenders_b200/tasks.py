@@ -164,7 +164,9 @@ class Ranking(torch.nn.Module, Task):
   A loss object of this package (`losses.BinaryCrossentropy` -- the default -- or `losses.MeanSquaredError`) runs in the
   fused ranking-loss kernel, and that same launch produces the batch statistics of every package metric of the call
   (BinaryAccuracy, AUC, (Root)MeanSquaredError, and `Mean` as a prediction / label metric); the metrics add them into their
-  device-resident sums.  Any other callable loss, or any other object with `update_state`, is called as is."""
+  device-resident sums.  A listwise loss (`losses.ListMLELoss`, `PairwiseHingeLoss`, `SoftmaxLoss`) runs in the fused per-list
+  kernel, and that launch also computes the NDCG of the call's `NDCGMetric`s that share the first one's topn.  Any other
+  callable loss, or any other object with `update_state`, is called as is."""
 
   def __init__(self, loss: Optional[Callable] = None, metrics: Optional[List] = None, prediction_metrics: Optional[List] = None,
                label_metrics: Optional[List] = None, loss_metrics: Optional[List] = None, name: Optional[Text] = None) -> None:
@@ -201,14 +203,24 @@ class Ranking(torch.nn.Module, Task):
       return None
     return (0.5 if thr is None else thr), (2 if T is None else T), fused
 
+  def _ndcg_plan(self):
+    """The NDCGMetrics that share the first one's topn: a listwise loss's launch computes their statistics."""
+    ndcg = [m for m in self._ranking_metrics if isinstance(m, tfrs_metrics.NDCGMetric)]
+    return [m for m in ndcg if m.topn == ndcg[0].topn]
+
   def call(self, labels: torch.Tensor, predictions: torch.Tensor, sample_weight: Optional[torch.Tensor] = None,
            training: bool = False, compute_metrics: bool = True) -> torch.Tensor:
     own_loss = isinstance(self._loss, tfrs_losses.Loss)
+    listwise = isinstance(self._loss, tfrs_losses.ListwiseLoss)
     if not isinstance(labels, torch.Tensor):
       labels = torch.as_tensor(labels, dtype=torch.float32, device=predictions.device)
     plan = self._stats_plan() if compute_metrics else None
     stats = None
-    if own_loss:
+    ndcg_fused = self._ndcg_plan() if (listwise and compute_metrics) else []
+    ndcg_stats = ops.ndcg_stats_buffer(predictions.device) if ndcg_fused else None
+    if listwise:   # one K13 launch: the list loss and the NDCG of the metrics that share the first one's topn
+      loss = self._loss._compute(labels, predictions, sample_weight, ndcg_stats, ndcg_fused[0].topn if ndcg_fused else None)
+    elif own_loss:
       stats = None if plan is None else ops.ranking_stats_buffer(plan[1], predictions.device)
       loss = self._loss._compute(labels, predictions, sample_weight, stats, *(plan[:2] if plan else ()))
     else:
@@ -219,9 +231,12 @@ class Ranking(torch.nn.Module, Task):
       if plan is not None and stats is None:
         stats = ops.ranking_metrics(predictions.detach(), labels, sample_weight, plan[0], plan[1])
       fused = set(map(id, plan[2])) if plan else set()
+      fused_ndcg = set(map(id, ndcg_fused))
       for metric in self._ranking_metrics:
         if id(metric) in fused:
           metric._add(stats)
+        elif id(metric) in fused_ndcg:
+          metric._add(ndcg_stats)
         else:
           metric.update_state(y_true=labels, y_pred=predictions.detach(), sample_weight=sample_weight)
       for metrics, slot, values in ((self._prediction_metrics, 2, predictions), (self._label_metrics, 3, labels)):
