@@ -53,7 +53,7 @@ int64_t tfrs_launch_count(void);
  *   out[i, out_col_off[t] .. +dims[t]) = tables[t][ids[t][i], :]     for t < n_tables, i < n
  * Writes straight into a concatenated [n, out_ld] activation (the layout Cross consumes).
  * Out-of-range ids produce zero rows.  dims[t] % 4 == 0 and 16-byte aligned rows take the
- * vectorised path; anything else a scalar path.
+ * vectorised path; anything else a scalar path.  n == 0 writes nothing (out and ids may be NULL).
  * ------------------------------------------------------------------------------------------- */
 int tfrs_gather_f32(const float* const* tables, const int64_t* rows, const int32_t* dims, int n_tables,
                     const void* const* ids, int ids_dtype, int64_t n, float* out, int64_t out_ld,
@@ -688,6 +688,7 @@ int tfrs_tree_ah_search_f32(const float* q, int64_t Q, int d, const float* centr
  * (self_interaction=0) or with the diagonal, [B, out_dim], or the full [B,F*F] matrix with the excluded part
  * zeroed (skip_gather=1).  Every dot is the canonical sequential fmaf chain.  F <= 64.
  * Backward: dfeats[b,i,:] = sum_j G'(i,j) feats[b,j,:] with G' the symmetrised upstream gradient.
+ * B == 0 writes nothing (pointers may be NULL); gout may be NULL when the output width is 0.
  * ------------------------------------------------------------------------------------------- */
 int tfrs_dot_interaction_out_dim(int F, int self_interaction, int skip_gather);
 int tfrs_dot_interaction_fwd_f32(const float* feats, int64_t B, int F, int d, int self_interaction, int skip_gather,

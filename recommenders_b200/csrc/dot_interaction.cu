@@ -96,7 +96,7 @@ extern "C" int tfrs_dot_interaction_out_dim(int F, int self_interaction, int ski
 }
 
 static int di_check(const float* feats, int64_t B, int F, int d) {
-  TFRS_CHECK_ARG(feats && B >= 0 && F > 0 && d > 0, "dot_interaction: bad arguments");
+  TFRS_CHECK_ARG((feats || B == 0) && B >= 0 && F > 0 && d > 0, "dot_interaction: bad arguments");  // empty batch: NULL
   if (F > DI_MAX_F || (size_t)DI_WARPS * (F * (d + 1) + F * F) * 4 > 200 * 1024) {
     set_error("dot_interaction: F=%d, d=%d outside the shared-memory staging range (F <= %d)", F, d, DI_MAX_F);
     return TFRS_ERR_UNSUPPORTED;
@@ -123,9 +123,10 @@ extern "C" int tfrs_dot_interaction_bwd_f32(const float* feats, const float* gou
                                             int skip_gather, float* dfeats, void* stream) {
   int rc = di_check(feats, B, F, d);
   if (rc) return rc;
-  TFRS_CHECK_ARG(gout && dfeats, "dot_interaction_bwd: NULL pointer");
   if (B == 0) return TFRS_OK;
   const int od = di_out_dim(F, self_interaction, skip_gather);
+  // a single feature without self-interaction has no outputs: its upstream gradient is empty (NULL) and dE is zero
+  TFRS_CHECK_ARG(dfeats && (gout || od == 0), "dot_interaction_bwd: NULL pointer");
   const size_t smem = (size_t)DI_WARPS * (F * (d + 1) + od) * 4;
   TFRS_DYN_SMEM(dot_interaction_bwd_kernel, 200 * 1024);
   dot_interaction_bwd_kernel<<<(unsigned)ceil_div(B, DI_WARPS), DI_WARPS * 32, smem, (cudaStream_t)stream>>>(

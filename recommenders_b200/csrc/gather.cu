@@ -165,10 +165,11 @@ using namespace tfrs;
 extern "C" int tfrs_gather_f32(const float* const* tables, const int64_t* rows, const int32_t* dims, int n_tables,
                                const void* const* ids, int ids_dtype, int64_t n, float* out, int64_t out_ld,
                                const int32_t* out_col_off, void* stream) {
-  TFRS_CHECK_ARG(n_tables > 0 && tables && rows && dims && ids && out && out_col_off, "gather: NULL argument");
+  TFRS_CHECK_ARG(n_tables > 0 && tables && rows && dims && ids && out_col_off, "gather: NULL argument");
   TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "gather: ids_dtype must be I32 or I64");
   TFRS_CHECK_ARG(n >= 0 && out_ld > 0, "gather: bad n / out_ld");
-  if (n == 0) return TFRS_OK;
+  if (n == 0) return TFRS_OK;  // an empty batch: the output (and every id array) may be NULL, as empty tensors are
+  TFRS_CHECK_ARG(out, "gather: NULL output");
   cudaStream_t st = (cudaStream_t)stream;
   for (int t0 = 0; t0 < n_tables; t0 += GT_MAX_TABLES) {
     int nt = n_tables - t0 < GT_MAX_TABLES ? n_tables - t0 : GT_MAX_TABLES;
