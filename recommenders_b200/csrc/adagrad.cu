@@ -234,10 +234,11 @@ ag_apply_long(const unsigned long long* __restrict__ keys, long long n, const fl
     for (long long m0 = i; m0 < end; m0 += tile_rows) {
       const int rows_here = (int)min((long long)tile_rows, end - m0);
       // the tile's gradient-row numbers first (one coalesced read), then every thread has 4 independent 16-byte row
-      // loads in flight: one DRAM round trip per tile instead of one per element
+      // loads in flight: one DRAM round trip per tile instead of one per element.  float4 only when every row starts on
+      // a 16-byte boundary: a contiguous view may start 4, 8 or 12 bytes into its storage
       if ((int)threadIdx.x < rows_here) pos_sh[threadIdx.x] = (unsigned int)(keys[m0 + threadIdx.x] & 0xFFFFFFull);
       __syncthreads();
-      if ((d & 3) == 0) {
+      if ((d & 3) == 0 && (reinterpret_cast<uintptr_t>(grad) & 15) == 0) {
         const unsigned int d4 = (unsigned int)d >> 2, total4 = (unsigned int)rows_here * d4;
         for (unsigned int e0 = threadIdx.x; e0 < total4; e0 += AL_THREADS * 4) {
           float4 v[4];

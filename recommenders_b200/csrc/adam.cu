@@ -52,7 +52,8 @@ __device__ __forceinline__ void ad_decay(float& var, float& m, float& v, const A
 }
 
 // The untouched-row rule on every row whose bit is clear.  A thread walks the (row, column group) pairs of a grid-stride
-// loop by increments, so no element pays a 64-bit division.  V = 4: float4 groups (d % 4 == 0), V = 1: single columns.
+// loop by increments, so no element pays a 64-bit division.  V = 4: float4 groups (d % 4 == 0 and table, m and v 16-byte
+// aligned), V = 1: single columns.
 template <int V>
 __global__ void __launch_bounds__(256)
 ad_decay_untouched(float* __restrict__ table, float* __restrict__ m, float* __restrict__ v, long long rows, int groups,
@@ -143,7 +144,9 @@ extern "C" int tfrs_sparse_adam_f32(float* table, float* m, float* v, int64_t ro
     if ((rc = ag_run_sums(gr, n, grad_rows, d, AdamRowOp{table, m, v, touched, k}, st)) != TFRS_OK) return rc;
   }
   if (touched) {
-    const int V = (d & 3) == 0 ? 4 : 1;
+    // float4 groups only when table, m and v all start on a 16-byte boundary (a contiguous view need not)
+    const bool aligned = ((reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15) == 0;
+    const int V = (d & 3) == 0 && aligned ? 4 : 1;
     const unsigned grid = elementwise_grid(rows * (d / V));
     if (V == 4) ad_decay_untouched<4><<<grid, 256, 0, st>>>(table, m, v, rows, d / 4, touched, k);
     else ad_decay_untouched<1><<<grid, 256, 0, st>>>(table, m, v, rows, d, touched, k);
