@@ -140,6 +140,12 @@ int tfrs_topk_tc_layout(int64_t Q, int64_t N, int d, int k, int64_t* out10);
  * at the tfrs_topk_tc_layout offset is the one whose records the workspace holds: thr_safe for a retried row. */
 int tfrs_topk_tc_retry_layout(int64_t Q, int64_t N, int d, int k, int64_t* out4);
 
+/* The sampled pass on a norm-sample index (tfrs_index_build takes the floor(N/8) rows of largest norm as the sample
+ * when N >= 2^19 and the norm spread predicts a tighter bound): out8 = {bin-maxima offset (float [padded Q, bins_ld]),
+ * bins_ld, bins, tiles per bin, bins per corpus part and column half, corpus parts, sample tiles, margin offset
+ * (float [padded Q])}.  Bins = 0: the shape has no norm-sample layout. */
+int tfrs_topk_tc_sample_layout(int64_t Q, int64_t N, int d, int k, int64_t* out8);
+
 /* Optional per-stage device timing of tfrs_topk_tc_f32 (CUDA events on the launch stream; used by
  * bench.py for the roofline figure).  tfrs_profile_read synchronises the device and returns the summed
  * times in ms of stage 0 = query image, 1 = sampled pass + threshold, 2 = full filter pass (the

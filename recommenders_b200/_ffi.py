@@ -42,6 +42,7 @@ _SIGNATURES = {
     "tfrs_topk_hits_accumulate": (c_i, [c_p, c_p, c_p, c_l, c_p, c_i, c_p, c_p]),
     "tfrs_topk_tc_layout": (c_i, [c_l, c_l, c_i, c_i, c_p]),
     "tfrs_topk_tc_retry_layout": (c_i, [c_l, c_l, c_i, c_i, c_p]),
+    "tfrs_topk_tc_sample_layout": (c_i, [c_l, c_l, c_i, c_i, c_p]),
     "tfrs_dot_interaction_out_dim": (c_i, [c_i, c_i, c_i]),
     "tfrs_dot_interaction_fwd_f32": (c_i, [c_p, c_l, c_i, c_i, c_i, c_i, c_p, c_p]),
     "tfrs_dot_interaction_bwd_f32": (c_i, [c_p, c_p, c_l, c_i, c_i, c_i, c_i, c_p, c_p]),

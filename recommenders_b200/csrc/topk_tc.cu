@@ -7,7 +7,8 @@
 //                K-major tiles (one contiguous 16 KB block per 64-wide K slab), + max row norm (scaled units).
 //   query time   (0) tc_qprep     : ONE kernel, a warp per query: per-ROW power-of-two rescale (scores of different
 //                    queries are never compared, so every query gets its own exponent), fp16 tile image, error margins
-//                (1) tc_scan<SAMPLE> : screening GEMM over every 4th corpus tile; each epilogue thread keeps the maximum
+//                (1) tc_scan<SAMPLE> : screening GEMM over every 4th corpus tile (or, on an index that chose it, the
+//                    highest-norm eighth of the corpus, see SAMPLE_NORM); each epilogue thread keeps the maximum
 //                    of a GROUP of tiles (a "bin") -> <= 1024 bins per query; tc_threshold (a warp per query, bins in
 //                    registers) takes the K-th largest bin maximum L_q: K distinct bins hold K distinct candidates
 //                    >= L_q, so L_q is a valid lower bound of the K-th best screening score; top-K and EXCLUDE calls
@@ -73,11 +74,37 @@ struct SideStats {              // corpus side, written at index time
   int exp;                      // rescale exponent e: x * 2^e has its largest magnitude in [2^14, 2^15)
   int pad;
 };
+// Sample of the sampled pass, chosen per index at build time (tfrs_index_build):
+//   SAMPLE_STRIDED  every stride-th tile of the corpus image (Plan::stride)
+//   SAMPLE_NORM     the norm-sample image: the floor(N/8) rows of largest norm (rounded down to whole tiles), in index
+//                   order, stored after the corpus image.  Winners of a dot-product top-K have above-average norms, so
+//                   half the strided sample's rows give as tight a k-th bin bound.  Taken when N >= 2^19 and both
+//                   (a) the random-direction model (norm_phi_*) gives the sample phi >= 0.35 of the expected top 1e-4;
+//                   (b) probe queries made of corpus rows find their neighbours in the sample: the model cannot see
+//                       queries that align with groups of rows (a clustered corpus, whose high-norm clusters are not
+//                       every query's own), where the sample's bound is loose and rows would take the exact fallback.
+//                       NORM_PROBES evenly spaced rows, each scored against the corpus (the exact top-(K+1) of the
+//                       strided-sample path, itself dropped): the share of each probe's K neighbours that lie in the
+//                       sample must average >= 0.35 and be >= 0.25 (the strided sample's own share) for every probe.
+// The choice is made once, at build; a query call never writes the index.
+enum { SAMPLE_STRIDED = 0, SAMPLE_NORM = 1 };
+constexpr long long NORM_SAMPLE_MIN_N = 1ll << 19;   // below this the sample's tiles cannot fill the bins
+constexpr int NORM_SAMPLE_DIV = 8;                   // sample rows = N / 8
+constexpr double NORM_SAMPLE_TAIL = 1e-4;            // phi is measured on the expected top N * 1e-4 scores
+constexpr double NORM_SAMPLE_MIN_PHI = 0.35;
+constexpr int NORM_PROBES = 256, NORM_PROBE_K = 100;
+constexpr float NORM_PROBE_MIN_MEAN = 0.35f, NORM_PROBE_MIN_EACH = 0.25f;
 struct IndexHeader {
   SideStats st;
-  int d, d_pad, kb, pad;
+  int d, d_pad, kb, sample;   // sample: SAMPLE_STRIDED / SAMPLE_NORM
   long long n, n_tiles;
+  float phi;                  // the norm sample's phi (0 below NORM_SAMPLE_MIN_N)
+  float probe_mean, probe_min;   // the probes' neighbour share in the sample (0 below NORM_SAMPLE_MIN_N)
 };
+// tiles of the norm-sample image of an N-row corpus (0: the index has none)
+__host__ __device__ inline long long norm_sample_tiles(long long N) {
+  return N >= NORM_SAMPLE_MIN_N && N < (1ll << 31) ? N / NORM_SAMPLE_DIV / 128 : 0;
+}
 
 __device__ __forceinline__ int rescale_exp(float amax) {
   int x = 0;
@@ -92,7 +119,8 @@ __device__ __forceinline__ int rescale_exp(float amax) {
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 tile_image_kernel(const float* __restrict__ src, long long rows, int d, int kb, long long n_tiles,
-                  const SideStats* __restrict__ st, unsigned char* __restrict__ img) {
+                  const SideStats* __restrict__ st, unsigned char* __restrict__ img, const int* __restrict__ rowmap) {
+  // rowmap (norm-sample image): image row i holds corpus row rowmap[i], with the same bits as in the corpus image
   const int scale_exp = st->exp;
   const long long total = n_tiles * TILE_N * (long long)kb * 8;  // 16-byte chunks
   for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256) {
@@ -102,10 +130,11 @@ tile_image_kernel(const float* __restrict__ src, long long rows, int d, int kb, 
     int r = (int)(row % TILE_N);
     long long tile = row / TILE_N;
     int k0 = slab * KSLAB + cj * 8;
+    const long long srow = (rowmap != nullptr && row < rows) ? (long long)rowmap[row] : row;
     __align__(16) __half v[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      float f = (row < rows && k0 + j < d) ? src[row * d + k0 + j] : 0.f;
+      float f = (row < rows && k0 + j < d) ? src[srow * d + k0 + j] : 0.f;
       v[j] = __float2half_rn(ldexpf(f, scale_exp));  // exact power-of-two rescale, then one rounding to fp16
     }
     unsigned char* dst = img + tile * ((long long)kb * SLAB_BYTES) + (long long)slab * SLAB_BYTES + r * 128 + ((cj ^ (r & 7)) * 16);
@@ -117,7 +146,8 @@ tile_image_kernel(const float* __restrict__ src, long long rows, int d, int kb, 
 // of the SCALED rows (so tiny or huge corpora neither underflow nor overflow the fp32 norm)
 template <int PASS>
 __global__ void __launch_bounds__(256)
-corpus_stats_kernel(const float* __restrict__ src, long long rows, int d, SideStats* __restrict__ st) {
+corpus_stats_kernel(const float* __restrict__ src, long long rows, int d, SideStats* __restrict__ st,
+                    unsigned int* __restrict__ norm2_key = nullptr) {   // PASS 1: each row's scaled norm^2 (float bits)
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * 256) >> 5;
@@ -135,6 +165,7 @@ corpus_stats_kernel(const float* __restrict__ src, long long rows, int d, SideSt
       const float other = __shfl_xor_sync(0xffffffffu, acc, o);
       acc = PASS ? acc + other : fmaxf(acc, other);
     }
+    if (PASS && norm2_key != nullptr && lane == 0) norm2_key[row] = __float_as_uint(acc);   // >= 0: uint order == float order
     best = fmaxf(best, acc);
   }
   if (lane == 0 && best > 0.f) {
@@ -144,6 +175,174 @@ corpus_stats_kernel(const float* __restrict__ src, long long rows, int d, SideSt
 }
 __global__ void side_exp_kernel(SideStats* st) { st->exp = rescale_exp(__uint_as_float(st->amax_bits)); }
 __global__ void header_kernel(IndexHeader* dst, IndexHeader h) { *dst = h; }
+
+// ---- norm sample (index time, all on the device; every reduction in a fixed order, so the index is deterministic) ----
+// State of the build in scratch memory.  The S-th largest norm key T is found bit by bit, from the top: cnt[b] =
+// #{key >= prefix | 2^b} with the bits above b decided by cnt[31..b+1] (norm_select_prefix), so one kernel per bit.
+struct NormSelect {
+  unsigned long long cnt[32];
+  long long need;      // rows with key == T that join the sample (the lowest indices among them)
+  double lo, hi;       // bisection bracket of the tail point t (norm_phi_*)
+};
+constexpr int NS_CHUNK = 8192;   // rows per block in the compaction and the phi sums (256 threads x 32)
+
+__device__ __forceinline__ unsigned int norm_select_prefix(const NormSelect* s, long long S, int lowest) {
+  unsigned int prefix = 0u;
+  for (int b = 31; b > lowest; --b)
+    if (s->cnt[b] >= (unsigned long long)S) prefix |= 1u << b;
+  return prefix;
+}
+
+__global__ void __launch_bounds__(256)
+norm_select_count_kernel(const unsigned int* __restrict__ key, long long n, long long S, int bit, NormSelect* s) {
+  const unsigned int cand = norm_select_prefix(s, S, bit) | (1u << bit);
+  unsigned int c = 0;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) c += key[i] >= cand ? 1u : 0u;
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s->cnt[bit], (unsigned long long)c);
+}
+
+// per chunk: #{key > T}, #{key == T}
+__global__ void __launch_bounds__(256)
+norm_select_chunks_kernel(const unsigned int* __restrict__ key, long long n, long long S, const NormSelect* s, int* __restrict__ blk) {
+  __shared__ int sh[2];
+  const unsigned int T = norm_select_prefix(s, S, -1);
+  if (threadIdx.x == 0) { sh[0] = 0; sh[1] = 0; }
+  __syncthreads();
+  int gt = 0, eq = 0;
+  const long long r0 = (long long)blockIdx.x * NS_CHUNK;
+  for (int t = threadIdx.x; t < NS_CHUNK; t += 256) {
+    const long long i = r0 + t;
+    if (i < n) { gt += key[i] > T ? 1 : 0; eq += key[i] == T ? 1 : 0; }
+  }
+  gt = __reduce_add_sync(0xffffffffu, gt); eq = __reduce_add_sync(0xffffffffu, eq);
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&sh[0], gt); atomicAdd(&sh[1], eq); }
+  __syncthreads();
+  if (threadIdx.x == 0) { blk[2 * blockIdx.x] = sh[0]; blk[2 * blockIdx.x + 1] = sh[1]; }
+}
+
+// one thread: chunk counts -> each chunk's first sample position and first tie rank (in place), and `need`
+__global__ void norm_select_offsets_kernel(int* __restrict__ blk, int nblk, long long S, NormSelect* s) {
+  long long gt = 0;
+  for (int b = 0; b < nblk; ++b) gt += blk[2 * b];
+  const long long need = S - gt;
+  long long sel = 0, eq = 0;
+  for (int b = 0; b < nblk; ++b) {
+    const long long g = blk[2 * b], e = blk[2 * b + 1];
+    const long long take = need - eq < 0 ? 0 : (need - eq < e ? need - eq : e);
+    blk[2 * b] = (int)sel; blk[2 * b + 1] = (int)eq;
+    sel += g + take; eq += e;
+  }
+  s->need = need;
+}
+
+// stable compaction: rowlist[] = the rows with key > T and the first `need` rows with key == T, in index order
+__global__ void __launch_bounds__(256)
+norm_select_write_kernel(const unsigned int* __restrict__ key, long long n, long long S, const NormSelect* s,
+                         const int* __restrict__ blk, int* __restrict__ rowlist) {
+  __shared__ int wsel[8], weq[8];
+  const unsigned int T = norm_select_prefix(s, S, -1);
+  const long long need = s->need;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int lt = (1u << lane) - 1u;
+  int sel_base = blk[2 * blockIdx.x], eq_base = blk[2 * blockIdx.x + 1];
+  const long long r0 = (long long)blockIdx.x * NS_CHUNK;
+  for (int t0 = 0; t0 < NS_CHUNK; t0 += 256) {
+    const long long i = r0 + t0 + threadIdx.x;
+    const unsigned int k = i < n ? key[i] : 0u;
+    const bool is_eq = i < n && k == T;
+    const unsigned int veq = __ballot_sync(0xffffffffu, is_eq);
+    if (lane == 0) weq[warp] = __popc(veq);
+    __syncthreads();
+    int eq_before = eq_base, eq_all = 0;
+    for (int w = 0; w < 8; ++w) { eq_before += w < warp ? weq[w] : 0; eq_all += weq[w]; }
+    eq_before += __popc(veq & lt);
+    const bool is_sel = i < n && (k > T || (is_eq && eq_before < need));
+    const unsigned int vsel = __ballot_sync(0xffffffffu, is_sel);
+    if (lane == 0) wsel[warp] = __popc(vsel);
+    __syncthreads();
+    int sel_before = sel_base, sel_all = 0;
+    for (int w = 0; w < 8; ++w) { sel_before += w < warp ? wsel[w] : 0; sel_all += wsel[w]; }
+    if (is_sel) rowlist[sel_before + __popc(vsel & lt)] = (int)i;
+    sel_base += sel_all; eq_base += eq_all;
+    __syncthreads();
+  }
+}
+
+// Random-direction model: a row of norm r scores r g, g ~ N(0, 1), so it exceeds t with probability erfc(t / (r sqrt 2)) / 2.
+// t solves sum_i P_i(t) = N * NORM_SAMPLE_TAIL (bisection); phi = sum over the sample of P_i(t) / (N * NORM_SAMPLE_TAIL).
+__device__ __forceinline__ double norm_tail(unsigned int norm2_key, double t) {
+  const double r = sqrt((double)__uint_as_float(norm2_key));
+  return r > 0.0 ? 0.5 * erfc(t / (r * 1.4142135623730951)) : 0.0;
+}
+// per chunk: sum of P_i(t) at the bracket's midpoint over key[rows[j]] (rows == nullptr: key[j]), j < n; fixed order
+__global__ void __launch_bounds__(256)
+norm_phi_partial_kernel(const unsigned int* __restrict__ key, const int* __restrict__ rows, long long n, const NormSelect* s,
+                        double* __restrict__ partial) {
+  __shared__ double sh[256];
+  const double t = 0.5 * (s->lo + s->hi);
+  double acc = 0.0;
+  const long long r0 = (long long)blockIdx.x * NS_CHUNK;
+  for (int u = threadIdx.x; u < NS_CHUNK; u += 256) {
+    const long long j = r0 + u;
+    if (j < n) acc += norm_tail(key[rows ? (long long)rows[j] : j], t);
+  }
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) partial[blockIdx.x] = sh[0];
+}
+// one thread.  final == 0: one bisection step;  final == 1: the sample's sum -> phi, and with the probes' neighbour
+// shares (share[NORM_PROBES]) the header's choice
+__global__ void norm_phi_step_kernel(const double* __restrict__ partial, int nblk, long long N, int final, NormSelect* s,
+                                     IndexHeader* hdr, const float* __restrict__ share) {
+  double sum = 0.0;
+  for (int b = 0; b < nblk; ++b) sum += partial[b];
+  const double target = (double)N * NORM_SAMPLE_TAIL;
+  if (!final) {
+    const double t = 0.5 * (s->lo + s->hi);
+    if (sum > target) s->lo = t; else s->hi = t;
+  } else {
+    const double phi = sum / target;
+    float mean = 0.f, mn = 1.f;
+    for (int i = 0; i < NORM_PROBES; ++i) { mean += share[i]; mn = fminf(mn, share[i]); }
+    mean /= NORM_PROBES;
+    hdr->phi = (float)phi; hdr->probe_mean = mean; hdr->probe_min = mn;
+    // NaN (non-finite rows) fails every comparison: strided
+    hdr->sample = phi >= NORM_SAMPLE_MIN_PHI && mean >= NORM_PROBE_MIN_MEAN && mn >= NORM_PROBE_MIN_EACH ? SAMPLE_NORM : SAMPLE_STRIDED;
+  }
+}
+
+// probe p = corpus row p * N / NORM_PROBES; one warp per probe row: its fp32 copy
+__global__ void norm_probe_gather_kernel(const float* __restrict__ corpus, long long N, int d, float* __restrict__ probes) {
+  const int pr = blockIdx.x;
+  const long long row = (long long)pr * N / NORM_PROBES;
+  for (int t = threadIdx.x; t < d; t += 32) probes[(long long)pr * d + t] = corpus[row * d + t];
+}
+// in_sample[row] = 1 for the sample's rows
+__global__ void norm_sample_flags_kernel(const int* __restrict__ rowlist, long long S, unsigned char* __restrict__ in_sample) {
+  for (long long j = (long long)blockIdx.x * 256 + threadIdx.x; j < S; j += (long long)gridDim.x * 256) in_sample[rowlist[j]] = 1;
+}
+// one warp per probe: the share of its K best neighbours (the top K + 1 without the probe's own row) in the sample
+__global__ void norm_probe_share_kernel(const long long* __restrict__ idx, long long N, const unsigned char* __restrict__ in_sample,
+                                        float* __restrict__ share) {
+  const int pr = blockIdx.x, lane = threadIdx.x;
+  const long long self = (long long)pr * N / NORM_PROBES;
+  int hit = 0, n = 0;
+  for (int j = lane; j < NORM_PROBE_K + 1; j += 32) {
+    const long long i = idx[(long long)pr * (NORM_PROBE_K + 1) + j];
+    if (i != self && i >= 0 && i < N) { ++n; hit += in_sample[i]; }
+  }
+  hit = __reduce_add_sync(0xffffffffu, hit); n = __reduce_add_sync(0xffffffffu, n);
+  if (lane == 0) share[pr] = n > 0 ? (float)hit / (float)n : 0.f;
+}
+__global__ void norm_phi_init_kernel(NormSelect* s, const SideStats* st) {
+  s->lo = 0.0;
+  s->hi = 40.0 * sqrt((double)__uint_as_float(st->max_norm2_bits)) + 1e-30;   // P <= erfc(28) ~ 1e-343 per row above it
+}
 
 // (0) query preparation, one warp per (padded) query row: per-row exponent, scaled norm -> margins, fp16 tile image.
 //   margin[row] = 2*eps + run-to-run slack  (filter threshold T = L - margin)
@@ -219,6 +418,10 @@ struct ScanParams {
   // SAMPLE: a bin = the maximum over `group` consecutive sampled tiles x 64 columns of one epilogue thread
   float* binmax; int bins_ld;     // [Qp, bins_ld]; bin = (part * bins_per_part + it / group) * 2 + half
   int group, bins_per_part;
+  // SAMPLE on an index whose header says SAMPLE_NORM (simg != null): the norm-sample image at stride 1, same parts
+  const IndexHeader* hdr;
+  const unsigned char* simg;
+  int n_seq_norm, group_norm, bins_per_part_norm;
   // FILTER
   const float* thr;               // [Qp]
   // Retry launch (null on the first filter pass): [Qp] marks of the rows the select kernel sends back at their guaranteed
@@ -233,9 +436,10 @@ struct ScanParams {
   int cap_part;                   // records per segment
 };
 
-template <int KB, int STAGES, int MODE>
-__global__ void __launch_bounds__(THREADS, 1)
-tc_scan_kernel(const ScanParams p) {
+// NORM: the sampled pass over the norm-sample image (a compile-time choice, so the strided tile sequence keeps its
+// parameter reads and the code it had before the norm sample existed)
+template <int KB, int STAGES, int MODE, bool NORM>
+__device__ __forceinline__ void tc_scan_body(const ScanParams& p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   // carve: [A: 2*KB slabs][B: STAGES*KB slabs][barriers]
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -248,8 +452,12 @@ tc_scan_kernel(const ScanParams p) {
 
   const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int qb = blockIdx.x % p.nqb, part = blockIdx.x / p.nqb;
-  const int u_begin = (int)((long long)part * p.n_seq / p.parts);
-  const int u_end = (int)((long long)(part + 1) * p.n_seq / p.parts);
+  // the tile sequence: the norm-sample image at stride 1, else every stride-th tile of the corpus image
+  const unsigned char* const cimg = NORM ? p.simg : p.cimg;
+  const int n_seq = NORM ? p.n_seq_norm : p.n_seq, stride = NORM ? 1 : p.stride;
+  const int group = NORM ? p.group_norm : p.group, bins_per_part = NORM ? p.bins_per_part_norm : p.bins_per_part;
+  const int u_begin = (int)((long long)part * n_seq / p.parts);
+  const int u_end = (int)((long long)(part + 1) * n_seq / p.parts);
   const int n_iter = u_end - u_begin;
   const bool issuer = threadIdx.x == 0;   // also drives the bulk-TMA ring
   // rows this launch (re)writes: every row on the first filter pass, the marked ones on a retry
@@ -267,13 +475,13 @@ tc_scan_kernel(const ScanParams p) {
 
   // tile `it` of this part -> ring slot `stage` (issuer only)
   auto load_tile = [&](int it, int stage) {
-    const long long tile = (long long)(u_begin + it) * p.stride;
+    const long long tile = (long long)(u_begin + it) * stride;
     mbar_expect_tx(&full[stage], KB * SLAB_BYTES);
     if (MODE == MODE_FILTER)   // streamed once per pass: evict-first, so the survivor records stay in L2 for the select kernel
-      bulk_g2s_hint(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage],
+      bulk_g2s_hint(sB + stage * KB * SLAB_BYTES, cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage],
                     l2_policy_evict_first());
     else
-      bulk_g2s(sB + stage * KB * SLAB_BYTES, p.cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage]);
+      bulk_g2s(sB + stage * KB * SLAB_BYTES, cimg + tile * ((long long)KB * SLAB_BYTES), KB * SLAB_BYTES, &full[stage]);
   };
   if (issuer) {
     mbar_expect_tx(a_full, 2 * KB * SLAB_BYTES);
@@ -340,13 +548,13 @@ tc_scan_kernel(const ScanParams p) {
       for (int j = 0; j < 8; ++j)
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) binm[2 * rr + H] = max3(binm[2 * rr + H], acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
-      if (H == 1 && (++in_group == p.group || it == n_iter - 1)) {   // close the bin after `group` tiles (loop-uniform)
+      if (H == 1 && (++in_group == group || it == n_iter - 1)) {   // close the bin after `group` tiles (loop-uniform)
 #pragma unroll
         for (int s = 0; s < 4; ++s) {
           const float m = quad_max(binm[s]);
           const long long row = row_a + 8 * (s >> 1);
           if (quad_leader && row < p.Q)
-            p.binmax[row * p.bins_ld + (long long)part * p.bins_per_part * 2 + (s & 1) + 2 * bin_out] = m;
+            p.binmax[row * p.bins_ld + (long long)part * bins_per_part * 2 + (s & 1) + 2 * bin_out] = m;
           binm[s] = -INFINITY;
         }
         ++bin_out; in_group = 0;
@@ -420,7 +628,7 @@ tc_scan_kernel(const ScanParams p) {
   // serializes the wgmma when an accumulator is in flight at a loop head or only on some paths.
   auto tile_step = [&](int it, auto last_tile) {
     constexpr bool LAST = decltype(last_tile)::value;
-    const long long col0 = (long long)(u_begin + it) * p.stride * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
+    const long long col0 = (long long)(u_begin + it) * stride * TILE_N;  // zero-padded rows of the last tile score 0: dropped in finalize (idx >= N)
     issue(acc1, stage, 1);
     epilogue(acc0, col0, it, std::integral_constant<int, 0>{});
     const int next_stage = stage + 1 == STAGES ? 0 : stage + 1;
@@ -462,8 +670,8 @@ tc_scan_kernel(const ScanParams p) {
     for (int s = 0; s < 4; ++s) {   // bins this part did not fill
       const long long row = row_a + 8 * (s >> 1);
       if (quad_leader && row < p.Q)
-        for (int b = bin_out; b < p.bins_per_part; ++b)
-          p.binmax[row * p.bins_ld + (long long)part * p.bins_per_part * 2 + (s & 1) + 2 * b] = -INFINITY;
+        for (int b = bin_out; b < bins_per_part; ++b)
+          p.binmax[row * p.bins_ld + (long long)part * bins_per_part * 2 + (s & 1) + 2 * b] = -INFINITY;
     }
   } else if (quad_leader) {
 #pragma unroll
@@ -472,6 +680,15 @@ tc_scan_kernel(const ScanParams p) {
         p.count[((row_a + 8 * (s >> 1)) * p.parts + part) * 2 + (s & 1)] =
             FILTER_ABLATION != FILTER_FULL ? sink : ((ovf >> s) & 1u) ? (cap + 1u) : cnt[s];
   }
+}
+
+template <int KB, int STAGES, int MODE>
+__global__ void __launch_bounds__(THREADS, 1)
+tc_scan_kernel(const __grid_constant__ ScanParams p) {
+  if constexpr (MODE == MODE_SAMPLE) {
+    if (p.simg != nullptr && p.hdr->sample == SAMPLE_NORM) { tc_scan_body<KB, STAGES, MODE, true>(p); return; }
+  }
+  tc_scan_body<KB, STAGES, MODE, false>(p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -534,13 +751,9 @@ __device__ __forceinline__ unsigned int warp_kth_largest_smem(const unsigned int
 // threshold thr = L_K' - margin at the smaller bin rank k_filter (Plan::k_filter; == k where the threshold must stay a
 // guarantee).  One warp per query, the query's <= 32*KPL bin maxima live in registers.
 template <int KPL>
-__global__ void __launch_bounds__(256)
-tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, int k, int k_filter, const float* __restrict__ margin,
-                    float* __restrict__ thr, float* __restrict__ thr_safe, unsigned int* __restrict__ overflow,
-                    unsigned int* __restrict__ retry, long long Q) {
-  const int lane = threadIdx.x & 31;
-  const long long row = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5;
-  if (row >= Q) return;
+__device__ __forceinline__ void thresholds_of_row(const float* __restrict__ binmax, int bins_ld, int n_bins, int k, int k_filter,
+                                                  const float* __restrict__ margin, float* __restrict__ thr, float* __restrict__ thr_safe,
+                                                  unsigned int* __restrict__ overflow, unsigned int* __restrict__ retry, long long row, int lane) {
   const float* src = binmax + row * bins_ld;
   unsigned int key[KPL];
 #pragma unroll
@@ -548,6 +761,20 @@ tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, i
   const float safe = key2f(warp_kth_largest_regs<KPL>(key, k)) - margin[row];
   const float filter = k_filter < k ? key2f(warp_kth_largest_regs<KPL>(key, k_filter)) - margin[row] : safe;
   if (lane == 0) { thr[row] = filter; thr_safe[row] = safe; overflow[row] = 0; retry[row] = 0; }
+}
+// On a norm-sample index
+// (n_bins_norm > 0 and the header says so) the pass filled n_bins_norm bins and both thresholds sit at rank k.
+template <int KPL>
+__global__ void __launch_bounds__(256)
+tc_threshold_kernel(const float* __restrict__ binmax, int bins_ld, int n_bins, int k, int k_filter, const float* __restrict__ margin,
+                    float* __restrict__ thr, float* __restrict__ thr_safe, unsigned int* __restrict__ overflow,
+                    unsigned int* __restrict__ retry, long long Q, const IndexHeader* __restrict__ hdr, int n_bins_norm) {
+  const int lane = threadIdx.x & 31;
+  const long long row = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5;
+  if (row >= Q) return;
+  if (n_bins_norm > 0 && hdr->sample == SAMPLE_NORM) { n_bins = n_bins_norm; k_filter = k; }
+  if (KPL > 16 && n_bins <= 512) thresholds_of_row<16>(binmax, bins_ld, n_bins, k, k_filter, margin, thr, thr_safe, overflow, retry, row, lane);
+  else thresholds_of_row<KPL>(binmax, bins_ld, n_bins, k, k_filter, margin, thr, thr_safe, overflow, retry, row, lane);
 }
 
 // (3) finalize: one WARP per query, no block-wide barriers.
@@ -1044,6 +1271,8 @@ struct Plan {
   int kb, stages; long long n_tiles; int nqb; long long Qp;
   int stride, n_sample, group, bins_per_part, n_bins, bins_ld, parts_sample, parts_full, cap_part, cap_keys, cap_band;
   int k_filter;   // bin rank of the filter threshold of TOPK / EXCLUDE calls (filter_bin_rank)
+  // the sampled pass on a norm-sample index: its tiles, and bins of `group_norm` tiles (0: the shape has no such index)
+  int n_seq_norm, group_norm, bins_per_part_norm, n_bins_norm;
   size_t smem;
   // workspace offsets
   size_t o_qimg, o_margin, o_cut, o_thr, o_qexp, o_count, o_ovf, o_binmax, o_cand, o_tmp, o_band, o_bandn, o_thr_safe, o_retry,
@@ -1100,7 +1329,20 @@ static bool make_plan(long long Q, long long N, int d, int k, Plan& pl) {
     pl.bins_per_part = (int)ceil_div(iters_max, g);
     pl.n_bins = pl.parts_sample * pl.bins_per_part * 2;
     if (pl.n_bins > MAX_BINS || pl.n_bins < 2 * k) return false;
-    pl.bins_ld = (pl.n_bins + 31) / 32 * 32;
+    // The norm sample runs on the same CTAs with groups of fewer tiles, up to MAX_BINS bins: its threshold is a
+    // guarantee at rank k, and finer bins keep it tight.
+    pl.n_seq_norm = (int)norm_sample_tiles(N);
+    pl.group_norm = pl.bins_per_part_norm = pl.n_bins_norm = 0;
+    if (pl.n_seq_norm >= pl.parts_sample) {
+      const int iters_norm = (int)ceil_div(pl.n_seq_norm, pl.parts_sample);
+      int gn = 1;
+      while ((long long)pl.parts_sample * ceil_div(iters_norm, gn) * 2 > MAX_BINS) ++gn;
+      const int bpp = (int)ceil_div(iters_norm, gn);
+      if (pl.parts_sample * bpp * 2 >= 4 * k) { pl.group_norm = gn; pl.bins_per_part_norm = bpp; pl.n_bins_norm = pl.parts_sample * bpp * 2; }
+    }
+    if (pl.n_bins_norm == 0) pl.n_seq_norm = 0;
+    const int bins_max = pl.n_bins > pl.n_bins_norm ? pl.n_bins : pl.n_bins_norm;
+    pl.bins_ld = (bins_max + 31) / 32 * 32;
   }
   {
     // octet records per (part, column-half) segment: expected lambda = k * stride / segments (the threshold sits near rank
@@ -1232,17 +1474,20 @@ static int run_call(const Call& c) {
   ScanParams sp{};
   sp.qimg = qimg; sp.cimg = cimg; sp.Q = c.Q; sp.N = c.N; sp.nqb = pl.nqb; sp.n_tiles = pl.n_tiles;
   sp.binmax = binmax; sp.bins_ld = pl.bins_ld; sp.group = pl.group; sp.bins_per_part = pl.bins_per_part;
+  sp.hdr = hdr;
+  sp.simg = pl.n_bins_norm > 0 ? cimg + pl.n_tiles * pl.kb * (long long)SLAB_BYTES : nullptr;
+  sp.n_seq_norm = pl.n_seq_norm; sp.group_norm = pl.group_norm; sp.bins_per_part_norm = pl.bins_per_part_norm;
   sp.thr = thr; sp.count = count; sp.cand_s = cand_s; sp.cand_i = cand_i; sp.cap_part = pl.cap_part;
   prof_mark(st, 1);
   // (1) sampled pass -> bin maxima -> k-th largest -> threshold
   int rc = launch_scan_mode(pl, sp, st, MODE_SAMPLE);
   if (rc) return rc;
-  if (pl.n_bins <= 512)
+  if (pl.n_bins <= 512 && pl.n_bins_norm <= 512)
     tc_threshold_kernel<16><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, k_filter, margin,
-                                                                                 thr, thr_safe, ovf, retry, c.Q);
+                                                                                 thr, thr_safe, ovf, retry, c.Q, hdr, pl.n_bins_norm);
   else
     tc_threshold_kernel<32><<<(unsigned)ceil_div(c.Q * 32, 256), 256, 0, st>>>(binmax, pl.bins_ld, pl.n_bins, c.k, k_filter, margin,
-                                                                                 thr, thr_safe, ovf, retry, c.Q);
+                                                                                 thr, thr_safe, ovf, retry, c.Q, hdr, pl.n_bins_norm);
   TFRS_LAUNCH_CHECK();
   if (c.hook) {
     rc = c.hook(c.hook_ctx, thr, margin, cut, qexp, &hdr->st.exp, c.Q, st);
@@ -1298,7 +1543,8 @@ using namespace tfrs::tc;
 extern "C" size_t tfrs_index_bytes(int64_t N, int d) {
   if (N <= 0 || d <= 0 || d > 128) return 0;
   int kb = (d + KSLAB - 1) / KSLAB;
-  return (size_t)HEADER_BYTES + (size_t)ceil_div(N, TILE_N) * kb * SLAB_BYTES;
+  // [header][corpus image][norm-sample image, from 2^19 rows: N/8 rows more]
+  return (size_t)HEADER_BYTES + (size_t)(ceil_div(N, TILE_N) + norm_sample_tiles(N)) * kb * SLAB_BYTES;
 }
 
 extern "C" int tfrs_index_build(const float* corpus, int64_t N, int d, void* index_buf, size_t index_bytes, void* stream) {
@@ -1318,13 +1564,96 @@ extern "C" int tfrs_index_build(const float* corpus, int64_t N, int d, void* ind
   TFRS_LAUNCH_CHECK();
   side_exp_kernel<<<1, 1, 0, st>>>(cst);
   TFRS_LAUNCH_CHECK();
-  corpus_stats_kernel<1><<<sgrid, 256, 0, st>>>(corpus, N, d, cst);
+  const long long s_tiles = norm_sample_tiles(N);
+  if (s_tiles == 0) {
+    corpus_stats_kernel<1><<<sgrid, 256, 0, st>>>(corpus, N, d, cst);
+    TFRS_LAUNCH_CHECK();
+  }
+  auto image = [&](long long rows, long long tiles, unsigned char* dst, const int* rowmap) {
+    const long long chunks = tiles * TILE_N * (long long)h.kb * 8;
+    const unsigned blocks = (unsigned)(ceil_div(chunks, 256) < (1 << 20) ? ceil_div(chunks, 256) : (1 << 20));
+    tile_image_kernel<<<blocks, 256, 0, st>>>(corpus, rows, d, h.kb, tiles, cst, dst, rowmap);
+  };
+  unsigned char* img = (unsigned char*)index_buf + HEADER_BYTES;
+  image(N, h.n_tiles, img, nullptr);
   TFRS_LAUNCH_CHECK();
-  long long chunks = h.n_tiles * TILE_N * (long long)h.kb * 8;
-  unsigned blocks = (unsigned)(ceil_div(chunks, 256) < (1 << 20) ? ceil_div(chunks, 256) : (1 << 20));
-  tile_image_kernel<<<blocks, 256, 0, st>>>(corpus, N, d, h.kb, h.n_tiles, cst, (unsigned char*)index_buf + HEADER_BYTES);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
+  if (s_tiles == 0) return TFRS_OK;
+
+  // norm sample: the S rows of largest norm (ties to the lower index), their image, and phi -> header
+  const long long S = s_tiles * TILE_N;
+  const int nblk = (int)ceil_div(N, NS_CHUNK), nblk_s = (int)ceil_div(S, NS_CHUNK);
+  const size_t o_rows = align_up((size_t)N * 4, 256), o_blk = o_rows + align_up((size_t)S * 4, 256);
+  const size_t o_part = o_blk + align_up((size_t)nblk * 8, 256), o_sel = o_part + align_up((size_t)nblk * 8, 256);
+  // probes: their rows, the exact top-(K+1) lists, the shares, the sample flags and the call's workspace
+  Plan ppl;
+  const bool probe_ok = make_plan(NORM_PROBES, N, d, NORM_PROBE_K + 1, ppl);
+  const size_t pk = (size_t)NORM_PROBES * (NORM_PROBE_K + 1);
+  const size_t o_probe = o_sel + align_up(sizeof(NormSelect), 256), o_ps = o_probe + align_up((size_t)NORM_PROBES * d * 4, 256);
+  const size_t o_pi = o_ps + align_up(pk * 4, 256), o_share = o_pi + align_up(pk * 8, 256);
+  const size_t o_flag = o_share + align_up((size_t)NORM_PROBES * 4, 256), o_pws = o_flag + align_up((size_t)N, 256);
+  const size_t ws_bytes = probe_ok ? ppl.total + 16 : 0;
+  unsigned char* scratch = nullptr;
+  TFRS_CUDA(cudaMallocAsync((void**)&scratch, o_pws + ws_bytes, st));
+  unsigned int* key = (unsigned int*)scratch;
+  int* rowlist = (int*)(scratch + o_rows);
+  int* blk = (int*)(scratch + o_blk);
+  double* partial = (double*)(scratch + o_part);
+  NormSelect* sel = (NormSelect*)(scratch + o_sel);
+  int rc = TFRS_OK;
+  // errors are recorded, not returned, so that the scratch memory is always freed
+  auto launched = [&]() {
+    count_launch();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess && rc == TFRS_OK) { set_error("index_build: %s", cudaGetErrorString(e)); rc = TFRS_ERR_CUDA; }
+  };
+  if (cudaMemsetAsync(sel, 0, sizeof(NormSelect), st) != cudaSuccess) { set_error("index_build: memset failed"); rc = TFRS_ERR_CUDA; }
+  corpus_stats_kernel<1><<<sgrid, 256, 0, st>>>(corpus, N, d, cst, key);
+  launched();
+  for (int bit = 31; bit >= 0; --bit) { norm_select_count_kernel<<<sgrid, 256, 0, st>>>(key, N, S, bit, sel); launched(); }
+  norm_select_chunks_kernel<<<nblk, 256, 0, st>>>(key, N, S, sel, blk);
+  launched();
+  norm_select_offsets_kernel<<<1, 1, 0, st>>>(blk, nblk, S, sel);
+  launched();
+  norm_select_write_kernel<<<nblk, 256, 0, st>>>(key, N, S, sel, blk, rowlist);
+  launched();
+  image(S, s_tiles, img + h.n_tiles * h.kb * (long long)SLAB_BYTES, rowlist);
+  launched();
+  norm_phi_init_kernel<<<1, 1, 0, st>>>(sel, cst);
+  launched();
+  IndexHeader* hdr = reinterpret_cast<IndexHeader*>(index_buf);
+  for (int it = 0; it < 48; ++it) {   // bracket [0, 40 max|c|] / 2^48
+    norm_phi_partial_kernel<<<nblk, 256, 0, st>>>(key, nullptr, N, sel, partial);
+    launched();
+    norm_phi_step_kernel<<<1, 1, 0, st>>>(partial, nblk, N, 0, sel, hdr, nullptr);
+    launched();
+  }
+  float* share = (float*)(scratch + o_share);
+  if (cudaMemsetAsync(share, 0, (size_t)NORM_PROBES * 4, st) != cudaSuccess && rc == TFRS_OK) { set_error("index_build: memset failed"); rc = TFRS_ERR_CUDA; }
+  if (probe_ok && rc == TFRS_OK) {
+    unsigned char* flags = scratch + o_flag;
+    if (cudaMemsetAsync(flags, 0, (size_t)N, st) != cudaSuccess) { set_error("index_build: memset failed"); rc = TFRS_ERR_CUDA; }
+    norm_sample_flags_kernel<<<sgrid, 256, 0, st>>>(rowlist, S, flags);
+    launched();
+    float* probes = (float*)(scratch + o_probe);
+    norm_probe_gather_kernel<<<NORM_PROBES, 32, 0, st>>>(corpus, N, d, probes);
+    launched();
+    // the header still says SAMPLE_STRIDED: an exact call on the strided-sample path
+    Call c{};
+    c.mode = FIN_TOPK; c.q = probes; c.Q = NORM_PROBES; c.corpus = corpus; c.index_buf = index_buf; c.N = N; c.d = d;
+    c.k = NORM_PROBE_K + 1; c.ws = scratch + o_pws; c.ws_bytes = ws_bytes; c.st = st;
+    c.out_s = (float*)(scratch + o_ps); c.out_i = (long long*)(scratch + o_pi);
+    const int prc = run_call(c);
+    if (prc != TFRS_OK && rc == TFRS_OK) rc = prc;
+    norm_probe_share_kernel<<<NORM_PROBES, 32, 0, st>>>(c.out_i, N, flags, share);
+    launched();
+  }
+  norm_phi_partial_kernel<<<nblk_s, 256, 0, st>>>(key, rowlist, S, sel, partial);
+  launched();
+  norm_phi_step_kernel<<<1, 1, 0, st>>>(partial, nblk_s, N, 1, sel, hdr, share);
+  launched();
+  const cudaError_t fe = cudaFreeAsync(scratch, st);
+  if (fe != cudaSuccess && rc == TFRS_OK) { set_error("index_build: %s", cudaGetErrorString(fe)); rc = TFRS_ERR_CUDA; }
+  return rc;
 }
 
 extern "C" size_t tfrs_topk_tc_workspace_bytes(int64_t Q, int64_t N, int d, int k) {
@@ -1401,6 +1730,16 @@ extern "C" int tfrs_topk_tc_retry_layout(int64_t Q, int64_t N, int d, int k, int
   Plan pl;
   if (!make_plan(Q, N, d, k, pl)) { set_error("topk_tc_retry_layout: unsupported shape"); return TFRS_ERR_UNSUPPORTED; }
   out4[0] = (int64_t)pl.o_thr_safe; out4[1] = (int64_t)pl.o_retry; out4[2] = pl.k_filter; out4[3] = pl.stride;
+  return TFRS_OK;
+}
+
+// The sampled pass on a norm-sample index: where the bin maxima and margins live, and how the bins are laid out.
+extern "C" int tfrs_topk_tc_sample_layout(int64_t Q, int64_t N, int d, int k, int64_t* out8) {
+  TFRS_CHECK_ARG(out8, "topk_tc_sample_layout: NULL pointer");
+  Plan pl;
+  if (!make_plan(Q, N, d, k, pl)) { set_error("topk_tc_sample_layout: unsupported shape"); return TFRS_ERR_UNSUPPORTED; }
+  out8[0] = (int64_t)pl.o_binmax; out8[1] = pl.bins_ld; out8[2] = pl.n_bins_norm; out8[3] = pl.group_norm;
+  out8[4] = pl.bins_per_part_norm; out8[5] = pl.parts_sample; out8[6] = pl.n_seq_norm; out8[7] = (int64_t)pl.o_margin;
   return TFRS_OK;
 }
 
