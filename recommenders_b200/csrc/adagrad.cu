@@ -169,11 +169,8 @@ ag_apply(const unsigned long long* __restrict__ keys, long long n, const float* 
          unsigned int* __restrict__ long_count, unsigned int* __restrict__ long_list) {
   const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per sorted slot
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
-  const unsigned long long key = keys[i];
-  const unsigned long long id = key >> 24;
-  if (id == AG_BAD_ID) return;
-  if (i > 0 && (keys[i - 1] >> 24) == id) return;  // not the head of its run
+  unsigned long long id;
+  if (i >= n || !ag_run_head(keys, i, id)) return;
   // run length: ballots over 32-slot windows
   long long end = i + 1;
   for (;;) {
@@ -282,6 +279,16 @@ ag_apply_long(const unsigned long long* __restrict__ keys, long long n, const fl
 
 static long long ag_pow2(long long n) { long long p = 1; while (p < n) p <<= 1; return p; }
 
+int ag_check_args(const char* who, bool state, long long rows, int d, int ids_dtype, long long n, const void* ids,
+                  const void* grad) {
+  TFRS_CHECK_ARG(state && rows > 0 && d > 0, "%s: bad table", who);
+  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "%s: ids_dtype must be I32 or I64", who);
+  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "%s: n=%lld must be < 2^24", who, n);
+  TFRS_CHECK_ARG(rows < (1ll << 40), "%s: rows must be < 2^40", who);
+  TFRS_CHECK_ARG(n == 0 || (ids && grad), "%s: NULL ids/grad", who);
+  return TFRS_OK;
+}
+
 size_t ag_group_workspace_bytes(long long n) {
   const size_t P = (size_t)ag_pow2(n > 2 ? n : 2);
   return P * 8 /*keys*/ + P * 8 /*bucketed keys*/ + P * 4 /*ranks*/ + (P / AG_LONG + 2) * 4 /*long-run list*/ + (AB_BUCKETS + 1) * 4 + 1024;
@@ -343,18 +350,14 @@ extern "C" size_t tfrs_sparse_adagrad_workspace_bytes(int64_t n, int d) {
 extern "C" int tfrs_sparse_adagrad_f32(float* table, float* accum, int64_t rows, int d, const void* ids,
                                        int ids_dtype, int64_t n, const float* grad_rows, float lr, float eps,
                                        int eps_inside_sqrt, void* ws, size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && accum && rows > 0 && d > 0, "sparse_adagrad: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_adagrad: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_adagrad: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_adagrad: rows must be < 2^40");
+  int rc;
+  if ((rc = ag_check_args("sparse_adagrad", table && accum, rows, d, ids_dtype, n, ids, grad_rows)) != TFRS_OK) return rc;
   if (n == 0) return TFRS_OK;
-  TFRS_CHECK_ARG(ids && grad_rows, "sparse_adagrad: NULL ids/grad");
   TFRS_CHECK_ARG(d <= 1024, "sparse_adagrad: d=%d > 1024", d);
   if (!ws || ws_bytes < tfrs_sparse_adagrad_workspace_bytes(n, d)) { set_error("sparse_adagrad: workspace too small"); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
   cudaStream_t st = (cudaStream_t)stream;
   AgGroups gr;
-  const int rc = ag_group(ids, ids_dtype, n, rows, ws, st, &gr);
-  if (rc != TFRS_OK) return rc;
+  if ((rc = ag_group(ids, ids_dtype, n, rows, ws, st, &gr)) != TFRS_OK) return rc;
   TFRS_CUDA(cudaMemsetAsync(gr.long_count, 0, 4, st));
   ag_apply<<<(unsigned)ceil_div(n * 32, 256), 256, 0, st>>>(gr.keys, n, grad_rows, d, table, accum, lr, eps, eps_inside_sqrt,
                                                             gr.long_count, gr.long_list);

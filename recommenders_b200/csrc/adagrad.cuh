@@ -1,7 +1,8 @@
-// adagrad.cuh -- K4's id grouping, shared by the sparse Adagrad (adagrad.cu) and the sparse ClippyAdagrad
-// (clippy_adagrad.cu) entry points, and K4's run-summing pattern with a pluggable epilogue (ClippyAdagrad's pass A).
-// K4 itself keeps its fused kernels ag_apply / ag_apply_long in adagrad.cu: the same code as a template on the epilogue
-// measured 8 % slower on uniform cfg3 batches (about 3.5 us of ~44 us on one H100).
+// adagrad.cuh -- K4's id grouping and argument checks, shared by every sparse optimizer step (SGD, Adagrad,
+// ClippyAdagrad, Adam, FTRL), and K4's run-summing pattern with a pluggable epilogue (ClippyAdagrad's pass A, Adam, FTRL).
+// K4 itself keeps its fused kernels ag_apply / ag_apply_long in adagrad.cu: instantiated from these templates, its warp
+// kernel measured 0.7 us (7 %) slower on uniform cfg3 batches, about 2 % of the step (H100, BASELINE.md).
+//   ag_check_args: the argument checks of the five sparse entry points (adagrad.cu)
 //   ag_group:      keys = (id << 24 | position), grouped by id with positions ascending (adagrad.cu)
 //   ag_run_sums:   one warp per run of equal ids (one CTA per run longer than AG_LONG) sums the run's gradient rows in
 //                  order of occurrence and hands every column's sum to an epilogue op:
@@ -20,12 +21,22 @@ struct AgGroups {
   unsigned int* long_count;     // runs longer than AG_LONG, queued for the CTA-per-run kernel
   unsigned int* long_list;
 };
+// The checks every sparse step makes before its first launch; each message starts with `who`.  `state` is false when the
+// table or one of its slots is NULL.  n < 2^24 and rows < 2^40: the key holds a 24-bit position and a 40-bit id.
+int ag_check_args(const char* who, bool state, long long rows, int d, int ids_dtype, long long n, const void* ids,
+                  const void* grad);
 size_t ag_group_workspace_bytes(long long n);
 // ws must hold ag_group_workspace_bytes(n) bytes; n >= 1, ids_dtype TFRS_I32 / TFRS_I64
 int ag_group(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st, AgGroups* out);
 // The bitonic branch of ag_group on its own: the first n keys at ws come out in ascending (id, position) order, i.e. the
 // groups in ascending id order as well (tree_ah.cu's leaf-major layout needs that global order).
 int ag_sort(const void* ids, int ids_dtype, long long n, long long rows, void* ws, cudaStream_t st);
+
+// Whether sorted slot i (< n) is the first slot of a run of an in-range id; the id comes back in `id`.
+__device__ __forceinline__ bool ag_run_head(const unsigned long long* __restrict__ keys, long long i, unsigned long long& id) {
+  id = keys[i] >> 24;
+  return id != AG_BAD_ID && (i == 0 || (keys[i - 1] >> 24) != id);
+}
 
 // One warp per run of equal ids (the warp of the run's first slot; the others exit).  Duplicates are summed in order of
 // occurrence -- the keys are sorted by (id, position) -- with the gradient rows of 8 members in flight per step, so a hot
@@ -39,11 +50,8 @@ ag_sum_runs(const unsigned long long* __restrict__ keys, long long n, const floa
          unsigned int* __restrict__ long_count, unsigned int* __restrict__ long_list) {
   const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per sorted slot
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
-  const unsigned long long key = keys[i];
-  const unsigned long long id = key >> 24;
-  if (id == AG_BAD_ID) return;
-  if (i > 0 && (keys[i - 1] >> 24) == id) return;  // not the head of its run
+  unsigned long long id;
+  if (i >= n || !ag_run_head(keys, i, id)) return;
   // run length: ballots over 32-slot windows
   long long end = i + 1;
   for (;;) {

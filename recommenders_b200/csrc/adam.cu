@@ -123,12 +123,9 @@ extern "C" size_t tfrs_sparse_adam_workspace_bytes(int64_t n, int64_t rows) {
 extern "C" int tfrs_sparse_adam_f32(float* table, float* m, float* v, int64_t rows, int d, const void* ids, int ids_dtype,
                                     int64_t n, const float* grad_rows, float alpha, float beta1, float beta2, float eps,
                                     int lazy, void* ws, size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && m && v && rows > 0 && d > 0, "sparse_adam: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_adam: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_adam: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_adam: rows must be < 2^40");
+  int rc;
+  if ((rc = ag_check_args("sparse_adam", table && m && v, rows, d, ids_dtype, n, ids, grad_rows)) != TFRS_OK) return rc;
   TFRS_CHECK_ARG(d <= 1024, "sparse_adam: d=%d > 1024", d);
-  TFRS_CHECK_ARG(n == 0 || (ids && grad_rows), "sparse_adam: NULL ids/grad");
   if (!ws || ws_bytes < tfrs_sparse_adam_workspace_bytes(n, rows)) {
     set_error("sparse_adam: workspace too small");
     return TFRS_ERR_WORKSPACE_TOO_SMALL;
@@ -137,7 +134,6 @@ extern "C" int tfrs_sparse_adam_f32(float* table, float* m, float* v, int64_t ro
   const AdamArgs k = ad_args(alpha, beta1, beta2, eps);
   unsigned int* touched = lazy ? nullptr : (unsigned int*)((char*)ws + align_up(ag_group_workspace_bytes(n), 256));
   if (touched) TFRS_CUDA(cudaMemsetAsync(touched, 0, ad_bitmap_bytes(rows), st));
-  int rc;
   if (n > 0) {
     AgGroups gr;
     if ((rc = ag_group(ids, ids_dtype, n, rows, ws, st, &gr)) != TFRS_OK) return rc;

@@ -79,10 +79,8 @@ cl_sparse_apply(const unsigned long long* __restrict__ keys, long long n, const 
                 float* __restrict__ table, float* __restrict__ accum, const float* __restrict__ factor, const ClippyArgs k) {
   const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
-  const unsigned long long id = keys[i] >> 24;
-  if (id == AG_BAD_ID) return;
-  if (i > 0 && (keys[i - 1] >> 24) == id) return;
+  unsigned long long id;
+  if (i >= n || !ag_run_head(keys, i, id)) return;
   const float scale = *factor;
   float* trow = table + (long long)id * d;
   float* arow = accum + (long long)id * d;
@@ -155,14 +153,11 @@ extern "C" int tfrs_sparse_clippy_adagrad_f32(float* table, float* accum, int64_
                                               int64_t n, const float* grad_rows, float lr, float eps, float var_rel,
                                               float acc_rel, float abs_thr, int flags, float* clipping_factor_out, void* ws,
                                               size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && accum && rows > 0 && d > 0, "sparse_clippy_adagrad: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_clippy_adagrad: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_clippy_adagrad: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_clippy_adagrad: rows must be < 2^40");
+  int rc;
+  if ((rc = ag_check_args("sparse_clippy_adagrad", table && accum, rows, d, ids_dtype, n, ids, grad_rows)) != TFRS_OK) return rc;
   TFRS_CHECK_ARG(d <= 1024, "sparse_clippy_adagrad: d=%d > 1024", d);
-  TFRS_CHECK_ARG(n == 0 || (ids && grad_rows), "sparse_clippy_adagrad: NULL ids/grad");
   ClippyArgs k;
-  int rc = cl_args(lr, eps, var_rel, acc_rel, abs_thr, flags, &k);
+  rc = cl_args(lr, eps, var_rel, acc_rel, abs_thr, flags, &k);
   if (rc != TFRS_OK) return rc;
   if (!ws || ws_bytes < tfrs_sparse_clippy_adagrad_workspace_bytes(n, d)) {
     set_error("sparse_clippy_adagrad: workspace too small");

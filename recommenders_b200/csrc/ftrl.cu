@@ -107,14 +107,10 @@ extern "C" size_t tfrs_sparse_ftrl_workspace_bytes(int64_t n) { return ag_group_
 extern "C" int tfrs_sparse_ftrl_f32(float* table, float* accum, float* linear, int64_t rows, int d, const void* ids,
                                     int ids_dtype, int64_t n, const float* grad_rows, float lr, float lr_power, float l1,
                                     float l2a, float l2_shrinkage, void* ws, size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && accum && linear && rows > 0 && d > 0, "sparse_ftrl: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_ftrl: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_ftrl: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_ftrl: rows must be < 2^40");
-  TFRS_CHECK_ARG(d <= 1024, "sparse_ftrl: d=%d > 1024", d);
-  TFRS_CHECK_ARG(n == 0 || (ids && grad_rows), "sparse_ftrl: NULL ids/grad");
-  FtrlArgs k;
   int mode, rc;
+  if ((rc = ag_check_args("sparse_ftrl", table && accum && linear, rows, d, ids_dtype, n, ids, grad_rows)) != TFRS_OK) return rc;
+  TFRS_CHECK_ARG(d <= 1024, "sparse_ftrl: d=%d > 1024", d);
+  FtrlArgs k;
   if ((rc = ft_args("sparse_ftrl", lr, lr_power, l1, l2a, l2_shrinkage, &k, &mode)) != TFRS_OK) return rc;
   if (n == 0) return TFRS_OK;
   if (!ws || ws_bytes < tfrs_sparse_ftrl_workspace_bytes(n)) {

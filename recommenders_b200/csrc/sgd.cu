@@ -18,10 +18,8 @@ sgd_sparse_runs(const unsigned long long* __restrict__ keys, long long n, const 
                 float* __restrict__ table, float lr) {
   const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per sorted slot
   const int lane = threadIdx.x & 31;
-  if (i >= n) return;
-  const unsigned long long id = keys[i] >> 24;
-  if (id == AG_BAD_ID) return;
-  if (i > 0 && (keys[i - 1] >> 24) == id) return;  // not the head of its run
+  unsigned long long id;
+  if (i >= n || !ag_run_head(keys, i, id)) return;
   long long end = i + 1;
   while (end < n && (keys[end] >> 24) == id) ++end;
   float* __restrict__ row = table + (long long)id * d;
@@ -65,11 +63,8 @@ extern "C" size_t tfrs_sparse_sgd_workspace_bytes(int64_t n) { return ag_group_w
 
 extern "C" int tfrs_sparse_sgd_f32(float* table, int64_t rows, int d, const void* ids, int ids_dtype, int64_t n,
                                    const float* grad_rows, float lr, void* ws, size_t ws_bytes, void* stream) {
-  TFRS_CHECK_ARG(table && rows > 0 && d > 0, "sparse_sgd: bad table");
-  TFRS_CHECK_ARG(ids_dtype == TFRS_I32 || ids_dtype == TFRS_I64, "sparse_sgd: ids_dtype must be I32 or I64");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 24), "sparse_sgd: n=%lld must be < 2^24", (long long)n);
-  TFRS_CHECK_ARG(rows < (1ll << 40), "sparse_sgd: rows must be < 2^40");
-  TFRS_CHECK_ARG(n == 0 || (ids && grad_rows), "sparse_sgd: NULL ids/grad");
+  int rc;
+  if ((rc = ag_check_args("sparse_sgd", table, rows, d, ids_dtype, n, ids, grad_rows)) != TFRS_OK) return rc;
   if (n == 0) return TFRS_OK;
   if (!ws || ws_bytes < tfrs_sparse_sgd_workspace_bytes(n)) {
     set_error("sparse_sgd: workspace too small");
@@ -77,7 +72,6 @@ extern "C" int tfrs_sparse_sgd_f32(float* table, int64_t rows, int d, const void
   }
   cudaStream_t st = (cudaStream_t)stream;
   AgGroups gr;
-  int rc;
   if ((rc = ag_group(ids, ids_dtype, n, rows, ws, st, &gr)) != TFRS_OK) return rc;
   sgd_sparse_runs<<<(unsigned)ceil_div(n * 32, 256), 256, 0, st>>>(gr.keys, n, grad_rows, d, table, lr);
   TFRS_LAUNCH_CHECK();

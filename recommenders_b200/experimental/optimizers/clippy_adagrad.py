@@ -115,13 +115,10 @@ class ClippyAdagrad(_AccumulatorOptimizer):
     self._order = list(tables) + list(dense)
     rule = self._rule()
     for t in tables:
-      grads = t.pop_sparse_grads()
-      if not grads:
-        continue
-      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)   # one variable: the IndexedSlices of all its lookups
-      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
-      factor = self._factor(t, t.weight.device) if self.export_clipping_factors else None
-      ops.sparse_clippy_adagrad_(t.weight, self._accum(t, t.weight), ids, rows, clipping_factor=factor, **rule)
+      g = self._table_grads(t)
+      if g is not None:
+        factor = self._factor(t, t.weight.device) if self.export_clipping_factors else None
+        ops.sparse_clippy_adagrad_(t.weight, self._accum(t, t.weight), *g, clipping_factor=factor, **rule)
     params = [p for p in dense if p.grad is not None]
     if params:
       factors = self._dense_factor_buffer(params) if self.export_clipping_factors else None

@@ -312,36 +312,78 @@ def embedding_bag_bwd(features: Sequence[BagFeature], grads: Sequence[torch.Tens
 # ------------------------------------------------------------------------------------------------
 # SGD (tf-keras legacy rules, momentum 0)
 # ------------------------------------------------------------------------------------------------
+def _f32_inplace(t: torch.Tensor, name: str) -> torch.Tensor:
+  require_cuda(t, name)
+  if t.dtype != torch.float32 or not t.is_contiguous():
+    raise ValueError(f"{name} must be contiguous float32 (it is updated in place)")
+  return t
+
+
+def _sparse_step_args(what: str, table: torch.Tensor, slots: dict, ids: torch.Tensor, grad_rows: torch.Tensor):
+  """The argument rules of every sparse optimizer step: `table` and its `slots` ({name: tensor}, updated in place) are
+  contiguous float32 of the table's 2-D shape on its device, and `ids` and `grad_rows` [n, d] live there too.  Returns
+  (ids flattened, grad_rows as contiguous float32, n, rows, d)."""
+  _f32_inplace(table, "table")
+  for name, s in slots.items():
+    _f32_inplace(s, name)
+  ids = require_cuda(ids, "ids").contiguous().view(-1)
+  g = f32c(grad_rows, "grad_rows")
+  if table.dim() != 2:
+    raise ValueError(f"{what}: table must be 2-D, got {tuple(table.shape)}")
+  n = ids.numel(); rows, d = table.shape
+  for name, s in slots.items():
+    if s.shape != table.shape or s.device != table.device:
+      raise ValueError(f"{what}: {name} must be {tuple(table.shape)} on {table.device}, got {tuple(s.shape)} on {s.device}")
+  if g.shape != (n, d):
+    raise ValueError(f"{what}: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
+  if ids.device != table.device or g.device != table.device:
+    raise ValueError(f"{what}: ids and grad_rows must live on the table's device")
+  return ids, g, n, rows, d
+
+
+def _dense_step_args(what: str, variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], slots: dict):
+  """The argument rules of every dense multi-tensor step: `variables`, `grads` and each slot list of `slots` ({name:
+  list}) have one entry per variable; variables and slots (updated in place) are contiguous float32; every tensor of a
+  variable has its shape; all live on one device.  Returns (the grads as contiguous float32, which must stay alive until
+  the call is enqueued, and the entry point's leading arguments: the variable, grad and slot pointer arrays, the numels
+  and the count)."""
+  lists = {"variables": variables, "grads": grads, **slots}
+  nv = len(variables)
+  if any(len(l) != nv for l in lists.values()):
+    names = list(lists)
+    raise ValueError(f"{what}: {', '.join(names[:-1])} and {names[-1]} must have the same length")
+  gs = []
+  for i, (x, g, *ss) in enumerate(zip(variables, grads, *slots.values())):
+    _f32_inplace(x, f"variables[{i}]")
+    for name, s in zip(slots, ss):
+      _f32_inplace(s, f"{name}[{i}]")
+    g = f32c(g, f"grads[{i}]")
+    if any(t.device != variables[0].device for t in (x, g, *ss)):
+      raise ValueError(f"{what}: every tensor must live on one device")
+    if g.shape != x.shape or any(s.shape != x.shape for s in ss):
+      raise ValueError(f"{what}: {' / '.join(f'{name}[{i}]' for name in ['grads', *slots])} must have the shape "
+                       f"{tuple(x.shape)}")
+    gs.append(g)
+  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
+  numels = (ctypes.c_int64 * nv)(*[x.numel() for x in variables])
+  return gs, (arr(variables), arr(gs), *[arr(s) for s in slots.values()], numels, nv)
+
+
 def sparse_sgd_(table: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor, lr: float) -> None:
   """table[ids[i]] -= lr * grad_rows[i] for every i, duplicates applied one by one in order of occurrence."""
-  table = require_cuda(table, "table")
-  if table.dtype != torch.float32 or not table.is_contiguous() or table.dim() != 2:
-    raise ValueError("sparse_sgd: table must be contiguous 2-D float32")
-  ids = require_cuda(ids, "ids").reshape(-1).contiguous()
-  n, d = ids.numel(), table.shape[1]
-  grad_rows = f32c(grad_rows, "grad_rows").reshape(n, d)
+  ids, g, n, rows, d = _sparse_step_args("sparse_sgd_", table, {}, ids, grad_rows)
   if n == 0:
     return
   ws = workspace(lib().tfrs_sparse_sgd_workspace_bytes(n), table.device, "sgd")
-  check(lib().tfrs_sparse_sgd_f32(ptr(table), table.shape[0], d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(grad_rows),
-                                  float(lr), ptr(ws), ws.numel(), stream()), "sparse_sgd")
+  check(lib().tfrs_sparse_sgd_f32(ptr(table), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), float(lr), ptr(ws),
+                                  ws.numel(), stream()), "sparse_sgd")
 
 
 def sgd_dense_(params: Sequence[torch.Tensor], grads: Sequence[torch.Tensor], lr: float) -> None:
   """p -= lr * g for every (p, g), in one multi-tensor launch per batch of variables."""
-  n = len(params)
-  if n == 0:
-    return
-  gs = []
-  for p, g in zip(params, grads):
-    require_cuda(p, "param")
-    if p.dtype != torch.float32 or not p.is_contiguous() or g.shape != p.shape:
-      raise ValueError("sgd_dense: parameters must be contiguous float32, gradients of the same shape")
-    gs.append(f32c(g, "grad"))
-  vp = (ctypes.c_void_p * n)(*[p.data_ptr() for p in params])
-  gp = (ctypes.c_void_p * n)(*[g.data_ptr() for g in gs])
-  ne = (ctypes.c_int64 * n)(*[p.numel() for p in params])
-  check(lib().tfrs_sgd_dense_f32(vp, gp, ne, n, float(lr), stream()), "sgd_dense")
+  gs, arrays = _dense_step_args("sgd_dense_", params, grads, {})
+  if gs:
+    check(lib().tfrs_sgd_dense_f32(*arrays, float(lr), stream()), "sgd_dense")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1028,17 +1070,9 @@ def hard_negative_softmax_loss(q: torch.Tensor, c: torch.Tensor, num_hard_negati
 # ------------------------------------------------------------------------------------------------
 def sparse_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor,
                     lr: float, eps: float = 1e-7, eps_inside_sqrt: bool = True) -> None:
-  require_cuda(table, "table"); require_cuda(accum, "accum")
-  if table.dtype != torch.float32 or not table.is_contiguous() or accum.dtype != torch.float32 or not accum.is_contiguous():
-    raise ValueError("sparse_adagrad_: table/accum must be contiguous float32")
-  ids = require_cuda(ids, "ids").contiguous().view(-1)
-  g = f32c(grad_rows, "grad_rows")
-  n = ids.numel(); d = table.shape[1]
-  if g.shape != (n, d):
-    raise ValueError(f"sparse_adagrad_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
-  wsb = lib().tfrs_sparse_adagrad_workspace_bytes(n, d)
-  ws = workspace(wsb, table.device, "adagrad")
-  check(lib().tfrs_sparse_adagrad_f32(ptr(table), ptr(accum), table.shape[0], d, ptr(ids), _ffi.ids_dtype_code(ids), n,
+  ids, g, n, rows, d = _sparse_step_args("sparse_adagrad_", table, {"accum": accum}, ids, grad_rows)
+  ws = workspace(lib().tfrs_sparse_adagrad_workspace_bytes(n, d), table.device, "adagrad")
+  check(lib().tfrs_sparse_adagrad_f32(ptr(table), ptr(accum), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n,
                                       ptr(g), c_f(lr), c_f(eps), int(eps_inside_sqrt), ptr(ws), ws.numel(), stream()),
         "sparse_adagrad")
 
@@ -1050,13 +1084,6 @@ def _clippy_flags(clip_accumulator_update: bool, use_standard_accumulator_update
   return (1 if clip_accumulator_update else 0) | (2 if use_standard_accumulator_update else 0)
 
 
-def _f32_inplace(t: torch.Tensor, name: str) -> torch.Tensor:
-  require_cuda(t, name)
-  if t.dtype != torch.float32 or not t.is_contiguous():
-    raise ValueError(f"{name} must be contiguous float32 (it is updated in place)")
-  return t
-
-
 def sparse_clippy_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.Tensor, grad_rows: torch.Tensor,
                            lr: float, eps: float, variable_relative_threshold: float, accumulator_relative_threshold: float,
                            absolute_threshold: float, clip_accumulator_update: bool = False,
@@ -1064,14 +1091,7 @@ def sparse_clippy_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.
                            clipping_factor: Optional[torch.Tensor] = None) -> None:
   """ClippyAdagrad step of one embedding table on the rows `ids` (duplicates summed in order of occurrence).  The
   variable's clipping factor is written to the 0-d float32 device tensor `clipping_factor` when given."""
-  _f32_inplace(table, "table"); _f32_inplace(accum, "accum")
-  ids = require_cuda(ids, "ids").contiguous().view(-1)
-  g = f32c(grad_rows, "grad_rows")
-  n = ids.numel(); d = table.shape[1]
-  if accum.shape != table.shape:
-    raise ValueError(f"sparse_clippy_adagrad_: accum must be {tuple(table.shape)}, got {tuple(accum.shape)}")
-  if g.shape != (n, d):
-    raise ValueError(f"sparse_clippy_adagrad_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
+  ids, g, n, rows, d = _sparse_step_args("sparse_clippy_adagrad_", table, {"accum": accum}, ids, grad_rows)
   if clipping_factor is not None:
     _f32_inplace(clipping_factor, "clipping_factor")
     if clipping_factor.numel() != 1:
@@ -1079,7 +1099,7 @@ def sparse_clippy_adagrad_(table: torch.Tensor, accum: torch.Tensor, ids: torch.
   wsb = lib().tfrs_sparse_clippy_adagrad_workspace_bytes(n, d)
   ws = workspace(wsb, table.device, "clippy")
   check(lib().tfrs_sparse_clippy_adagrad_f32(
-      ptr(table), ptr(accum), table.shape[0], d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(lr), c_f(eps),
+      ptr(table), ptr(accum), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(lr), c_f(eps),
       c_f(variable_relative_threshold), c_f(accumulator_relative_threshold), c_f(absolute_threshold),
       _clippy_flags(clip_accumulator_update, use_standard_accumulator_update), ptr(clipping_factor), ptr(ws), ws.numel(),
       stream()), "sparse_clippy_adagrad")
@@ -1092,31 +1112,17 @@ def clippy_adagrad_dense_(variables: Sequence[torch.Tensor], grads: Sequence[tor
                           clipping_factors: Optional[torch.Tensor] = None) -> None:
   """ClippyAdagrad step of a list of dense variables in one multi-tensor call (one clipping factor per variable,
   written to the float32 device tensor `clipping_factors` [len(variables)] when given)."""
-  nv = len(variables)
-  if len(grads) != nv or len(accums) != nv:
-    raise ValueError("clippy_adagrad_dense_: variables, grads and accums must have the same length")
-  if nv == 0:
+  gs, arrays = _dense_step_args("clippy_adagrad_dense_", variables, grads, {"accums": accums})
+  if not gs:
     return
-  dev = variables[0].device
-  gs = []
-  for i, (v, g, a) in enumerate(zip(variables, grads, accums)):
-    _f32_inplace(v, f"variables[{i}]"); _f32_inplace(a, f"accums[{i}]")
-    g = f32c(g, f"grads[{i}]")
-    if v.device != dev or g.device != dev or a.device != dev:
-      raise ValueError("clippy_adagrad_dense_: every tensor must live on one device")
-    if g.shape != v.shape or a.shape != v.shape:
-      raise ValueError(f"clippy_adagrad_dense_: grads[{i}] / accums[{i}] must have the shape {tuple(v.shape)}")
-    gs.append(g)
+  nv, dev = len(gs), variables[0].device
   if clipping_factors is not None:
     _f32_inplace(clipping_factors, "clipping_factors")
     if clipping_factors.numel() != nv or clipping_factors.device != dev:
       raise ValueError(f"clippy_adagrad_dense_: clipping_factors must hold {nv} floats on {dev}")
-  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
-  numels = (ctypes.c_int64 * nv)(*[v.numel() for v in variables])
-  wsb = lib().tfrs_clippy_adagrad_dense_workspace_bytes(nv)
-  ws = workspace(wsb, dev, "clippy")
+  ws = workspace(lib().tfrs_clippy_adagrad_dense_workspace_bytes(nv), dev, "clippy")
   check(lib().tfrs_clippy_adagrad_dense_f32(
-      arr(variables), arr(gs), arr(accums), numels, nv, c_f(lr), c_f(eps), c_f(variable_relative_threshold),
+      *arrays, c_f(lr), c_f(eps), c_f(variable_relative_threshold),
       c_f(accumulator_relative_threshold), c_f(absolute_threshold),
       _clippy_flags(clip_accumulator_update, use_standard_accumulator_update), ptr(clipping_factors), ptr(ws), ws.numel(),
       stream()), "clippy_adagrad_dense")
@@ -1137,19 +1143,7 @@ def sparse_adam_(table: torch.Tensor, m: torch.Tensor, v: torch.Tensor, ids: tor
   """Adam step of one embedding table whose gradient rows `grad_rows` belong to the rows `ids` (duplicates summed in order
   of occurrence, out-of-range ids skipped).  `alpha` is the step size of `adam_alpha`.  Not lazy: every row of the table
   and of its slots `m` / `v` is updated (the untouched ones decay); lazy: only the touched rows."""
-  _f32_inplace(table, "table"); _f32_inplace(m, "m"); _f32_inplace(v, "v")
-  ids = require_cuda(ids, "ids").contiguous().view(-1)
-  g = f32c(grad_rows, "grad_rows")
-  if table.dim() != 2:
-    raise ValueError(f"sparse_adam_: table must be 2-D, got {tuple(table.shape)}")
-  n = ids.numel(); rows, d = table.shape
-  for name, s in (("m", m), ("v", v)):
-    if s.shape != table.shape or s.device != table.device:
-      raise ValueError(f"sparse_adam_: {name} must be {tuple(table.shape)} on {table.device}, got {tuple(s.shape)} on {s.device}")
-  if g.shape != (n, d):
-    raise ValueError(f"sparse_adam_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
-  if ids.device != table.device or g.device != table.device:
-    raise ValueError("sparse_adam_: ids and grad_rows must live on the table's device")
+  ids, g, n, rows, d = _sparse_step_args("sparse_adam_", table, {"m": m, "v": v}, ids, grad_rows)
   ws = workspace(lib().tfrs_sparse_adam_workspace_bytes(n, rows), table.device, "adam")
   check(lib().tfrs_sparse_adam_f32(
       ptr(table), ptr(m), ptr(v), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(alpha), c_f(beta_1),
@@ -1160,25 +1154,9 @@ def adam_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor]
                 vs: Sequence[torch.Tensor], alpha: float, beta_1: float, beta_2: float, epsilon: float) -> None:
   """Adam step of a list of dense variables and their slots `ms` / `vs` in one multi-tensor call; `alpha` is the step
   size of `adam_alpha`."""
-  nv = len(variables)
-  if len(grads) != nv or len(ms) != nv or len(vs) != nv:
-    raise ValueError("adam_dense_: variables, grads, ms and vs must have the same length")
-  if nv == 0:
-    return
-  dev = variables[0].device
-  gs = []
-  for i, (x, g, m, v) in enumerate(zip(variables, grads, ms, vs)):
-    _f32_inplace(x, f"variables[{i}]"); _f32_inplace(m, f"ms[{i}]"); _f32_inplace(v, f"vs[{i}]")
-    g = f32c(g, f"grads[{i}]")
-    if any(t.device != dev for t in (x, g, m, v)):
-      raise ValueError("adam_dense_: every tensor must live on one device")
-    if g.shape != x.shape or m.shape != x.shape or v.shape != x.shape:
-      raise ValueError(f"adam_dense_: grads[{i}] / ms[{i}] / vs[{i}] must have the shape {tuple(x.shape)}")
-    gs.append(g)
-  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
-  numels = (ctypes.c_int64 * nv)(*[x.numel() for x in variables])
-  check(lib().tfrs_adam_dense_f32(arr(variables), arr(gs), arr(ms), arr(vs), numels, nv, c_f(alpha), c_f(beta_1),
-                                  c_f(beta_2), c_f(epsilon), stream()), "adam_dense")
+  gs, arrays = _dense_step_args("adam_dense_", variables, grads, {"ms": ms, "vs": vs})
+  if gs:
+    check(lib().tfrs_adam_dense_f32(*arrays, c_f(alpha), c_f(beta_1), c_f(beta_2), c_f(epsilon), stream()), "adam_dense")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1197,19 +1175,7 @@ def sparse_ftrl_(table: torch.Tensor, accum: torch.Tensor, linear: torch.Tensor,
   """FTRL step of one embedding table whose gradient rows `grad_rows` belong to the rows `ids` (duplicates summed in order
   of occurrence, out-of-range ids skipped).  `l2a` is the l2 strength of `ftrl_l2`.  Only the touched rows of the table
   and of its slots `accum` / `linear` change."""
-  _f32_inplace(table, "table"); _f32_inplace(accum, "accum"); _f32_inplace(linear, "linear")
-  ids = require_cuda(ids, "ids").contiguous().view(-1)
-  g = f32c(grad_rows, "grad_rows")
-  if table.dim() != 2:
-    raise ValueError(f"sparse_ftrl_: table must be 2-D, got {tuple(table.shape)}")
-  n = ids.numel(); rows, d = table.shape
-  for name, s in (("accum", accum), ("linear", linear)):
-    if s.shape != table.shape or s.device != table.device:
-      raise ValueError(f"sparse_ftrl_: {name} must be {tuple(table.shape)} on {table.device}, got {tuple(s.shape)} on {s.device}")
-  if g.shape != (n, d):
-    raise ValueError(f"sparse_ftrl_: grad_rows must be [{n},{d}], got {tuple(g.shape)}")
-  if ids.device != table.device or g.device != table.device:
-    raise ValueError("sparse_ftrl_: ids and grad_rows must live on the table's device")
+  ids, g, n, rows, d = _sparse_step_args("sparse_ftrl_", table, {"accum": accum, "linear": linear}, ids, grad_rows)
   ws = workspace(lib().tfrs_sparse_ftrl_workspace_bytes(n), table.device, "ftrl")
   check(lib().tfrs_sparse_ftrl_f32(
       ptr(table), ptr(accum), ptr(linear), rows, d, ptr(ids), _ffi.ids_dtype_code(ids), n, ptr(g), c_f(lr), c_f(lr_power),
@@ -1221,25 +1187,10 @@ def ftrl_dense_(variables: Sequence[torch.Tensor], grads: Sequence[torch.Tensor]
                 l2_shrinkage: float) -> None:
   """FTRL step of a list of dense variables and their slots `accums` / `linears` in one multi-tensor call; `l2a` is the
   l2 strength of `ftrl_l2`."""
-  nv = len(variables)
-  if len(grads) != nv or len(accums) != nv or len(linears) != nv:
-    raise ValueError("ftrl_dense_: variables, grads, accums and linears must have the same length")
-  if nv == 0:
-    return
-  dev = variables[0].device
-  gs = []
-  for i, (x, g, a, z) in enumerate(zip(variables, grads, accums, linears)):
-    _f32_inplace(x, f"variables[{i}]"); _f32_inplace(a, f"accums[{i}]"); _f32_inplace(z, f"linears[{i}]")
-    g = f32c(g, f"grads[{i}]")
-    if any(t.device != dev for t in (x, g, a, z)):
-      raise ValueError("ftrl_dense_: every tensor must live on one device")
-    if g.shape != x.shape or a.shape != x.shape or z.shape != x.shape:
-      raise ValueError(f"ftrl_dense_: grads[{i}] / accums[{i}] / linears[{i}] must have the shape {tuple(x.shape)}")
-    gs.append(g)
-  arr = lambda ts: (ctypes.c_void_p * nv)(*[t.data_ptr() for t in ts])
-  numels = (ctypes.c_int64 * nv)(*[x.numel() for x in variables])
-  check(lib().tfrs_ftrl_dense_f32(arr(variables), arr(gs), arr(accums), arr(linears), numels, nv, c_f(lr), c_f(lr_power),
-                                  c_f(l1), c_f(l2a), c_f(l2_shrinkage), stream()), "ftrl_dense")
+  gs, arrays = _dense_step_args("ftrl_dense_", variables, grads, {"accums": accums, "linears": linears})
+  if gs:
+    check(lib().tfrs_ftrl_dense_f32(*arrays, c_f(lr), c_f(lr_power), c_f(l1), c_f(l2a), c_f(l2_shrinkage), stream()),
+          "ftrl_dense")
 
 
 # ------------------------------------------------------------------------------------------------

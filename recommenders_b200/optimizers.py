@@ -85,6 +85,15 @@ class _SlotOptimizer:
       self._slots[(id(owner), attr)] = a
     return a
 
+  @staticmethod
+  def _table_grads(t: Embedding) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """A table's gradient for this step, taken off the table: the (ids, rows) of all its lookups concatenated, one
+    variable like the IndexedSlices of the reference; None when no lookup has one."""
+    grads = t.pop_sparse_grads()
+    if not grads:
+      return None
+    return torch.cat([i.reshape(-1) for i, _ in grads], 0), torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
+
   def zero_grad(self):
     self._refresh()
     clear_grads(self._tables, self._dense)
@@ -139,13 +148,9 @@ class Adagrad(_AccumulatorOptimizer):
 
   def _apply(self, tables, dense):
     for t in tables:
-      grads = t.pop_sparse_grads()
-      if not grads:
-        continue
-      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)
-      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
-      ops.sparse_adagrad_(t.weight, self._accum(t, t.weight), ids, rows, self.learning_rate, self.epsilon,
-                          self.eps_inside_sqrt)
+      g = self._table_grads(t)
+      if g is not None:
+        ops.sparse_adagrad_(t.weight, self._accum(t, t.weight), *g, self.learning_rate, self.epsilon, self.eps_inside_sqrt)
     for p in dense:
       if p.grad is None:
         continue
@@ -185,13 +190,10 @@ class Adam(_SlotOptimizer):
     alpha = ops.adam_alpha(self.learning_rate, self.beta_1, self.beta_2, self.iterations + 1)
     rule = dict(alpha=alpha, beta_1=self.beta_1, beta_2=self.beta_2, epsilon=self.epsilon)
     for t in tables:
-      grads = t.pop_sparse_grads()
-      if not grads:
-        continue
-      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)   # one variable: the IndexedSlices of all its lookups
-      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
-      ops.sparse_adam_(t.weight, self._slot(t, self._M_ATTR, t.weight, 0.0), self._slot(t, self._V_ATTR, t.weight, 0.0),
-                       ids, rows, lazy=self.lazy_embeddings, **rule)
+      g = self._table_grads(t)
+      if g is not None:
+        ops.sparse_adam_(t.weight, self._slot(t, self._M_ATTR, t.weight, 0.0), self._slot(t, self._V_ATTR, t.weight, 0.0),
+                         *g, lazy=self.lazy_embeddings, **rule)
     params = [p for p in dense if p.grad is not None]
     if params:
       ops.adam_dense_(params, [p.grad for p in params], [self._slot(p, self._M_ATTR, p, 0.0) for p in params],
@@ -249,12 +251,9 @@ class Ftrl(_SlotOptimizer):
                 l2a=ops.ftrl_l2(self.l2_regularization_strength, self.beta, self.learning_rate),
                 l2_shrinkage=self.l2_shrinkage_regularization_strength)
     for t in tables:
-      grads = t.pop_sparse_grads()
-      if not grads:
-        continue
-      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)   # one variable: the IndexedSlices of all its lookups
-      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
-      ops.sparse_ftrl_(t.weight, *self._slots_of(t, t.weight), ids, rows, **rule)
+      g = self._table_grads(t)
+      if g is not None:
+        ops.sparse_ftrl_(t.weight, *self._slots_of(t, t.weight), *g, **rule)
     params = [p for p in dense if p.grad is not None]
     if params:
       slots = [self._slots_of(p, p) for p in params]
@@ -290,12 +289,9 @@ class SGD(_SlotOptimizer):
 
   def _apply(self, tables, dense):
     for t in tables:
-      grads = t.pop_sparse_grads()
-      if not grads:
-        continue
-      ids = torch.cat([i.reshape(-1) for i, _ in grads], 0)
-      rows = torch.cat([g.reshape(-1, t.output_dim) for _, g in grads], 0)
-      ops.sparse_sgd_(t.weight, ids, rows, self.learning_rate)
+      g = self._table_grads(t)
+      if g is not None:
+        ops.sparse_sgd_(t.weight, *g, self.learning_rate)
     params = [p for p in dense if p.grad is not None]
     if params:
       with torch.no_grad():

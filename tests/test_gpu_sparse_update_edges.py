@@ -39,7 +39,7 @@ from oracle import oracle as orc
 gpu = pytest.mark.gpu
 F32 = np.float32
 
-# csrc/adagrad.cu and csrc/adagrad.cuh (test_constants_match_the_sources reads them back)
+# csrc/adagrad.cu and csrc/adagrad.cuh (test_constants_and_shared_checks_match_the_sources reads them back)
 AG_RANK_MAX = 16384      # bucketed rank sort up to here, bitonic sort beyond
 AG_TILE = 8192           # keys per shared-memory tile of the bitonic sort
 AB_BUCKETS = 256
@@ -601,7 +601,7 @@ def _src(name):
     return f.read()
 
 
-def test_constants_match_the_sources():
+def test_constants_and_shared_checks_match_the_sources():
   cu, cuh = _src("adagrad.cu"), _src("adagrad.cuh")
   src = cu + cuh
   for name, want in (("AG_RANK_MAX", AG_RANK_MAX), ("AG_TILE", AG_TILE), ("AB_BUCKETS", AB_BUCKETS), ("AB_SPLIT", AB_SPLIT),
@@ -614,8 +614,11 @@ def test_constants_match_the_sources():
   assert "(unsigned int)(key >> 24) ^ (unsigned int)(key >> 56)" in cu and "(id * 0x9E3779B1u) >> 24" in cu
   # the position field and n's limit
   assert "0xFFFFFFull" in cu and "0xFFFFFFull" in cuh and "<< 24" in cu
+  # n's limit: ag_check_args holds it, and every sparse entry point calls ag_check_args under its own name
+  # (tests/test_sparse_step_args.py also calls each entry point with n = 2^24)
+  assert "n < (1ll << 24)" in cu
   for f in ("sgd.cu", "adagrad.cu", "clippy_adagrad.cu", "adam.cu", "ftrl.cu"):
-    assert "n < (1ll << 24)" in _src(f), f
+    assert f'ag_check_args("sparse_{f[:-3]}", ' in _src(f), f
 
 
 def test_run_lengths_cover_every_window_and_tile_edge():
