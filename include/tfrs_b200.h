@@ -169,6 +169,35 @@ int tfrs_topk_merge_sorted_strided(const float* scores, const int64_t* idx, int6
                                    float* out_scores, int64_t* out_idx, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K14  exact top-K with overridden rows, and its hit count: the device side of examples.movielens.evaluate
+ * (examples/movielens.py:71-88, `scores[train_movies] = -1e6; top_movies = argsort(-scores)[:k]`).  Query u lists the
+ * rows rows[offsets[u] .. offsets[u+1]) (CSR, int64, sorted and unique per query, in [0, N)); those rows score exactly
+ * -1e6f instead of their canonical dot.  Order = (score desc, row asc); k_out = min(k, N) entries per query.
+ * `users` (nullable = 0 .. n-1) maps position j of a call to query users[j]: its row of q, its list and its output row
+ * (out_* rows are out_ld apart).  Both routes give the same bits.
+ *
+ * tfrs_topk_override_merge_f32   scan route: list_* = [n, w] the top w of each query by canonical score (what
+ *                                tfrs_topk_scan_f32 / tfrs_topk_tc_f32 emit) with w >= min(N, k + list length) and
+ *                                k_out <= w <= 256.  Drops the listed rows, merges the first k survivors with the listed
+ *                                rows at -1e6, writes k_out.  No workspace.
+ * tfrs_topk_overriding_dense_f32 dense route, any list length, k <= 2048: chunks of queries are scored into the workspace
+ *                                ([chunk, N] fp32 plus the chunk's query rows and selections), the listed entries are
+ *                                overwritten and the rows selected.  The chunk is the largest the given workspace holds;
+ *                                tfrs_topk_overriding_dense_workspace_bytes sizes one of at most 256 MB.
+ * tfrs_count_listed              out_count[u] = #{t in [offsets[u], offsets[u+1]) : rows[t] is among top_rows[u, 0..kk)}
+ *                                (entries counted with multiplicity; rows need not be sorted here).  kk <= 2048.
+ * ------------------------------------------------------------------------------------------- */
+int tfrs_topk_override_merge_f32(const float* list_scores, const int64_t* list_idx, int64_t n, int w, const int64_t* users,
+                                 const int64_t* offsets, const int64_t* rows, int k, int k_out, float* out_scores,
+                                 int64_t* out_idx, int out_ld, void* stream);
+size_t tfrs_topk_overriding_dense_workspace_bytes(int64_t n, int64_t N, int d, int k);
+int tfrs_topk_overriding_dense_f32(const float* q, const int64_t* users, int64_t n, const float* corpus, int64_t N, int d,
+                                   int k, const int64_t* offsets, const int64_t* rows, float* out_scores, int64_t* out_idx,
+                                   int out_ld, void* ws, size_t ws_bytes, void* stream);
+int tfrs_count_listed(const int64_t* top_rows, int64_t Q, int kk, int64_t ld, const int64_t* offsets, const int64_t* rows,
+                      int32_t* out_count, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * C1  the collective of the row-sharded scan (SURVEY 8b/8e; the reference has no sharded scan -- its corpus is one
  * variable, layers/factorized_top_k.py:571-580 -- and its only collective helper is tasks/retrieval.py:238-321).
  * One process per GPU; shard g owns a contiguous row block, so global index order == (shard, local index) order and

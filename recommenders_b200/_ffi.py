@@ -50,6 +50,10 @@ _SIGNATURES = {
     "tfrs_profile_read": (c_i, [c_p, c_p]),
     "tfrs_topk_merge_strided": (c_i, [c_p, c_p, c_l, c_l, c_i, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_topk_merge_sorted_strided": (c_i, [c_p, c_p, c_l, c_l, c_i, c_l, c_i, c_i, c_p, c_p, c_p]),
+    "tfrs_topk_override_merge_f32": (c_i, [c_p, c_p, c_l, c_i, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_p]),
+    "tfrs_topk_overriding_dense_workspace_bytes": (c_sz, [c_l, c_l, c_i, c_i]),
+    "tfrs_topk_overriding_dense_f32": (c_i, [c_p, c_p, c_l, c_p, c_l, c_i, c_i, c_p, c_p, c_p, c_p, c_i, c_p, c_sz, c_p]),
+    "tfrs_count_listed": (c_i, [c_p, c_l, c_i, c_l, c_p, c_p, c_p, c_p]),
     "tfrs_comm_unique_id": (c_i, [c_p]),
     "tfrs_comm_create": (c_i, [c_p, c_i, c_i, c_p]),
     "tfrs_comm_destroy": (c_i, [c_p]),

@@ -576,6 +576,119 @@ def topk_merge(scores: torch.Tensor, idx: torch.Tensor, k: int, sorted_lists: bo
 
 
 # ------------------------------------------------------------------------------------------------
+# K14 top-k with overridden rows (examples.movielens.evaluate; DESIGN.md §2 pins the rules)
+# ------------------------------------------------------------------------------------------------
+OVERRIDE_SCORE = np.float32(-1e6)
+OVERRIDE_MAX_K = 2048
+
+
+def _csr(offsets, rows, Q: int, N: int, device, what: str, sorted_unique: bool):
+  """Host offsets (int64 NumPy [Q+1]) and device offsets / rows (int64) of per-query row lists, checked on the host."""
+  off = np.ascontiguousarray(offsets.detach().cpu().numpy() if isinstance(offsets, torch.Tensor) else offsets, np.int64)
+  r = np.ascontiguousarray(rows.detach().cpu().numpy() if isinstance(rows, torch.Tensor) else rows, np.int64).reshape(-1)
+  if off.shape != (Q + 1,) or off[0] != 0 or off[-1] != r.shape[0] or (np.diff(off) < 0).any():
+    raise ValueError(f"{what}: offsets must be [Q+1] = [{Q + 1}] non-decreasing from 0 to len(rows) = {r.shape[0]}")
+  if r.size and (r.min() < 0 or r.max() >= N):
+    raise ValueError(f"{what}: rows must lie in [0, {N})")
+  if sorted_unique and r.size > 1:
+    ok = np.diff(r) > 0
+    starts = off[1:-1]
+    ok[starts[(starts > 0) & (starts < r.shape[0])] - 1] = True   # a new list may start lower
+    if not ok.all():
+      raise ValueError(f"{what}: every query's rows must be sorted and unique")
+  return off, torch.from_numpy(off).to(device), torch.from_numpy(r).to(device)
+
+
+def _override_out(q: torch.Tensor, corpus: torch.Tensor, k: int, what: str):
+  q = f32c(q, "queries"); corpus = f32c(corpus, "candidates")
+  if q.dim() != 2 or corpus.dim() != 2 or q.shape[1] != corpus.shape[1]:
+    raise ValueError(f"{what}: shape mismatch {tuple(q.shape)} vs {tuple(corpus.shape)}")
+  if not 0 < k <= OVERRIDE_MAX_K:
+    raise ValueError(f"{what}: k={k} out of range (1..{OVERRIDE_MAX_K})")
+  k_out = min(k, corpus.shape[0])
+  out_s = torch.empty((q.shape[0], k_out), dtype=torch.float32, device=q.device)
+  out_i = torch.empty((q.shape[0], k_out), dtype=torch.int64, device=q.device)
+  return q, corpus, out_s, out_i
+
+
+def _overriding_dense(q, corpus, k, off_d, rows_d, users, out_s, out_i, max_chunk_bytes) -> None:
+  n = q.shape[0] if users is None else users.numel()
+  (_, d), N = q.shape, corpus.shape[0]
+  if n == 0 or out_s.shape[1] == 0:
+    return
+  nb = lib().tfrs_topk_overriding_dense_workspace_bytes(n, N, d, k)
+  if max_chunk_bytes is not None:
+    nb = min(nb, int(max_chunk_bytes))
+  ws = workspace(nb, q.device, "override")
+  check(lib().tfrs_topk_overriding_dense_f32(ptr(q), ptr(users), n, ptr(corpus), N, d, k, ptr(off_d), ptr(rows_d), ptr(out_s),
+                                             ptr(out_i), out_s.shape[1], ptr(ws), nb, stream()), "topk_overriding_dense")
+
+
+def topk_overriding_dense(q: torch.Tensor, corpus: torch.Tensor, k: int, offsets, rows,
+                          max_chunk_bytes: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+  """`topk_overriding` on its dense route for every query: exact scores of a chunk of queries, the listed entries set to
+  -1e6, then a per-row selection.  `max_chunk_bytes` caps the workspace of one chunk (default: at most 256 MB)."""
+  q, corpus, out_s, out_i = _override_out(q, corpus, k, "topk_overriding_dense")
+  _, off_d, rows_d = _csr(offsets, rows, q.shape[0], corpus.shape[0], q.device, "topk_overriding_dense", True)
+  _overriding_dense(q, corpus, k, off_d, rows_d, None, out_s, out_i, max_chunk_bytes)
+  return out_s, out_i
+
+
+def override_width(k: int, list_lengths: np.ndarray, N: int) -> np.ndarray:
+  """Width of the top-w list each query's scan route reads: min(N, k + e) rounded up to a power of two (at least k, at
+  most TC_MAX_K), so the queries fall into a few width classes.  0 marks a query for the dense route."""
+  need = np.minimum(N, k + np.asarray(list_lengths, np.int64))
+  w = np.maximum(k, 1 << np.ceil(np.log2(np.maximum(need, 1))).astype(np.int64))
+  w = np.minimum(np.minimum(w, TC_MAX_K), N)
+  return np.where(need <= TC_MAX_K, w, 0)
+
+
+def topk_overriding(q: torch.Tensor, corpus: torch.Tensor, k: int, offsets, rows, image=None
+                    ) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Exact top-k of each query over the corpus rows where query u's listed rows rows[offsets[u]:offsets[u+1]] (sorted,
+  unique, any length 0..N) score exactly -1e6 instead of their canonical dot.  Order = (score desc, row asc).
+  Returns ([Q, min(k, N)] f32 scores, [Q, min(k, N)] i64 rows).
+
+  A query with min(N, k + e) <= TC_MAX_K (e = its list length) takes the scan route: `topk` at its width class
+  (`override_width`; the tensor-core scan when `uses_tc_scan` holds and an `image` is given, the exact scan otherwise),
+  then one merge kernel drops the listed rows and merges the first k survivors with them.  The top w by true score hold
+  at least k survivors, and any survivor outside them ranks after the k-th, so this is exact.  Other queries take
+  `topk_overriding_dense`'s route; both routes give the same bits.  `image` is the corpus's tensor-core image
+  (index_build), the name of a scratch slot to build it in once, or None.  `offsets` are read on the host."""
+  q, corpus, out_s, out_i = _override_out(q, corpus, k, "topk_overriding")
+  (Q, d), N = q.shape, corpus.shape[0]
+  off_h, off_d, rows_d = _csr(offsets, rows, Q, N, q.device, "topk_overriding", True)
+  k_out = out_s.shape[1]
+  if Q == 0 or k_out == 0:
+    return out_s, out_i
+  width = override_width(k, np.diff(off_h), N)
+  if isinstance(image, str) and any(uses_tc_scan(Q, N, d, int(w)) for w in np.unique(width) if w):
+    image = index_build(corpus, reuse_slot=image)
+  for w in np.unique(width[width > 0]).tolist():
+    users = torch.from_numpy(np.nonzero(width == w)[0]).to(q.device)
+    ls, li = topk(q.index_select(0, users), corpus, w, image=image)
+    check(lib().tfrs_topk_override_merge_f32(ptr(ls), ptr(li), users.numel(), ls.shape[1], ptr(users), ptr(off_d), ptr(rows_d),
+                                             k, k_out, ptr(out_s), ptr(out_i), k_out, stream()), "topk_override_merge")
+  dense = np.nonzero(width == 0)[0]
+  if dense.size:
+    _overriding_dense(q, corpus, k, off_d, rows_d, torch.from_numpy(dense).to(q.device), out_s, out_i, None)
+  return out_s, out_i
+
+
+def count_listed(top_rows: torch.Tensor, offsets, rows) -> torch.Tensor:
+  """int32 [Q]: per query, how many of its listed rows rows[offsets[u]:offsets[u+1]] (duplicates counted each time)
+  appear among top_rows[u] ([Q, kk] int64, kk <= 2048)."""
+  top = require_cuda(top_rows, "top_rows").to(torch.int64).contiguous()
+  Q, kk = top.shape
+  if kk > OVERRIDE_MAX_K:
+    raise ValueError(f"count_listed: {kk} rows per query, at most {OVERRIDE_MAX_K}")
+  _, off_d, rows_d = _csr(offsets, rows, Q, np.iinfo(np.int64).max, top.device, "count_listed", False)
+  out = torch.empty((Q,), dtype=torch.int32, device=top.device)
+  check(lib().tfrs_count_listed(ptr(top), Q, kk, kk, ptr(off_d), ptr(rows_d), ptr(out), stream()), "count_listed")
+  return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K9 tree-AH: index build and search (DESIGN.md §2 pins every rule)
 # ------------------------------------------------------------------------------------------------
 TREE_AH_MAX_TRAIN = 100000
