@@ -731,6 +731,45 @@ int tfrs_dot_interaction_fwd_f32(const float* feats, int64_t B, int F, int d, in
 int tfrs_dot_interaction_bwd_f32(const float* feats, const float* gout, int64_t B, int F, int d, int self_interaction,
                                  int skip_gather, float* dfeats, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K15 vocabulary lookup: tf.keras.layers.StringLookup / IntegerLookup (tf-keras index_lookup.py) as the reference's
+ * towers use them (`Sequential([StringLookup(vocabulary=ids, mask_token=None), Embedding(len(ids) + 1, d)])`).
+ *
+ * A table maps each of V distinct keys (V < 2^30) to its position 0..V-1: an int64 vocabulary (kind TFRS_I64, `keys`
+ * int64 [V]) or a string one (TFRS_BYTES, `keys` = the bytes back to back, `offsets` int64 [V+1]).  The caller keeps the
+ * keys alive as long as the table; `slots` is tfrs_lookup_table_bytes(V, kind) bytes of device memory, 256-byte aligned,
+ * that tfrs_lookup_build fills (its contents may differ from build to build; results never do).  The mask token
+ * (has_mask != 0) is `mask` for TFRS_I64 and the mask_len bytes at `mask_bytes` (device) for TFRS_BYTES.
+ *   tfrs_lookup_slots: the table's slot count for V keys (a power of two >= 2V, at least 64), -1 when V is out of range.
+ *   tfrs_lookup_build: fills `slots`; *dup = 1 when two keys are equal (compared as int64, or as byte strings), else 0.
+ *     One launch for TFRS_I64, two for TFRS_BYTES, after two memsets.
+ *   tfrs_lookup: out[i] (int64) = 0 if value i equals the mask token, base + p if it equals key p, otherwise `oov` --
+ *     or, when `miss` is not NULL, -1 and *miss = 1 (the caller zeroes *miss).  `values`: TFRS_I32 / TFRS_I64 against an
+ *     I64 table (compared as int64), TFRS_BYTES with `offsets` [n+1] against a BYTES table.  One launch; n == 0 writes
+ *     nothing.
+ *   tfrs_lookup_invert: out[i] = keys[x - base] (or x - base when keys is NULL) for x = idx[i] (TFRS_I32 / TFRS_I64) in
+ *     [base, base + V); mask_out for x == 0 when has_mask; oov_out for every other x.  One launch.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct tfrs_lookup_table {
+  const void* keys;            /* TFRS_I64: int64 [V]; TFRS_BYTES: the keys' bytes */
+  const int64_t* offsets;      /* TFRS_BYTES: [V + 1]; key p = bytes [offsets[p], offsets[p+1]) of keys */
+  int64_t V;
+  int32_t kind;                /* TFRS_I64 or TFRS_BYTES */
+  int32_t has_mask;
+  int64_t mask;                /* TFRS_I64: the mask token */
+  const uint8_t* mask_bytes;   /* TFRS_BYTES: the mask token's bytes */
+  int64_t mask_len;
+  void* slots;                 /* tfrs_lookup_table_bytes(V, kind) bytes */
+} tfrs_lookup_table;
+
+int64_t tfrs_lookup_slots(int64_t V);
+size_t tfrs_lookup_table_bytes(int64_t V, int kind);
+int tfrs_lookup_build(const tfrs_lookup_table* table, int32_t* dup, void* stream);
+int tfrs_lookup(const tfrs_lookup_table* table, const void* values, const int64_t* offsets, int kind, int64_t n,
+                int64_t base, int64_t oov, int32_t* miss, int64_t* out, void* stream);
+int tfrs_lookup_invert(const void* idx, int kind, int64_t n, const int64_t* keys, int64_t V, int64_t base, int has_mask,
+                       int64_t mask_out, int64_t oov_out, int64_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

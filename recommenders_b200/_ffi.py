@@ -139,6 +139,11 @@ _SIGNATURES = {
     "tfrs_tree_ah_search_workspace_bytes": (c_sz, [c_l, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_l]),
     "tfrs_tree_ah_search_f32": (c_i, [c_p, c_l, c_i, c_p, c_i, c_p, c_p, c_i, c_p, c_p, c_l, c_p, c_i, c_i, c_i, c_p, c_p,
                                       c_p, c_sz, c_p]),
+    "tfrs_lookup_slots": (c_l, [c_l]),
+    "tfrs_lookup_table_bytes": (c_sz, [c_l, c_i]),
+    "tfrs_lookup_build": (c_i, [c_p, c_p, c_p]),
+    "tfrs_lookup": (c_i, [c_p, c_p, c_p, c_i, c_l, c_l, c_l, c_p, c_p, c_p]),
+    "tfrs_lookup_invert": (c_i, [c_p, c_i, c_l, c_p, c_l, c_l, c_i, c_l, c_l, c_p, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

@@ -13,13 +13,13 @@
 // Pooled slots then take one more launch: a group of dim/4 lanes per (bag, slot) sums the bag's rows in value order.
 // Backward: one launch writes each table's gradient rows, contiguous, in the caller's order.  No float atomics.
 #include "common.cuh"
+#include "siphash.cuh"
 
 namespace tfrs {
 
 constexpr int UE_THREADS = 256;
 constexpr int UE_MAX_FEATURES = 64;     // per launch; longer calls are split into groups of whole features
 constexpr int UE_MAX_SLOTS = 256;
-constexpr int UE_SHORT = 23;            // messages up to this many bytes live in three 64-bit registers
 
 struct UeFeat {
   const void* values;
@@ -48,23 +48,6 @@ struct UeParams {
 };
 static_assert(sizeof(UeParams) <= 32000, "kernel parameters must stay under the 32 KB limit");
 
-__device__ __forceinline__ uint64_t rotl(uint64_t x, int b) { return (x << b) | (x >> (64 - b)); }
-
-struct Sip {
-  uint64_t v0, v1, v2, v3;
-  __device__ __forceinline__ Sip(uint64_t k0, uint64_t k1)
-      : v0(k0 ^ 0x736f6d6570736575ull), v1(k1 ^ 0x646f72616e646f6dull), v2(k0 ^ 0x6c7967656e657261ull),
-        v3(k1 ^ 0x7465646279746573ull) {}
-  __device__ __forceinline__ void round() {
-    v0 += v1; v1 = rotl(v1, 13); v1 ^= v0; v0 = rotl(v0, 32);
-    v2 += v3; v3 = rotl(v3, 16); v3 ^= v2;
-    v0 += v3; v3 = rotl(v3, 21); v3 ^= v0;
-    v2 += v1; v1 = rotl(v1, 17); v1 ^= v2; v2 = rotl(v2, 32);
-  }
-  __device__ __forceinline__ void block(uint64_t m) { v3 ^= m; round(); round(); v0 ^= m; }
-  __device__ __forceinline__ uint64_t finish() { v2 ^= 0xff; round(); round(); round(); round(); return v0 ^ v1 ^ v2 ^ v3; }
-};
-
 // x mod d with magic = floor((2^64 - 1) / d), d >= 1: the estimate q = hi64(x * magic) is at most 2 below floor(x / d)
 // (DESIGN.md K8), so two conditional subtractions make the remainder exact for every d < 2^64.
 __device__ __forceinline__ uint64_t mod_magic(uint64_t x, uint64_t d, uint64_t magic) {
@@ -73,15 +56,6 @@ __device__ __forceinline__ uint64_t mod_magic(uint64_t x, uint64_t d, uint64_t m
   if (r >= d) r -= d;
   return r;
 }
-
-// 192-bit little-endian message register: push(c) shifts every byte up by one and puts c at byte 0
-struct Msg {
-  uint64_t w0 = 0, w1 = 0, w2 = 0;
-  int len = 0;
-  __device__ __forceinline__ void push(uint32_t c) {
-    w2 = (w2 << 8) | (w1 >> 56); w1 = (w1 << 8) | (w0 >> 56); w0 = (w0 << 8) | c; ++len;
-  }
-};
 
 // tf.as_string of an int64: digits generated least significant first and pushed at byte 0, so the most significant
 // digit ends at byte 0.  |x| is split into 32-bit pieces below 10^9.
@@ -109,29 +83,6 @@ __device__ __forceinline__ Msg decimal_msg(long long x) {
   return m;
 }
 
-__device__ __forceinline__ uint64_t load_word(const uint8_t* p, int nbytes) {
-  uint64_t w = 0;
-  for (int k = nbytes - 1; k >= 0; --k) w = (w << 8) | p[k];
-  return w;
-}
-
-// SipHash-2-4 of a formed message: short ones from registers, longer strings from memory (`p`, `len` bytes).
-__device__ __forceinline__ uint64_t siphash(const Msg& m, const uint8_t* p, uint64_t k0, uint64_t k1) {
-  Sip s(k0, k1);
-  const int nb = m.len >> 3;
-  uint64_t last;
-  if (m.len <= UE_SHORT) {
-    if (nb > 0) s.block(m.w0);
-    if (nb > 1) s.block(m.w1);
-    last = nb == 0 ? m.w0 : (nb == 1 ? m.w1 : m.w2);
-  } else {
-    for (int b = 0; b < nb; ++b) s.block(load_word(p + 8 * b, 8));
-    last = load_word(p + 8 * nb, m.len & 7);
-  }
-  s.block(last | ((uint64_t)(m.len & 0xff) << 56));
-  return s.finish();
-}
-
 // The message of value i of a feature (kind: TFRS_I32, TFRS_I64, TFRS_BYTES); *p is the start of a byte string.
 __device__ __forceinline__ Msg form_msg(const UeFeat& f, long long i, const uint8_t** p) {
   *p = nullptr;
@@ -140,13 +91,7 @@ __device__ __forceinline__ Msg form_msg(const UeFeat& f, long long i, const uint
   const long long o0 = f.offsets[i], o1 = f.offsets[i + 1];
   const uint8_t* b = reinterpret_cast<const uint8_t*>(f.values) + o0;
   Msg m;
-  const long long len = o1 > o0 ? o1 - o0 : 0;
-  if (len <= UE_SHORT) {
-    for (int k = (int)len - 1; k >= 0; --k) m.push(b[k]);
-  } else {
-    m.len = (int)min(len, (long long)INT32_MAX);
-    *p = b;
-  }
+  bytes_msg(m, b, o1 > o0 ? o1 - o0 : 0, p);
   return m;
 }
 

@@ -4,4 +4,6 @@ from . import embedding
 from . import factorized_top_k
 from . import feature_interaction
 from . import loss
+from . import preprocessing
 from .feature_interaction import dcn
+from .preprocessing import IntegerLookup, StringLookup

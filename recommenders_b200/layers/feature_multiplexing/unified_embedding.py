@@ -26,6 +26,7 @@ import numpy as np
 import torch
 
 from ... import ops
+from ..._strings import is_strings as _is_strings, pack_strings as _pack_strings
 from ..embedding import Embedding
 
 
@@ -110,31 +111,6 @@ class UnifiedEmbeddingConfig:
   @property
   def hashing_config(self):
     return self._hashing_configs
-
-
-def _pack_strings(values) -> Tuple[np.ndarray, np.ndarray, Tuple[int, ...]]:
-  """(UTF-8 bytes of every string back to back, int64 offsets [n+1], shape), vectorised over the array."""
-  a = np.asarray(values)
-  if a.dtype.kind == "O":
-    first = next(iter(a.flat), "")
-    a = a.astype("S" if isinstance(first, (bytes, np.bytes_)) else "U")
-  if a.dtype.kind == "U":
-    a = np.char.encode(a, "utf-8")
-  flat = np.ascontiguousarray(a.reshape(-1))
-  lens = np.char.str_len(flat).astype(np.int64) if flat.size else np.zeros(0, np.int64)
-  offsets = np.zeros(flat.size + 1, np.int64)
-  np.cumsum(lens, out=offsets[1:])
-  w = flat.dtype.itemsize
-  if flat.size == 0 or w == 0:
-    return np.zeros(0, np.uint8), offsets, a.shape
-  data = flat.view(np.uint8).reshape(flat.size, w)[np.arange(w) < lens[:, None]]
-  return data, offsets, a.shape
-
-
-def _is_strings(x) -> bool:
-  if isinstance(x, np.ndarray):
-    return x.dtype.kind in "USO"
-  return isinstance(x, list) and len(x) > 0 and isinstance(x[0], (str, bytes))
 
 
 class _Feature:

@@ -1772,5 +1772,114 @@ def listwise_ndcg(predictions: torch.Tensor, labels, sample_weight=None, topn: O
   return (stats, nd) if per_list else stats
 
 
+# ------------------------------------------------------------------------------------------------
+# K15 vocabulary lookup: the hash tables of layers.StringLookup / IntegerLookup
+# ------------------------------------------------------------------------------------------------
+class _LookupTableDesc(ctypes.Structure):
+  _fields_ = [("keys", ctypes.c_void_p), ("offsets", ctypes.c_void_p), ("V", ctypes.c_int64), ("kind", ctypes.c_int32),
+              ("has_mask", ctypes.c_int32), ("mask", ctypes.c_int64), ("mask_bytes", ctypes.c_void_p),
+              ("mask_len", ctypes.c_int64), ("slots", ctypes.c_void_p)]
+
+
+class LookupTable(NamedTuple):
+  """A built vocabulary table: int64 `keys` [V], or uint8 string bytes with int64 `offsets` [V+1]; `mask` is the int mask
+  token or the uint8 bytes of the string one (None: no mask); `slots` is the table memory the build filled."""
+  keys: torch.Tensor
+  offsets: Optional[torch.Tensor]
+  mask: object
+  slots: torch.Tensor
+
+  @property
+  def size(self) -> int:
+    return self.keys.numel() if self.offsets is None else self.offsets.numel() - 1
+
+  def desc(self) -> _LookupTableDesc:
+    d = _LookupTableDesc()
+    d.keys, d.V, d.slots = self.keys.data_ptr(), self.size, self.slots.data_ptr()
+    d.kind = _ffi.I64 if self.offsets is None else _ffi.BYTES
+    if self.offsets is not None:
+      d.offsets = self.offsets.data_ptr()
+    if self.mask is not None:
+      d.has_mask = 1
+      if self.offsets is None:
+        d.mask = int(self.mask)
+      else:
+        d.mask_bytes, d.mask_len = self.mask.data_ptr(), self.mask.numel()
+    return d
+
+
+def lookup_build(keys: torch.Tensor, offsets: Optional[torch.Tensor] = None, mask=None) -> LookupTable:
+  """Builds the table of a vocabulary on its device: CUDA int64 `keys` [V], or the uint8 bytes of V strings with their int64
+  `offsets` [V+1].  `mask` is the mask token (an int, or a CUDA uint8 tensor of the string's bytes) or None.  Raises
+  ValueError when two keys are equal; that check is the only host read (4 bytes) of the build."""
+  require_cuda(keys, "keys")
+  if offsets is None:
+    if keys.dtype != torch.int64 or keys.dim() != 1:
+      raise TypeError("lookup_build: integer keys must be a 1-D int64 tensor")
+    kind, V = _ffi.I64, keys.numel()
+  else:
+    require_cuda(offsets, "offsets")
+    if keys.dtype != torch.uint8 or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+      raise TypeError("lookup_build: string keys must be uint8 bytes with 1-D int64 offsets [V+1]")
+    if mask is not None:
+      require_cuda(mask, "mask")
+      if mask.dtype != torch.uint8:
+        raise TypeError("lookup_build: the string mask token must be uint8 bytes")
+      mask = mask.contiguous()
+    kind, V = _ffi.BYTES, offsets.numel() - 1
+  nb = lib().tfrs_lookup_table_bytes(V, kind)
+  if nb == 0:
+    raise ValueError(f"lookup_build: {V} keys; a table holds fewer than 2^30")
+  table = LookupTable(keys.contiguous(), None if offsets is None else offsets.contiguous(), mask,
+                      torch.empty((nb,), dtype=torch.uint8, device=keys.device))
+  dup = torch.empty((1,), dtype=torch.int32, device=keys.device)
+  desc = table.desc()
+  check(lib().tfrs_lookup_build(ctypes.byref(desc), ptr(dup), stream()), "lookup_build")
+  if int(dup.item()):
+    raise ValueError("lookup_build: the vocabulary has duplicate entries")
+  return table
+
+
+def lookup(table: LookupTable, values, base: int, oov: Optional[int]) -> torch.Tensor:
+  """int64 index of every value, in the values' shape: 0 for the mask token, base + p for vocabulary key p, `oov` for any
+  other value.  `values` is a CUDA int32 / int64 tensor (integer tables) or a (uint8 bytes, int64 offsets [n+1]) pair of
+  CUDA tensors (string tables, 1-D output).  With oov=None a value outside the vocabulary raises ValueError, which costs
+  one 4-byte read; otherwise the call never reads device memory on the host.  One launch."""
+  values, offsets = values if isinstance(values, tuple) else (values, None)
+  kind = _value_kind(values, offsets)
+  values = values.contiguous()
+  offsets = offsets.contiguous() if offsets is not None else None
+  n = values.numel() if offsets is None else offsets.numel() - 1
+  out = torch.empty(values.shape if offsets is None else (n,), dtype=torch.int64, device=values.device)
+  if n == 0:
+    return out
+  miss = torch.zeros((1,), dtype=torch.int32, device=values.device) if oov is None else None
+  desc = table.desc()
+  check(lib().tfrs_lookup(ctypes.byref(desc), ptr(values), ptr(offsets), kind, n, int(base), -1 if oov is None else int(oov),
+                          ptr(miss), ptr(out), stream()), "lookup")
+  if miss is not None and int(miss.item()):
+    raise ValueError("lookup: a value is not in the vocabulary, and there is no out-of-vocabulary index "
+                     "(num_oov_indices=0)")
+  return out
+
+
+def lookup_invert(idx: torch.Tensor, size: int, base: int, keys: Optional[torch.Tensor], mask_out: Optional[int],
+                  oov_out: int) -> torch.Tensor:
+  """int64 [idx's shape]: keys[x - base] for an index x in [base, base + size) (x - base when keys is None), mask_out for
+  x == 0 when mask_out is not None, oov_out for every other x.  One launch."""
+  require_cuda(idx, "indices")
+  kind = _ffi.ids_dtype_code(idx)
+  idx = idx.contiguous()
+  out = torch.empty(idx.shape, dtype=torch.int64, device=idx.device)
+  if keys is not None:
+    require_cuda(keys, "keys")
+    if keys.dtype != torch.int64 or keys.numel() != size:
+      raise ValueError("lookup_invert: keys must be int64 [size]")
+  check(lib().tfrs_lookup_invert(ptr(idx), kind, idx.numel(), ptr(keys), int(size), int(base), int(mask_out is not None),
+                                 0 if mask_out is None else int(mask_out), int(oov_out), ptr(out), stream()),
+        "lookup_invert")
+  return out
+
+
 def launch_count() -> int:
   return int(lib().tfrs_launch_count())
