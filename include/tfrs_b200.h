@@ -770,6 +770,62 @@ int tfrs_lookup(const tfrs_lookup_table* table, const void* values, const int64_
 int tfrs_lookup_invert(const void* idx, int kind, int64_t n, const int64_t* keys, int64_t V, int64_t base, int has_mask,
                        int64_t mask_out, int64_t oov_out, int64_t* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K16 text vectorization: tf.keras.layers.TextVectorization(output_mode="int", split="whitespace") as the reference's
+ * movie towers use it (`TextVectorization(max_tokens=10_000)` -> `Embedding(..., mask_zero=True)` -> pooling).
+ *
+ * n strings (TFRS_BYTES layout: `data` with int64 `offsets` [n+1], nbytes = offsets[n] < 2^32 bytes in all).
+ *   tfrs_text_standardize: for each string, ASCII-lowercases the bytes (flags & TFRS_TEXT_LOWER) and deletes the 32 bytes
+ *     of Python's string.punctuation (flags & TFRS_TEXT_STRIP), writing the result to `scratch` at the string's own
+ *     offsets and filling the rest of its range with spaces.  counts[i] (int32) = the number of tokens of string i: the
+ *     runs of bytes other than " \t\n\v\f\r".  When max_count is not NULL, *max_count = the largest count (0 for n == 0).
+ *     One launch after a 4-byte memset.
+ *   tfrs_text_lookup: out [n, T] int64: token j of string i (j < T) looked up in a BYTES lookup table, base + p for
+ *     vocabulary entry p and `oov` for any other token; 0 after the string's last token.  Tokens past T are dropped.
+ *     One launch; no atomics.
+ *   tfrs_text_spans: the tokens themselves: token j of string i is spans[2k] = its first byte's offset in scratch and
+ *     spans[2k+1] = its length, k = token_offsets[i] + j (token_offsets [n+1]: the exclusive sum of counts).  One launch.
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_TEXT_LOWER = 1, TFRS_TEXT_STRIP = 2 };
+
+int tfrs_text_standardize(const uint8_t* data, const int64_t* offsets, int64_t n, int64_t nbytes, int flags,
+                          uint8_t* scratch, int32_t* counts, int32_t* max_count, void* stream);
+int tfrs_text_lookup(const tfrs_lookup_table* table, const uint8_t* scratch, const int64_t* offsets, int64_t n, int64_t T,
+                     int64_t base, int64_t oov, int64_t* out, void* stream);
+int tfrs_text_spans(const uint8_t* scratch, const int64_t* offsets, int64_t n, const int64_t* token_offsets,
+                    int64_t* spans, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * K17 numeric columns and pooling: tf.keras.layers.Discretization, Normalization and GlobalAveragePooling1D as the
+ * reference's context-feature towers use them.  Values are TFRS_I32, TFRS_I64, TFRS_F32 or TFRS_F64 (device, contiguous).
+ *   tfrs_bucketize: out[i] (int64) = #{j : b[j] <= x_i} over the nb sorted float32 boundaries (std::upper_bound; NaN gives
+ *     nb).  Integers are rounded to float32 first; float64 values are compared as doubles.  One launch.
+ *   tfrs_normalize: out[i] = (f32(x_i) - mean[c]) / max(sqrt(var[c]), 1e-7f), or with invert mean[c] + f32(x_i) *
+ *     max(sqrt(var[c]), 1e-7f), c = i % C; one IEEE float32 operation per step, no FMA.  One launch.
+ *   tfrs_normalization_adapt: merges the batches of x ([N, R] rows, channel of element (r, e) = e % C; C divides R) into
+ *     state [2, C] = (mean, variance) float32 and *count (int64), as Keras's Normalization.update_state does: batch k holds
+ *     rows [k*batch_rows, (k+1)*batch_rows).  Batch moments: float32 of the float64 sums (in row-major order) of f32(x)
+ *     and of f32((f32(x) - m)^2), over the batch's count; then, in float32, w = n_b / n_total, mean' = mean*(1-w) +
+ *     m*w, var' = (var + (mean-mean')^2)*(1-w) + (v + (m-mean')^2)*w.  One launch when N <= batch_rows, else two (every
+ *     batch's moments, then one fold per channel); ws is tfrs_normalization_adapt_workspace_bytes bytes.
+ *   tfrs_mean_pool_fwd: out [B, d] = sum_t x[b,t,:]*m[b,t] / sum_t m[b,t] (products and the sum in float32, t ascending
+ *     from +0.0f; an all-masked row is 0/0), or without a mask sum_t x[b,t,:] / T.  x is addressed by element strides;
+ *     mask [B, T] contiguous of mask_kind TFRS_I32 / TFRS_I64 / TFRS_BOOL (nonzero = kept), or NULL.  One launch.
+ *   tfrs_mean_pool_bwd: dx [B, T, d] contiguous = f32(g[b,:] / sum_t m[b,t]) * m[b,t], or g[b,:] / T.  One launch.
+ * ------------------------------------------------------------------------------------------- */
+enum { TFRS_F32 = 3, TFRS_F64 = 4, TFRS_BOOL = 5 };
+
+int tfrs_bucketize(const void* x, int kind, int64_t n, const float* bounds, int64_t nb, int64_t* out, void* stream);
+int tfrs_normalize(const void* x, int kind, int64_t n, int64_t C, const float* mean, const float* var, int invert,
+                   float* out, void* stream);
+size_t tfrs_normalization_adapt_workspace_bytes(int64_t N, int64_t C, int64_t batch_rows);
+int tfrs_normalization_adapt(const void* x, int kind, int64_t N, int64_t R, int64_t C, int64_t batch_rows, float* state,
+                             int64_t* count, void* ws, size_t ws_bytes, void* stream);
+int tfrs_mean_pool_fwd(const float* x, int64_t B, int64_t T, int64_t d, int64_t sb, int64_t st, int64_t sd,
+                       const void* mask, int mask_kind, float* out, void* stream);
+int tfrs_mean_pool_bwd(const float* g, int64_t B, int64_t T, int64_t d, const void* mask, int mask_kind, float* dx,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

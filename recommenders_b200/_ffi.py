@@ -17,6 +17,7 @@ LIB_PATH = os.environ.get("TFRS_B200_LIB", os.path.join(_HERE, "libtfrs_b200.so"
 _lib: Optional[ctypes.CDLL] = None
 
 I32, I64, BYTES = 0, 1, 2
+F32, F64, BOOL = 3, 4, 5
 c_p = ctypes.c_void_p
 c_i = ctypes.c_int
 c_l = ctypes.c_int64
@@ -144,6 +145,15 @@ _SIGNATURES = {
     "tfrs_lookup_build": (c_i, [c_p, c_p, c_p]),
     "tfrs_lookup": (c_i, [c_p, c_p, c_p, c_i, c_l, c_l, c_l, c_p, c_p, c_p]),
     "tfrs_lookup_invert": (c_i, [c_p, c_i, c_l, c_p, c_l, c_l, c_i, c_l, c_l, c_p, c_p]),
+    "tfrs_text_standardize": (c_i, [c_p, c_p, c_l, c_l, c_i, c_p, c_p, c_p, c_p]),
+    "tfrs_text_lookup": (c_i, [c_p, c_p, c_p, c_l, c_l, c_l, c_l, c_p, c_p]),
+    "tfrs_text_spans": (c_i, [c_p, c_p, c_l, c_p, c_p, c_p]),
+    "tfrs_bucketize": (c_i, [c_p, c_i, c_l, c_p, c_l, c_p, c_p]),
+    "tfrs_normalize": (c_i, [c_p, c_i, c_l, c_l, c_p, c_p, c_i, c_p, c_p]),
+    "tfrs_normalization_adapt_workspace_bytes": (c_sz, [c_l, c_l, c_l]),
+    "tfrs_normalization_adapt": (c_i, [c_p, c_i, c_l, c_l, c_l, c_l, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_mean_pool_fwd": (c_i, [c_p, c_l, c_l, c_l, c_l, c_l, c_l, c_p, c_i, c_p, c_p]),
+    "tfrs_mean_pool_bwd": (c_i, [c_p, c_l, c_l, c_l, c_p, c_i, c_p, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

@@ -12,8 +12,9 @@
 //   tfrs_lookup         one thread per value, one launch: the mask test, then the probe (strings: fingerprint, then length,
 //                       then bytes).  One int64 store per value; no atomics.  With a miss flag, a miss sets it.
 //   tfrs_lookup_invert  one thread per index: a gather from the vocabulary, or a position code for strings.
-#include "common.cuh"
-#include "siphash.cuh"
+//
+// The table view and the string probe live in lookup.cuh, so that K16 (text.cu) probes the same tables the same way.
+#include "lookup.cuh"
 
 namespace tfrs {
 
@@ -29,32 +30,9 @@ __host__ __device__ __forceinline__ uint64_t lk_mix64(uint64_t z) {   // splitmi
   return z ^ (z >> 31);
 }
 
-__device__ __forceinline__ bool lk_bytes_equal(const uint8_t* a, const uint8_t* b, long long n) {
-  for (long long k = 0; k < n; ++k)
-    if (a[k] != b[k]) return false;
-  return true;
-}
-
 __device__ __forceinline__ uint64_t lk_fingerprint(const uint8_t* b, long long len) {
-  const uint8_t* p = nullptr;
-  Msg m;
-  bytes_msg(m, b, len, &p);
-  return siphash(m, p, LK_K0, LK_K1);
+  return lk_fingerprint(b, len, LK_K0, LK_K1);
 }
-
-struct LkTable {
-  int* slots;
-  unsigned long long cmask;             // cap - 1
-  const long long* keys;                // I64 keys [V]
-  const uint8_t* bytes;                 // BYTES keys
-  const long long* offsets;             // BYTES offsets [V + 1]
-  unsigned long long* fp;               // BYTES fingerprints [V]
-  long long V;
-  int has_mask;
-  long long mask;                       // I64 mask value
-  const uint8_t* mask_bytes;            // BYTES mask token
-  long long mask_len;
-};
 
 // ---- build ----------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(LK_THREADS) lk_build_i64_kernel(const LkTable t, int* __restrict__ dup) {
@@ -131,20 +109,9 @@ lk_lookup_bytes_kernel(const LkTable t, const uint8_t* __restrict__ data, const 
   const uint8_t* b = data + o0;
   long long r = 0;
   if (!(t.has_mask && len == t.mask_len && lk_bytes_equal(b, t.mask_bytes, len))) {
-    const unsigned long long h = lk_fingerprint(b, len);
-    unsigned long long s = h & t.cmask;
-    for (;;) {
-      const int p = __ldg(t.slots + s);
-      if (p < 0) {
-        if (miss) { *miss = 1; r = -1; } else { r = oov; }
-        break;
-      }
-      if (__ldg(t.fp + p) == h) {
-        const long long c0 = __ldg(t.offsets + p);
-        if (__ldg(t.offsets + p + 1) - c0 == len && lk_bytes_equal(t.bytes + c0, b, len)) { r = base + p; break; }
-      }
-      s = (s + 1) & t.cmask;
-    }
+    lk_probe_bytes(t, b, len, LK_K0, LK_K1, [&](int p) { r = base + p; }, [&] {
+      if (miss) { *miss = 1; r = -1; } else { r = oov; }
+    });
   }
   out[i] = r;
 }
@@ -171,7 +138,9 @@ static int64_t lk_slots(int64_t V) {
 
 static size_t lk_slot_bytes(int64_t V) { return align_up((size_t)lk_slots(V) * 4, 256); }
 
-static int lk_table(const tfrs_lookup_table* d, LkTable* t, const char* what) {
+const uint64_t lk_string_key[2] = {LK_K0, LK_K1};
+
+int lk_table(const tfrs_lookup_table* d, LkTable* t, const char* what) {
   TFRS_CHECK_ARG(d, "%s: NULL table", what);
   TFRS_CHECK_ARG(d->V >= 0 && d->V <= LK_MAX_V, "%s: V = %lld, must be in [0, 2^30)", what, (long long)d->V);
   TFRS_CHECK_ARG(d->kind == TFRS_I64 || d->kind == TFRS_BYTES, "%s: table kind must be I64 or BYTES", what);

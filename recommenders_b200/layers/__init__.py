@@ -4,6 +4,8 @@ from . import embedding
 from . import factorized_top_k
 from . import feature_interaction
 from . import loss
+from . import pooling
 from . import preprocessing
 from .feature_interaction import dcn
-from .preprocessing import IntegerLookup, StringLookup
+from .pooling import GlobalAveragePooling1D
+from .preprocessing import Discretization, IntegerLookup, Normalization, StringLookup, TextVectorization

@@ -28,9 +28,12 @@ class _GatherFn(torch.autograd.Function):
 
 
 class Embedding(torch.nn.Module):
-  """`tf.keras.layers.Embedding(input_dim, output_dim)`; default init uniform(-0.05, 0.05) like Keras."""
+  """`tf.keras.layers.Embedding(input_dim, output_dim, mask_zero=False)`; default init uniform(-0.05, 0.05) like Keras.
 
-  def __init__(self, input_dim: int, output_dim: int, device=None, embeddings_initializer="uniform"):
+  With mask_zero=True, `compute_mask(ids)` is `ids != 0`, and the output carries its mask for a following
+  GlobalAveragePooling1D (`ops.attached_mask`; honoured only for that very tensor, unmodified: `_version` + `data_ptr`)."""
+
+  def __init__(self, input_dim: int, output_dim: int, device=None, embeddings_initializer="uniform", mask_zero=False):
     super().__init__()
     device = device or torch.device("cuda", torch.cuda.current_device())
     w = torch.empty((input_dim, output_dim), dtype=torch.float32, device=device)
@@ -47,6 +50,12 @@ class Embedding(torch.nn.Module):
     self._sparse_grads: List[Tuple[torch.Tensor, torch.Tensor]] = []
     self._anchor = torch.nn.Parameter(torch.zeros((), device=device))  # keeps the autograd edge alive
     self.input_dim, self.output_dim = input_dim, output_dim
+    self.mask_zero = bool(mask_zero)
+
+  def compute_mask(self, ids, mask=None):
+    if not self.mask_zero:
+      return None
+    return ids != 0
 
   def forward(self, ids: torch.Tensor) -> torch.Tensor:
     if ids.dtype.is_floating_point:  # README feeds float ids from tf.strings.to_number (README.md:50-53)
@@ -57,7 +66,10 @@ class Embedding(torch.nn.Module):
       out = _GatherFn.apply(self._anchor, self, flat)
     else:
       out = ops.gather([self.weight], [flat])
-    return out.reshape(*shape, self.output_dim)
+    out = out.reshape(*shape, self.output_dim)
+    if self.mask_zero:
+      out._tfrs_mask = (ids, out._version, out.data_ptr())     # the ids themselves: nonzero = kept
+    return out
 
   def pop_sparse_grads(self):
     g, self._sparse_grads = self._sparse_grads, []

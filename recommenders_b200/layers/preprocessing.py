@@ -8,6 +8,10 @@ vocabulary[i] to m + o + i; `vocabulary_size()` is m + o + V.  The lookup runs o
 
 Deviations: an entry of the vocabulary equal to the mask or OOV token raises ValueError (tf-keras accepts those tokens at
 the head of the list and strips them), and strings lose trailing NUL bytes (NumPy's fixed-width string types drop them).
+
+The text and numeric feature layers of the reference's featurization / context_features / deep_recommenders towers
+follow: `TextVectorization` (K16, on the table of an inner StringLookup), `Discretization` and `Normalization` (K17);
+DESIGN.md §2, A21.
 """
 from __future__ import annotations
 
@@ -373,3 +377,322 @@ class StringLookup(_IndexLookup):
 
   def get_config(self) -> Dict[str, Any]:
     return {**super().get_config(), "encoding": self.encoding}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Text and numeric feature columns (DESIGN.md §2, A21): TextVectorization (K16), Discretization and Normalization (K17)
+# ---------------------------------------------------------------------------------------------------------------------
+_STANDARDIZE = {None: 0, "lower": ops.TEXT_LOWER, "strip_punctuation": ops.TEXT_STRIP,
+                "lower_and_strip_punctuation": ops.TEXT_LOWER | ops.TEXT_STRIP}
+_TEXT_OUTPUT_MODES = ("multi_hot", "count", "tf_idf")
+
+
+class TextVectorization(torch.nn.Module):
+  """`tf.keras.layers.TextVectorization` with output_mode="int" and split="whitespace": strings -> int64 [B, T] token
+  indices.  Inputs are NumPy str / bytes / object arrays or lists of shape [B] or [B, 1], packed on the host and copied
+  to the device once per call.  The output is an int64 CUDA tensor padded with 0; T is `output_sequence_length` when it
+  is given (longer token lists are truncated), else the longest token count of the batch (one 4-byte host read).
+
+  Standardize lowercases ASCII and deletes the 32 ASCII punctuation bytes; the split is on runs of " \\t\\n\\v\\f\\r".
+  Index 0 is padding, 1 is OOV, vocabulary entry i is 2 + i.  As in Keras, the vocabulary lives in an inner
+  `StringLookup(mask_token="", oov_token="[UNK]")`, whose K15 table the K16 kernels probe: two launches per call."""
+
+  def __init__(self, max_tokens=None, standardize="lower_and_strip_punctuation", split="whitespace", ngrams=None,
+               output_mode="int", output_sequence_length=None, pad_to_max_tokens=False, vocabulary=None,
+               idf_weights=None, sparse=False, ragged=False, encoding="utf-8", name=None):
+    super().__init__()
+    if callable(standardize):
+      raise NotImplementedError("a callable standardize is not supported")
+    if standardize not in _STANDARDIZE:
+      raise ValueError(f"Unknown standardize {standardize!r}; expected one of {tuple(_STANDARDIZE)} or a callable")
+    if split is None or split == "character" or callable(split):
+      raise NotImplementedError(f"split={split!r} is not supported; only 'whitespace' is")
+    if split != "whitespace":
+      raise ValueError(f"Unknown split {split!r}; expected 'whitespace', 'character', None or a callable")
+    if ngrams is not None:
+      raise NotImplementedError("ngrams are not supported")
+    if output_mode != "int":
+      if output_mode in _TEXT_OUTPUT_MODES:
+        raise NotImplementedError(f"output_mode={output_mode!r} is not supported; only 'int' is")
+      raise ValueError(f"Unknown output_mode {output_mode!r}; expected one of {('int',) + _TEXT_OUTPUT_MODES}")
+    if output_sequence_length is not None and (isinstance(output_sequence_length, bool) or
+                                               not isinstance(output_sequence_length, (int, np.integer)) or
+                                               output_sequence_length < 1):
+      raise ValueError(f"output_sequence_length must be a positive int or None, got {output_sequence_length!r}")
+    if ragged:
+      raise NotImplementedError("ragged=True is not supported")
+    if max_tokens is not None and max_tokens < 1:
+      raise ValueError(f"max_tokens must be > 1, got {max_tokens}")
+    self.standardize, self.split, self.ngrams, self.output_mode = standardize, split, ngrams, output_mode
+    self.output_sequence_length = None if output_sequence_length is None else int(output_sequence_length)
+    self.ragged, self.name = ragged, name
+    self._lookup_layer = StringLookup(max_tokens=max_tokens, num_oov_indices=1, mask_token="", oov_token="[UNK]",
+                                      vocabulary=vocabulary, idf_weights=idf_weights, encoding=encoding,
+                                      output_mode="int", sparse=sparse, pad_to_max_tokens=pad_to_max_tokens)
+
+  @property
+  def _flags(self) -> int:
+    return _STANDARDIZE[self.standardize]
+
+  # -- vocabulary: the inner StringLookup's ---------------------------------------------------------------------------
+  def get_vocabulary(self, include_special_tokens: bool = True) -> List[Any]:
+    return self._lookup_layer.get_vocabulary(include_special_tokens)
+
+  def vocabulary_size(self) -> int:
+    return self._lookup_layer.vocabulary_size()
+
+  def set_vocabulary(self, vocabulary, idf_weights=None) -> None:
+    self._lookup_layer.set_vocabulary(vocabulary, idf_weights)
+
+  def adapt(self, data, batch_size=None, steps=None) -> None:
+    """The vocabulary from `data` (an array, a list, or a `data.Dataset` of strings or batches of strings): every token
+    the call would produce, by count descending, ties by token descending bytewise (tf-keras's
+    `np.lexsort((tokens, counts))[::-1]`), cut to max_tokens - 2.  The tokens come from the device kernels of a call;
+    counting and ordering run on the host."""
+    counts: Dict[bytes, int] = {}
+    for el in (data if isinstance(data, Dataset) else [data]):
+      flat = self._batch(el, adapt=True)
+      if flat.size == 0:
+        continue
+      data_h, offsets, _ = pack_strings(flat)
+      byts, offs = upload_packed(data_h, offsets, _device())
+      buf, spans = ops.text_tokens(byts, offs, self._flags)
+      buf = buf.tobytes()
+      for s, n in spans.tolist():
+        tok = buf[s:s + n]
+        counts[tok] = counts.get(tok, 0) + 1
+    vocab = sorted(counts, key=lambda t: (counts[t], t), reverse=True)
+    max_tokens = self._lookup_layer.max_tokens
+    if max_tokens is not None:
+      vocab = vocab[:max(max_tokens - 2, 0)]
+    try:
+      words = np.asarray([t.decode("utf-8") for t in vocab], dtype=object)
+    except UnicodeDecodeError:
+      words = np.asarray(vocab, dtype=object)
+    self._lookup_layer.set_vocabulary(words if len(vocab) else np.zeros((0,), "U1"))
+
+  # -- calls -----------------------------------------------------------------------------------------------------------
+  @staticmethod
+  def _batch(inputs, adapt=False) -> np.ndarray:
+    if isinstance(inputs, torch.Tensor):
+      raise TypeError("TextVectorization takes NumPy string arrays or lists of strings, got a tensor")
+    if isinstance(inputs, (str, bytes)):
+      inputs = [inputs]
+    a = StringLookup._strings(inputs)
+    if adapt and a.ndim == 0:
+      return a.reshape(1)
+    if a.ndim == 2 and a.shape[1] == 1:
+      return a.reshape(-1)
+    if a.ndim != 1:
+      raise ValueError(f"TextVectorization takes inputs of shape [B] or [B, 1], got {a.shape}")
+    return a
+
+  def forward(self, inputs) -> torch.Tensor:
+    if isinstance(inputs, tuple) and len(inputs) == 2:
+      raise NotImplementedError("ragged (values, row_splits) inputs are not supported")
+    flat = self._batch(inputs)
+    dev = _device()
+    T = self.output_sequence_length
+    if flat.size == 0:
+      return torch.zeros((0, T or 0), dtype=torch.int64, device=dev)
+    data, offsets, _ = pack_strings(flat)
+    table = self._lookup_layer._table_on(dev)
+    byts, offs = upload_packed(data, offsets, dev)
+    lk = self._lookup_layer
+    return ops.text_vectorize(table, byts, offs, self._flags, T, lk._base(), lk._m)
+
+  # -- checkpointing and config ---------------------------------------------------------------------------------------
+  def get_config(self) -> Dict[str, Any]:
+    lk = self._lookup_layer
+    return {"name": self.name, "max_tokens": lk.max_tokens, "standardize": self.standardize, "split": self.split,
+            "ngrams": self.ngrams, "output_mode": self.output_mode,
+            "output_sequence_length": self.output_sequence_length, "pad_to_max_tokens": False,
+            "vocabulary": lk.get_vocabulary(include_special_tokens=False), "idf_weights": None, "sparse": False,
+            "ragged": self.ragged, "encoding": lk.encoding}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)
+
+
+_DISCRETIZATION_OUTPUT_MODES = ("one_hot", "multi_hot", "count")
+
+
+def _numeric_input(inputs, what: str) -> torch.Tensor:
+  """A CUDA int32 / int64 / float32 / float64 tensor, or NumPy numbers uploaded once (other int / float widths widened)."""
+  if isinstance(inputs, torch.Tensor):
+    ops.require_cuda(inputs, "inputs")
+    return inputs
+  a = np.asarray(inputs)
+  if a.dtype.kind in "iub":
+    a = a if a.dtype in (np.int32, np.int64) else a.astype(np.int64)
+  elif a.dtype.kind == "f":
+    a = a if a.dtype in (np.float32, np.float64) else a.astype(np.float32)
+  else:
+    raise TypeError(f"{what} takes numbers, got dtype {a.dtype}")
+  return torch.from_numpy(np.ascontiguousarray(a)).to(_device())
+
+
+class Discretization(torch.nn.Module):
+  """`tf.keras.layers.Discretization(bin_boundaries)` with output_mode="int": each value -> the int64 index of its bucket,
+  #{i : b_i <= x} over the boundaries rounded once to float32 (TF's Bucketize on the CPU).  Integers are compared after
+  rounding to float32, float64 values as doubles; NaN falls in the last bucket.  Inputs are CUDA or NumPy int32 / int64
+  / float32 / float64 of any shape; one K17 launch per call.  `num_bins`, `epsilon` and `adapt` (Keras's approximate
+  quantiles) are not offered."""
+
+  def __init__(self, bin_boundaries=None, num_bins=None, epsilon=0.01, output_mode="int", sparse=False, name=None):
+    super().__init__()
+    if num_bins is not None:
+      if bin_boundaries is not None:
+        raise ValueError("Both `num_bins` and `bin_boundaries` should not be set.")
+      raise NotImplementedError("num_bins (bucket boundaries from adapt) is not supported; pass bin_boundaries")
+    if epsilon != 0.01:
+      raise NotImplementedError("epsilon only applies to adapt, which is not supported")
+    if output_mode != "int":
+      if output_mode in _DISCRETIZATION_OUTPUT_MODES:
+        raise NotImplementedError(f"output_mode={output_mode!r} is not supported; only 'int' is")
+      raise ValueError(f"Unknown output_mode {output_mode!r}; expected one of {('int',) + _DISCRETIZATION_OUTPUT_MODES}")
+    if sparse:
+      raise NotImplementedError("sparse=True is not supported")
+    if bin_boundaries is None:
+      raise NotImplementedError("Discretization without bin_boundaries needs adapt, which is not supported")
+    b = np.asarray(bin_boundaries, dtype=np.float64)
+    if b.ndim != 1:
+      raise ValueError(f"bin_boundaries must be a 1-D list, got shape {b.shape}")
+    b32 = b.astype(np.float32)
+    if np.isnan(b32).any() or (b32[1:] < b32[:-1]).any():
+      raise ValueError("bin_boundaries must be sorted (after rounding to float32) and not NaN")
+    self.bin_boundaries = b.tolist()
+    self._b32 = b32
+    self._bounds: Dict[torch.device, torch.Tensor] = {}
+    self.output_mode, self.name = output_mode, name
+
+  def adapt(self, data, batch_size=None, steps=None) -> None:
+    raise NotImplementedError("Discretization.adapt (approximate quantiles) is not supported; pass bin_boundaries")
+
+  def forward(self, inputs) -> torch.Tensor:
+    x = _numeric_input(inputs, "Discretization")
+    b = self._bounds.get(x.device)
+    if b is None:
+      b = self._bounds[x.device] = torch.from_numpy(self._b32).to(x.device)
+    return ops.bucketize(x, b)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "bin_boundaries": list(self.bin_boundaries), "num_bins": None, "epsilon": 0.01,
+            "output_mode": self.output_mode, "sparse": False}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)
+
+
+class Normalization(torch.nn.Module):
+  """`tf.keras.layers.Normalization(axis, mean, variance, invert)`: (f32(x) - mean) / max(sqrt(var), 1e-7) as float32, or
+  mean + f32(x) * max(sqrt(var), 1e-7) with invert=True.  `axis` is None (one mean and variance) or -1 (one per index
+  of the last axis).  The statistics come from `mean` / `variance`, or from `adapt`, which merges batches as Keras's
+  update_state does, on the device (K17).  Inputs are CUDA or NumPy int32 / int64 / float32 / float64; the layer
+  preprocesses data, so an input that requires grad raises NotImplementedError."""
+
+  def __init__(self, axis=-1, mean=None, variance=None, invert=False, name=None):
+    super().__init__()
+    if isinstance(axis, (list, tuple)) and len(axis) == 1:
+      axis = axis[0]
+    if axis is not None and axis != -1:
+      raise NotImplementedError(f"axis={axis!r} is not supported; only None and -1 (the last axis) are")
+    if (mean is None) != (variance is None):
+      raise ValueError("When setting values directly, both `mean` and `variance` must be set. "
+                       f"Got mean: {mean} and variance: {variance}")
+    self.axis, self.invert, self.name = axis, bool(invert), name
+    self.input_mean = None if mean is None else np.asarray(mean, np.float32)
+    self.input_variance = None if variance is None else np.asarray(variance, np.float32)
+    if axis is None and mean is not None and (self.input_mean.size != 1 or self.input_variance.size != 1):
+      raise ValueError("With axis=None, mean and variance must be scalars")
+    self._state: Optional[torch.Tensor] = None       # float32 [2, C] on the device: mean, variance
+    self._count: Optional[torch.Tensor] = None       # int64 [1]: the values adapt has seen per channel
+
+  def _channels(self, shape) -> int:
+    if self.axis is None:
+      return 1
+    if len(shape) < 2:
+      raise NotImplementedError(f"axis=-1 takes inputs of rank >= 2 (one statistic per last index), got shape "
+                                f"{tuple(shape)}; reshape to [N, 1] or use axis=None")
+    return int(shape[-1])
+
+  def _reset(self, C: int, device) -> None:
+    self._state = torch.tensor([[0.0] * C, [1.0] * C], dtype=torch.float32, device=device)
+    self._count = torch.zeros((1,), dtype=torch.int64, device=device)
+
+  def adapt(self, data, batch_size=None, steps=None) -> None:
+    """Mean and variance from `data`: an array or a tensor, cut into batches of `batch_size` rows (32 by default, as in
+    Keras), or a `data.Dataset` whose elements are the batches.  The host reads nothing."""
+    if self.input_mean is not None:
+      raise ValueError("Cannot adapt a Normalization layer that was given mean and variance")
+    if isinstance(data, Dataset):
+      rows, parts = None, list(data)
+    else:
+      rows, parts = int(batch_size or 32), [data]
+    self._state = None
+    for el in parts:
+      C = self._channels(tuple(el.shape) if isinstance(el, torch.Tensor) else np.shape(el) or (1,))
+      x = _numeric_input(el, "Normalization.adapt")
+      if x.dim() == 0:
+        x = x.reshape(1)
+      if self._state is None:
+        self._reset(C, x.device)
+      elif self._state.shape[1] != C:
+        raise ValueError(f"Normalization.adapt: a batch with {C} channels after one with {self._state.shape[1]}")
+      ops.normalization_adapt(x, C, rows if rows is not None else max(x.shape[0], 1), self._state, self._count)
+
+  @property
+  def mean(self) -> Optional[torch.Tensor]:
+    return None if self._state is None else self._state[0]
+
+  @property
+  def variance(self) -> Optional[torch.Tensor]:
+    return None if self._state is None else self._state[1]
+
+  def _statistics(self, shape, device):
+    C = self._channels(shape)
+    if self.input_mean is not None:
+      try:
+        m = np.broadcast_to(self.input_mean.reshape(-1) if self.input_mean.size > 1 else self.input_mean.reshape(()), (C,))
+        v = np.broadcast_to(self.input_variance.reshape(-1) if self.input_variance.size > 1 else
+                            self.input_variance.reshape(()), (C,))
+      except ValueError:
+        raise ValueError(f"mean / variance of shape {self.input_mean.shape} do not broadcast to {C} channels") from None
+      if self._state is None or self._state.device != device or self._state.shape[1] != C:
+        self._state = torch.from_numpy(np.stack([m, v]).astype(np.float32)).to(device)
+    elif self._state is None:
+      self._reset(C, device)
+    elif self._state.shape[1] != C:
+      raise ValueError(f"Normalization was adapted on {self._state.shape[1]} channels, the input has {C}")
+    elif self._state.device != device:
+      self._state, self._count = self._state.to(device), self._count.to(device)
+    return self._state[0], self._state[1]
+
+  def forward(self, inputs) -> torch.Tensor:
+    if isinstance(inputs, torch.Tensor) and inputs.requires_grad:
+      raise NotImplementedError("Normalization preprocesses data; an input that requires grad is not supported")
+    x = _numeric_input(inputs, "Normalization")
+    mean, var = self._statistics(x.shape, x.device)
+    return ops.normalize(x, mean, var, self.invert)
+
+  # -- checkpointing and config ---------------------------------------------------------------------------------------
+  def get_extra_state(self):
+    if self._state is None or self.input_mean is not None:
+      return {}
+    return {"state": self._state.cpu(), "count": self._count.cpu()}
+
+  def set_extra_state(self, state):
+    if state:
+      dev = _device()
+      self._state, self._count = state["state"].to(dev), state["count"].to(dev)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "axis": self.axis, "invert": self.invert,
+            "mean": None if self.input_mean is None else self.input_mean.tolist(),
+            "variance": None if self.input_variance is None else self.input_variance.tolist()}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)

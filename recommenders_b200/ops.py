@@ -1883,3 +1883,160 @@ def lookup_invert(idx: torch.Tensor, size: int, base: int, keys: Optional[torch.
 
 def launch_count() -> int:
   return int(lib().tfrs_launch_count())
+
+
+# ------------------------------------------------------------------------------------------------
+# K16 text vectorization: layers.TextVectorization on the K15 table of its inner StringLookup
+# ------------------------------------------------------------------------------------------------
+TEXT_LOWER, TEXT_STRIP = 1, 2
+
+
+def _text_standardize(data: torch.Tensor, offsets: torch.Tensor, flags: int, with_max: bool):
+  n = offsets.numel() - 1
+  scratch = torch.empty_like(data)
+  counts = torch.empty((n,), dtype=torch.int32, device=offsets.device)
+  mx = torch.empty((1,), dtype=torch.int32, device=offsets.device) if with_max else None
+  check(lib().tfrs_text_standardize(ptr(data), ptr(offsets), n, data.numel(), int(flags), ptr(scratch), ptr(counts),
+                                    ptr(mx), stream()), "text_standardize")
+  return scratch, counts, mx
+
+
+def text_vectorize(table: LookupTable, data: torch.Tensor, offsets: torch.Tensor, flags: int, T: Optional[int], base: int,
+                   oov: int) -> torch.Tensor:
+  """int64 [n, T]: the tokens of n strings (uint8 `data`, int64 `offsets` [n+1] on the device), standardized by `flags`
+  (TEXT_LOWER | TEXT_STRIP) and split on ASCII whitespace, each looked up in the string table: base + p for vocabulary
+  entry p, `oov` for any other token, 0 after a string's last token.  T=None takes the longest token count, at the cost
+  of one 4-byte host read; with T given, the call never reads device memory on the host.  Two launches."""
+  if table.offsets is None:
+    raise TypeError("text_vectorize: the table must be a string table")
+  scratch, _, mx = _text_standardize(data, offsets, flags, T is None)
+  if T is None:
+    T = int(mx.item())
+  out = torch.empty((offsets.numel() - 1, T), dtype=torch.int64, device=offsets.device)
+  desc = table.desc()
+  check(lib().tfrs_text_lookup(ctypes.byref(desc), ptr(scratch), ptr(offsets), out.shape[0], T, int(base), int(oov),
+                               ptr(out), stream()), "text_lookup")
+  return out
+
+
+def text_tokens(data: torch.Tensor, offsets: torch.Tensor, flags: int) -> Tuple[np.ndarray, np.ndarray]:
+  """The tokens of n strings as text_vectorize finds them, for adapt: (standardized bytes, int64 [tokens, 2] of (offset,
+  length) into them, string by string), both read back to the host."""
+  scratch, counts, _ = _text_standardize(data, offsets, flags, False)
+  tok_off = np.zeros(counts.numel() + 1, np.int64)
+  np.cumsum(counts.cpu().numpy(), out=tok_off[1:])
+  spans = torch.empty((int(tok_off[-1]), 2), dtype=torch.int64, device=offsets.device)
+  tok_off_d = torch.from_numpy(tok_off).to(offsets.device)
+  check(lib().tfrs_text_spans(ptr(scratch), ptr(offsets), counts.numel(), ptr(tok_off_d), ptr(spans), stream()),
+        "text_spans")
+  return scratch.cpu().numpy(), spans.cpu().numpy()
+
+
+# ------------------------------------------------------------------------------------------------
+# K17 numeric columns and pooling: layers.Discretization, layers.Normalization, layers.GlobalAveragePooling1D
+# ------------------------------------------------------------------------------------------------
+_VALUE_KINDS = {torch.int32: _ffi.I32, torch.int64: _ffi.I64, torch.float32: _ffi.F32, torch.float64: _ffi.F64}
+_MASK_KINDS = {torch.int32: _ffi.I32, torch.int64: _ffi.I64, torch.bool: _ffi.BOOL}
+
+
+def _numeric(x: torch.Tensor, what: str) -> Tuple[torch.Tensor, int]:
+  require_cuda(x, what)
+  if x.dtype not in _VALUE_KINDS:
+    raise TypeError(f"{what}: values must be int32, int64, float32 or float64, got {x.dtype}")
+  return x.contiguous(), _VALUE_KINDS[x.dtype]
+
+
+def bucketize(x: torch.Tensor, boundaries: torch.Tensor) -> torch.Tensor:
+  """int64 [x's shape]: the number of float32 `boundaries` (sorted, CUDA) at or below each value; NaN gives their count.
+  Integers are rounded to float32 first; float64 values are compared as doubles.  One launch."""
+  x, kind = _numeric(x, "bucketize")
+  require_cuda(boundaries, "boundaries")
+  if boundaries.dtype != torch.float32 or boundaries.dim() != 1:
+    raise TypeError("bucketize: boundaries must be a 1-D float32 tensor")
+  b = boundaries.contiguous()
+  out = torch.empty(x.shape, dtype=torch.int64, device=x.device)
+  check(lib().tfrs_bucketize(ptr(x), kind, x.numel(), ptr(b), b.numel(), ptr(out), stream()), "bucketize")
+  return out
+
+
+def normalize(x: torch.Tensor, mean: torch.Tensor, var: torch.Tensor, invert: bool = False) -> torch.Tensor:
+  """float32 [x's shape]: (f32(x) - mean) / max(sqrt(var), 1e-7), or mean + f32(x) * max(sqrt(var), 1e-7) with invert;
+  `mean` and `var` are float32 [C] (CUDA), C = 1 or x's last dimension.  One launch."""
+  x, kind = _numeric(x, "normalize")
+  C = mean.numel()
+  if mean.dtype != torch.float32 or var.dtype != torch.float32 or var.numel() != C or C < 1:
+    raise TypeError("normalize: mean and variance must be float32 tensors of one size C >= 1")
+  if C > 1 and (x.dim() == 0 or x.shape[-1] != C):
+    raise ValueError(f"normalize: {C} statistics for an input of shape {tuple(x.shape)}")
+  out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+  check(lib().tfrs_normalize(ptr(x), kind, x.numel(), C, ptr(mean.contiguous()), ptr(var.contiguous()), int(bool(invert)),
+                             ptr(out), stream()), "normalize")
+  return out
+
+
+def normalization_adapt(x: torch.Tensor, C: int, batch_rows: int, state: torch.Tensor, count: torch.Tensor) -> None:
+  """Merges the batches of `batch_rows` rows of x (axis 0; channel = last index mod C) into `state` (float32 [2, C]: mean,
+  variance) and `count` (int64 [1]) in place, as Keras's Normalization.adapt does.  One launch for a single batch, two
+  otherwise; nothing is read on the host."""
+  x, kind = _numeric(x, "normalization_adapt")
+  if state.dtype != torch.float32 or state.shape != (2, C) or count.dtype != torch.int64 or count.numel() != 1:
+    raise TypeError("normalization_adapt: state must be float32 [2, C] and count int64 [1]")
+  N = x.shape[0] if x.dim() else 1
+  R = x.numel() // N if N else 1
+  nb = lib().tfrs_normalization_adapt_workspace_bytes(N, C, batch_rows)
+  ws = workspace(nb, x.device, "normalization_adapt") if nb else None
+  check(lib().tfrs_normalization_adapt(ptr(x), kind, N, R, C, batch_rows, ptr(state), ptr(count), ptr(ws), nb, stream()),
+        "normalization_adapt")
+
+
+def _mask_arg(mask: Optional[torch.Tensor], B: int, T: int):
+  if mask is None:
+    return None, 0
+  require_cuda(mask, "mask")
+  if mask.dtype not in _MASK_KINDS:
+    raise TypeError(f"mean_pool: the mask must be bool, int32 or int64, got {mask.dtype}")
+  if tuple(mask.shape) != (B, T):
+    raise ValueError(f"mean_pool: the mask has shape {tuple(mask.shape)}, the input [{B}, {T}, d]")
+  return mask.contiguous(), _MASK_KINDS[mask.dtype]
+
+
+class _MeanPool(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, x, mask):
+    B, T, d = x.shape
+    m, mk = _mask_arg(mask, B, T)
+    out = torch.empty((B, d), dtype=torch.float32, device=x.device)
+    check(lib().tfrs_mean_pool_fwd(ptr(x), B, T, d, x.stride(0), x.stride(1), x.stride(2), ptr(m), mk, ptr(out),
+                                   stream()), "mean_pool_fwd")
+    ctx.save_for_backward(m)
+    ctx.shape, ctx.mk = (B, T, d), mk
+    return out
+
+  @staticmethod
+  def backward(ctx, g):
+    (m,) = ctx.saved_tensors
+    B, T, d = ctx.shape
+    g = g.to(torch.float32).contiguous()
+    dx = torch.empty((B, T, d), dtype=torch.float32, device=g.device)
+    check(lib().tfrs_mean_pool_bwd(ptr(g), B, T, d, ptr(m), ctx.mk, ptr(dx), stream()), "mean_pool_bwd")
+    return dx, None
+
+
+def mean_pool(x: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+  """float32 [B, d]: the mean over t of x [B, T, d] (float32, any strides), counting only the positions where `mask` ([B,
+  T] bool / int32 / int64, CUDA) is nonzero; an all-masked row is 0/0.  Products and sums in float32, t ascending from
+  +0.0f.  Backward: dx = f32(g / count) * mask, or g / T.  One launch each way."""
+  require_cuda(x, "inputs")
+  if x.dtype != torch.float32 or x.dim() != 3:
+    raise TypeError(f"mean_pool: inputs must be float32 [B, T, d], got {x.dtype} {tuple(x.shape)}")
+  return _MeanPool.apply(x, mask)
+
+
+def attached_mask(x: torch.Tensor) -> Optional[torch.Tensor]:
+  """The mask (the ids, nonzero = kept) an Embedding with mask_zero=True attached to its output `x`, if `x` is that very
+  tensor, unmodified."""
+  hint = getattr(x, "_tfrs_mask", None)
+  if hint is not None and hint[1] == x._version and hint[2] == x.data_ptr() and tuple(hint[0].shape) == tuple(x.shape[:-1]):
+    return hint[0]
+  return None
