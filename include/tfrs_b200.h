@@ -578,7 +578,8 @@ int tfrs_listwise_bwd_f32(const float* dlds, int64_t B, int L, int reduction, fl
  * divided as in the forward (pooled; a value outside every bag gets zeros).  Only n, row_splits, n_bags, combiner and
  * n_chunks of the features and dim, ld, col_off, grad and grad_rows of the slots are read.  No float atomics.
  * Pooled features need n_bags >= 1 unless n == 0.  An empty call (n == 0 and no bags) may pass NULL outputs.
- * tfrs_hash_bins: bins[i] = bin(value i) for one stream and one salt (I32, I64, or BYTES with offsets [n+1]).
+ * tfrs_hash_bins: bins[i] = bin(value i) for one stream and one salt (I32, I64, or BYTES with offsets [n+1]); it is
+ * tfrs_hashing (K18, below) with that salt and no mask.
  * ------------------------------------------------------------------------------------------- */
 enum { TFRS_BYTES = 2 };
 enum { TFRS_COMBINER_SUM = 0, TFRS_COMBINER_MEAN = 1, TFRS_COMBINER_SQRTN = 2 };
@@ -825,6 +826,21 @@ int tfrs_mean_pool_fwd(const float* x, int64_t B, int64_t T, int64_t d, int64_t 
                        const void* mask, int mask_kind, float* out, void* stream);
 int tfrs_mean_pool_bwd(const float* g, int64_t B, int64_t T, int64_t d, const void* mask, int mask_kind, float* dx,
                        void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * K18 feature hashing: tf.keras.layers.Hashing(num_bins, mask_value, salt) as the reference's uet and featurization
+ * tutorials use it (`Sequential([Hashing(num_bins=buckets), Embedding(buckets, d)])`).
+ *   h = FarmHash Fingerprint64(message) when `salt` is NULL (tf.strings.to_hash_bucket_fast), else
+ *       SipHash-2-4(k0 = salt[0], k1 = salt[1], message) (to_hash_bucket_strong).  `salt` is a HOST array of two uint64.
+ *   message: the bytes of a TFRS_BYTES value (offsets [n+1]; strings may start at any byte); for TFRS_I32 / TFRS_I64
+ *       values the decimal text of tf.as_string.
+ *   bins[i] (int64) = h mod num_bins, unsigned.  With has_mask and num_bins > 1, bin 0 is reserved: 0 when value i
+ *       equals the mask (`mask` as int64 for integer values; the mask_len device bytes at mask_bytes for strings), else
+ *       1 + h mod (num_bins - 1).  With num_bins == 1 nothing is reserved.
+ * One launch; n == 0 writes nothing.
+ * ------------------------------------------------------------------------------------------- */
+int tfrs_hashing(const void* values, const int64_t* offsets, int kind, int64_t n, const uint64_t* salt, int64_t num_bins,
+                 int has_mask, int64_t mask, const uint8_t* mask_bytes, int64_t mask_len, int64_t* bins, void* stream);
 
 #ifdef __cplusplus
 }

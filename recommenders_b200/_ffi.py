@@ -154,6 +154,7 @@ _SIGNATURES = {
     "tfrs_normalization_adapt": (c_i, [c_p, c_i, c_l, c_l, c_l, c_l, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_mean_pool_fwd": (c_i, [c_p, c_l, c_l, c_l, c_l, c_l, c_l, c_p, c_i, c_p, c_p]),
     "tfrs_mean_pool_bwd": (c_i, [c_p, c_l, c_l, c_l, c_p, c_i, c_p, c_p]),
+    "tfrs_hashing": (c_i, [c_p, c_p, c_i, c_l, c_p, c_l, c_i, c_l, c_p, c_l, c_p, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

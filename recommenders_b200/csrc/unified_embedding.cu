@@ -12,8 +12,9 @@
 // (when the caller asks for them) into per-table buffers, which is all a pooled (ragged) slot does in this launch.
 // Pooled slots then take one more launch: a group of dim/4 lanes per (bag, slot) sums the bag's rows in value order.
 // Backward: one launch writes each table's gradient rows, contiguous, in the caller's order.  No float atomics.
+// Bucket ids alone (tfrs_hash_bins) come from K18's hash-only kernel (hashing.cu).
 #include "common.cuh"
-#include "siphash.cuh"
+#include "bucket.cuh"
 
 namespace tfrs {
 
@@ -47,41 +48,6 @@ struct UeParams {
   short y_feat[UE_MAX_SLOTS];
 };
 static_assert(sizeof(UeParams) <= 32000, "kernel parameters must stay under the 32 KB limit");
-
-// x mod d with magic = floor((2^64 - 1) / d), d >= 1: the estimate q = hi64(x * magic) is at most 2 below floor(x / d)
-// (DESIGN.md K8), so two conditional subtractions make the remainder exact for every d < 2^64.
-__device__ __forceinline__ uint64_t mod_magic(uint64_t x, uint64_t d, uint64_t magic) {
-  uint64_t r = x - __umul64hi(x, magic) * d;
-  if (r >= d) r -= d;
-  if (r >= d) r -= d;
-  return r;
-}
-
-// tf.as_string of an int64: digits generated least significant first and pushed at byte 0, so the most significant
-// digit ends at byte 0.  |x| is split into 32-bit pieces below 10^9.
-__device__ __forceinline__ Msg decimal_msg(long long x) {
-  Msg m;
-  const bool neg = x < 0;
-  const uint64_t u = neg ? 0ull - (uint64_t)x : (uint64_t)x;
-  const uint64_t q1 = u / 1000000000ull;
-  const uint64_t q2 = q1 / 1000000000ull;
-  const uint32_t piece[3] = {(uint32_t)(u - q1 * 1000000000ull), (uint32_t)(q1 - q2 * 1000000000ull), (uint32_t)q2};
-  const int top = q2 ? 2 : (q1 ? 1 : 0);
-#pragma unroll
-  for (int p = 0; p < 3; ++p) {
-    if (p > top) break;
-    uint32_t v = piece[p];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-      if (p == top && k > 0 && v == 0) break;    // the leading piece has no leading zeros
-      const uint32_t q = v / 10u;
-      m.push('0' + (v - q * 10u));
-      v = q;
-    }
-  }
-  if (neg) m.push('-');
-  return m;
-}
 
 // The message of value i of a feature (kind: TFRS_I32, TFRS_I64, TFRS_BYTES); *p is the start of a byte string.
 __device__ __forceinline__ Msg form_msg(const UeFeat& f, long long i, const uint8_t** p) {
@@ -313,27 +279,6 @@ static int ue_groups(const tfrs_ue_feature* features, int n_features, const tfrs
 
 }  // namespace tfrs
 using namespace tfrs;
-
-extern "C" int tfrs_hash_bins(const void* values, const int64_t* offsets, int kind, int64_t n, const uint64_t* salt,
-                              int64_t num_bins, int64_t* bins, void* stream) {
-  TFRS_CHECK_ARG(salt && bins && (n == 0 || values), "hash_bins: NULL argument");
-  TFRS_CHECK_ARG(kind == TFRS_I32 || kind == TFRS_I64 || (kind == TFRS_BYTES && offsets),
-                 "hash_bins: kind must be I32, I64 or BYTES (with offsets)");
-  TFRS_CHECK_ARG(n >= 0 && n < (1ll << 38) && num_bins >= 1, "hash_bins: bad n / num_bins");
-  if (n == 0) return TFRS_OK;
-  // the forward kernel on one feature with one chunk that only writes its bucket ids
-  UeParams p;
-  UeFeat& f = p.f[0];
-  f = UeFeat{};
-  f.values = values; f.offsets = offsets; f.n = n; f.n_chunks = 1; f.kind = kind; f.copy = 0;
-  UeSlot& s = p.s[0];
-  s = UeSlot{};
-  s.k0 = salt[0]; s.k1 = salt[1]; s.nbins = (unsigned long long)num_bins; s.magic = ~0ull / s.nbins;
-  s.ids = reinterpret_cast<long long*>(bins);
-  ue_lookup_fwd_kernel<<<dim3((unsigned)ceil_div(n, UE_THREADS), 1), UE_THREADS, 0, (cudaStream_t)stream>>>(p);
-  TFRS_LAUNCH_CHECK();
-  return TFRS_OK;
-}
 
 extern "C" int tfrs_unified_lookup_fwd_f32(const tfrs_ue_feature* features, int n_features, const tfrs_ue_slot* slots,
                                            int n_slots, void* stream) {

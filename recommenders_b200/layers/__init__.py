@@ -8,4 +8,4 @@ from . import pooling
 from . import preprocessing
 from .feature_interaction import dcn
 from .pooling import GlobalAveragePooling1D
-from .preprocessing import Discretization, IntegerLookup, Normalization, StringLookup, TextVectorization
+from .preprocessing import Discretization, Hashing, IntegerLookup, Normalization, StringLookup, TextVectorization

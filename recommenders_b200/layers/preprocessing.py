@@ -11,7 +11,7 @@ the head of the list and strips them), and strings lose trailing NUL bytes (NumP
 
 The text and numeric feature layers of the reference's featurization / context_features / deep_recommenders towers
 follow: `TextVectorization` (K16, on the table of an inner StringLookup), `Discretization` and `Normalization` (K17);
-DESIGN.md §2, A21.
+DESIGN.md §2, A21.  `Hashing` (K18; DESIGN.md §2, A22) is the vocabulary-free alternative to the lookups.
 """
 from __future__ import annotations
 
@@ -692,6 +692,106 @@ class Normalization(torch.nn.Module):
     return {"name": self.name, "axis": self.axis, "invert": self.invert,
             "mean": None if self.input_mean is None else self.input_mean.tolist(),
             "variance": None if self.input_variance is None else self.input_variance.tolist()}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Feature hashing (DESIGN.md §2, A22): Hashing (K18)
+# ---------------------------------------------------------------------------------------------------------------------
+_HASHING_OUTPUT_MODES = ("one_hot", "multi_hot", "count")
+
+
+def _is_int(x) -> bool:
+  return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+
+
+class Hashing(torch.nn.Module):
+  """`tf.keras.layers.Hashing(num_bins, mask_value, salt)` with output_mode="int": each value -> its int64 bin, as
+  tf-keras's `_hash_values_to_bins` computes it.  Without a salt the bin is FarmHash Fingerprint64 mod num_bins
+  (`tf.strings.to_hash_bucket_fast`); with one it is SipHash-2-4 keyed by the salt (`to_hash_bucket_strong`); an int
+  salt s is the key [s, s].  Integers are hashed as their decimal text (`tf.as_string`).  With a `mask_value` and
+  num_bins > 1, bin 0 is the mask's and every other value goes to 1 + h mod (num_bins - 1).
+
+  Inputs are CUDA int32 / int64 tensors of any shape (one K18 launch), NumPy or list ints (uploaded once), or NumPy str /
+  bytes / object arrays or lists of strings of any shape (`str` encoded as UTF-8, packed on the host and copied to the
+  device once, as StringLookup does; trailing NUL bytes are lost the same way).  The output is an int64 CUDA tensor of
+  the input's shape.  There is no CPU path: a CPU tensor raises TypeError."""
+
+  def __init__(self, num_bins, mask_value=None, salt=None, output_mode="int", sparse=False, name=None):
+    super().__init__()
+    if num_bins is None or not _is_int(num_bins) or num_bins <= 0:
+      raise ValueError(f"The `num_bins` for `Hashing` cannot be `None` or non-positive values. Received: "
+                       f"num_bins={num_bins!r}.")
+    if num_bins >= 2**63:
+      raise ValueError(f"num_bins must be below 2^63, got {num_bins}")
+    if output_mode != "int":
+      if output_mode in _HASHING_OUTPUT_MODES:
+        raise NotImplementedError(f"output_mode={output_mode!r} is not supported; only 'int' is")
+      raise ValueError(f"Unknown output_mode {output_mode!r}; expected one of {('int',) + _HASHING_OUTPUT_MODES}")
+    if sparse:
+      raise NotImplementedError("sparse=True is not supported")
+    if salt is not None:
+      if isinstance(salt, (tuple, list)) and len(salt) == 2 and all(_is_int(s) for s in salt):
+        salt = [int(s) for s in salt]
+      elif _is_int(salt):
+        salt = [int(salt), int(salt)]
+      else:
+        raise ValueError(f"The `salt` argument for `Hashing` can only be a tuple of size 2 integers, or a single "
+                         f"integer. Received: salt={salt!r}.")
+      if not all(-2**63 <= s < 2**64 for s in salt):
+        raise ValueError(f"salt values must fit in 64 bits, got {salt}")
+    if mask_value is not None and not (_is_int(mask_value) or isinstance(mask_value, (str, bytes))):
+      raise ValueError(f"mask_value must be an int, a str, bytes or None, got {mask_value!r}")
+    self.num_bins = int(num_bins)
+    self.mask_value = int(mask_value) if _is_int(mask_value) else mask_value
+    self.salt = salt
+    self.output_mode, self.sparse, self.name = output_mode, False, name
+
+  def _int_mask(self):
+    if self.mask_value is not None and not _is_int(self.mask_value):
+      raise TypeError(f"Hashing: the string mask_value {self.mask_value!r} cannot mask integer inputs")
+    return self.mask_value
+
+  def forward(self, inputs) -> torch.Tensor:
+    if isinstance(inputs, tuple) and len(inputs) == 2:
+      raise NotImplementedError("ragged (values, row_splits) inputs are not supported")
+    if isinstance(inputs, torch.Tensor):
+      if not inputs.is_cuda:
+        raise TypeError(f"Hashing takes CUDA tensors (there is no CPU path), got one on {inputs.device}")
+      if inputs.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"Hashing takes int32 / int64 tensors or strings, got {inputs.dtype}")
+      return ops.hashing(inputs, self.num_bins, self.salt, self._int_mask())
+    try:
+      a = np.asarray(inputs, dtype=object) if isinstance(inputs, (list, tuple)) else np.asarray(inputs)
+    except ValueError:
+      raise NotImplementedError("ragged inputs are not supported") from None
+    if a.dtype.kind == "O":
+      a = a.astype(np.int64) if all(_is_int(v) for v in a.flat) else StringLookup._strings(a)
+    if a.dtype.kind in "iu":
+      if a.dtype.kind == "u" and a.size and a.max() > np.iinfo(np.int64).max:
+        raise ValueError("Hashing: unsigned values must fit in int64")
+      x = torch.from_numpy(np.ascontiguousarray(a if a.dtype in (np.int32, np.int64) else a.astype(np.int64)))
+      return ops.hashing(x.to(_device()), self.num_bins, self.salt, self._int_mask())
+    if a.dtype.kind not in "US":
+      raise TypeError(f"Hashing takes integers or strings, got dtype {a.dtype}")
+    if self.mask_value is not None and _is_int(self.mask_value):
+      raise TypeError(f"Hashing: the integer mask_value {self.mask_value} cannot mask string inputs")
+    data, offsets, shape = pack_strings(a if a.size else np.zeros(a.shape, "S1"))
+    dev = _device()
+    if self.mask_value is None:
+      byts, offs = upload_packed(data, offsets, dev)
+      mask = None
+    else:
+      byts, offs, mask = upload_packed(data, offsets, dev, np.frombuffer(StringLookup._as_bytes(self.mask_value), np.uint8))
+    return ops.hashing((byts, offs), self.num_bins, self.salt, mask).reshape(shape)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"name": self.name, "num_bins": self.num_bins, "mask_value": self.mask_value,
+            "salt": None if self.salt is None else list(self.salt), "output_mode": self.output_mode,
+            "sparse": self.sparse}
 
   @classmethod
   def from_config(cls, config: Dict[str, Any]):

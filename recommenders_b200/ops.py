@@ -138,6 +138,43 @@ def hash_bins(values, num_bins: int, salt) -> torch.Tensor:
   return out
 
 
+# ------------------------------------------------------------------------------------------------
+# K18 feature hashing: layers.Hashing
+# ------------------------------------------------------------------------------------------------
+def hashing(values, num_bins: int, salt=None, mask=None) -> torch.Tensor:
+  """tf-keras `Hashing(num_bins, mask_value=mask, salt=salt)` on the device, int64 in the values' shape (1-D for strings).
+  `values` is a CUDA int32 / int64 tensor (hashed as its decimal text) or a (uint8 bytes, int64 offsets [n+1]) pair of
+  CUDA tensors.  Without a salt the hash is FarmHash Fingerprint64 (`to_hash_bucket_fast`), with one SipHash-2-4 keyed
+  by `salt_key(salt)`.  `mask` is an int for integer values or a CUDA uint8 tensor of the mask string's bytes; with
+  num_bins > 1 it takes bin 0 and every other value 1 + h mod (num_bins - 1).  One launch."""
+  values, offsets = values if isinstance(values, tuple) else (values, None)
+  kind = _value_kind(values, offsets)
+  if isinstance(num_bins, bool) or not isinstance(num_bins, (int, np.integer)) or not 1 <= num_bins < 2**63:
+    raise ValueError(f"hashing: num_bins must be an int in [1, 2^63), got {num_bins!r}")
+  values = values.contiguous()
+  offsets = offsets.contiguous() if offsets is not None else None
+  n = values.numel() if offsets is None else offsets.numel() - 1
+  out = torch.empty(values.shape if offsets is None else (n,), dtype=torch.int64, device=values.device)
+  key = None if salt is None else (ctypes.c_uint64 * 2)(*salt_key(salt))
+  mask_int, mask_bytes = 0, None
+  if mask is not None:
+    if offsets is None:
+      if isinstance(mask, (bool, torch.Tensor)) or not isinstance(mask, (int, np.integer)):
+        raise TypeError(f"hashing: the mask of integer values must be an int, got {mask!r}")
+      if not -2**63 <= int(mask) < 2**63:
+        raise ValueError(f"hashing: the mask {mask} does not fit in int64")
+      mask_int = int(mask)
+    else:
+      require_cuda(mask, "mask")
+      if mask.dtype != torch.uint8:
+        raise TypeError("hashing: the mask of string values must be uint8 bytes")
+      mask_bytes = mask.contiguous()
+  check(lib().tfrs_hashing(ptr(values), ptr(offsets), kind, n, key, int(num_bins), int(mask is not None), mask_int,
+                           ptr(mask_bytes), 0 if mask_bytes is None else mask_bytes.numel(), ptr(out), stream()),
+        "hashing")
+  return out
+
+
 def _out_rows(x: LookupInput) -> int:
   return x.n if x.row_splits is None else x.row_splits.numel() - 1
 
