@@ -276,7 +276,8 @@ extern "C" int tfrs_sgemm_f32(int transA, int transB, int64_t M, int64_t N, int6
                               const float* B, int64_t ldb, float* C, int64_t ldc, int accumulate, void* stream) {
   TFRS_CHECK_ARG(M >= 0 && N >= 0 && K >= 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "sgemm: bad shape");
   if (M == 0 || N == 0) return TFRS_OK;
-  TFRS_CHECK_ARG(A && B && C, "sgemm: NULL pointer");
+  // K == 0: C = 0 (or C += 0); A and B are never read, and an empty operand may well be NULL
+  TFRS_CHECK_ARG(C && (K == 0 || (A && B)), "sgemm: NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
   EpiStoreAcc epi{C, ldc, accumulate != 0};
   if (!transA && transB) return launch_sgemm<false, true>(A, lda, B, ldb, (int)M, (int)N, (int)K, 1, epi, st);

@@ -1445,6 +1445,9 @@ static int run_call(const Call& c) {
     return TFRS_ERR_UNSUPPORTED;
   }
   if (!c.ws || c.ws_bytes < pl.total + 16) { set_error("topk_tc: workspace too small (%zu < %zu)", c.ws_bytes, pl.total + 16); return TFRS_ERR_WORKSPACE_TOO_SMALL; }
+  // the exact re-scoring (exact_score, the d = 64 band loader) reads fp32 corpus rows as float4 when d % 4 == 0
+  TFRS_CHECK_ARG((c.d & 3) != 0 || (reinterpret_cast<uintptr_t>(c.corpus) & 15) == 0,
+                 "topk_tc: the corpus must be 16-byte aligned when d %% 4 == 0 (d=%d); pass an aligned copy", c.d);
   cudaStream_t st = c.st;
   unsigned char* w = (unsigned char*)(((uintptr_t)c.ws + 15) & ~(uintptr_t)15);
   unsigned char* qimg = w + pl.o_qimg;

@@ -453,10 +453,19 @@ def topk_scan(q: torch.Tensor, corpus: torch.Tensor, k: int, index_offset: int =
   return out_s[:, :k_out], out_i[:, :k_out]
 
 
+def tc_corpus(corpus: torch.Tensor) -> torch.Tensor:
+  """The fp32 corpus as the tensor-core scan reads it.  Its exact re-scoring loads corpus rows as float4 when d % 4 == 0,
+  so a corpus that starts off a 16-byte boundary (a contiguous view with a storage offset, e.g. `flat[1:].view(N, d)`)
+  is handed over as an aligned copy; any other corpus is returned as is, without a copy."""
+  if corpus.shape[-1] % 4 == 0 and corpus.data_ptr() % 16 != 0:
+    return corpus.clone(memory_format=torch.contiguous_format)
+  return corpus
+
+
 def index_build(corpus: torch.Tensor, reuse_slot: Optional[str] = None) -> torch.Tensor:
   """Builds the tensor-core screening image (fp16 GMMA tiles + norm bound) of a corpus.  `reuse_slot` builds it in a
   per-stream scratch buffer instead of a fresh allocation (Streaming's per-chunk images)."""
-  corpus = f32c(corpus, "candidates")
+  corpus = tc_corpus(f32c(corpus, "candidates"))
   N, d = corpus.shape
   nb = lib().tfrs_index_bytes(N, d)
   if nb == 0:
@@ -478,7 +487,7 @@ def _tc_query_chunks(q: torch.Tensor, N: int, k_ws: int):
 def topk_tc(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor, k: int, index_offset: int = 0,
             out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
   """wgmma screening + exact rescoring; bit-identical to topk_scan."""
-  q = f32c(q, "queries"); corpus = f32c(corpus, "candidates")
+  q = f32c(q, "queries"); corpus = tc_corpus(f32c(corpus, "candidates"))
   Q, d = q.shape; N = corpus.shape[0]
   if out is None:
     out_s = torch.empty((Q, k), dtype=torch.float32, device=q.device)
@@ -513,6 +522,7 @@ def topk(q: torch.Tensor, corpus: torch.Tensor, k: int, image=None, index_offset
   st_k = 0 if state is None else state[0].shape[1]
   if image is None or st_k not in (0, k) or not uses_tc_scan(q.shape[0], N, d, k):
     return topk_scan(q, corpus, k, index_offset=index_offset, state=state, out=out)
+  corpus = tc_corpus(f32c(corpus, "candidates"))   # one aligned copy for the image and the scan, if one is needed
   if isinstance(image, str):
     image = index_build(corpus, reuse_slot=image)
   s, i = topk_tc(q, corpus, image, k, index_offset=index_offset, out=out)
@@ -532,7 +542,7 @@ def topk_tc_exclude(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tens
   """`query_with_exclusions` fused into the tensor-core scan's finalize step: ([Q,k] f32 original scores,
   [Q,k] i64 global indices).  `identifiers` (integer tensor covering the corpus, or None = the row index) and
   `exclusions` [Q,E] are compared as int64."""
-  q = f32c(q, "queries"); corpus = f32c(corpus, "candidates")
+  q = f32c(q, "queries"); corpus = tc_corpus(f32c(corpus, "candidates"))
   Q, d = q.shape; N = corpus.shape[0]
   ex = _i64(exclusions, "exclusions", q.device)
   E = int(ex.shape[1])
@@ -550,7 +560,7 @@ def topk_tc_count(q: torch.Tensor, corpus: torch.Tensor, index_buf: torch.Tensor
                   ) -> torch.Tensor:
   """min(k, #{candidates scoring strictly above the positive}) per query, int32 [Q] -- the fused score branch of
   FactorizedTopK (no top-K list is produced)."""
-  q = f32c(q, "queries"); corpus = f32c(corpus, "candidates")
+  q = f32c(q, "queries"); corpus = tc_corpus(f32c(corpus, "candidates"))
   pos = f32c(positive_scores, "positive_scores").view(-1)
   Q, d = q.shape; N = corpus.shape[0]
   out = torch.empty((Q,), dtype=torch.int32, device=q.device)
@@ -699,6 +709,8 @@ def topk_overriding(q: torch.Tensor, corpus: torch.Tensor, k: int, offsets, rows
   if Q == 0 or k_out == 0:
     return out_s, out_i
   width = override_width(k, np.diff(off_h), N)
+  if image is not None:
+    corpus = tc_corpus(corpus)   # one aligned copy for the image and every width class, if one is needed
   if isinstance(image, str) and any(uses_tc_scan(Q, N, d, int(w)) for w in np.unique(width) if w):
     image = index_build(corpus, reuse_slot=image)
   for w in np.unique(width[width > 0]).tolist():
@@ -845,7 +857,7 @@ def tree_ah_search(q: torch.Tensor, index: dict, rows: Optional[torch.Tensor], n
 def topk_sharded(comm, q: torch.Tensor, corpus_local: torch.Tensor, index_buf: Optional[torch.Tensor], k: int,
                  index_offset: int) -> Tuple[torch.Tensor, torch.Tensor]:
   """The row-sharded BruteForce call through the C ABI: local scan -> one NCCL all-gather -> merge, on every rank."""
-  q = f32c(q, "queries"); corpus_local = f32c(corpus_local, "candidates")
+  q = f32c(q, "queries"); corpus_local = tc_corpus(f32c(corpus_local, "candidates"))
   Q, d = q.shape; N = corpus_local.shape[0]
   out_s = torch.empty((Q, k), dtype=torch.float32, device=q.device)
   out_i = torch.empty((Q, k), dtype=torch.int64, device=q.device)
