@@ -19,7 +19,7 @@
 namespace tfrs {
 
 constexpr int UE_THREADS = 256;
-constexpr int UE_MAX_FEATURES = 64;     // per launch; longer calls are split into groups of whole features
+constexpr int UE_MAX_FEATURES = 64;     // per launch; longer calls are split into groups (ue_groups)
 constexpr int UE_MAX_SLOTS = 256;
 
 struct UeFeat {
@@ -200,16 +200,15 @@ ue_lookup_bwd_kernel(const __grid_constant__ UeParams P) {
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Host side: the caller's features and slots are validated once, then packed into one UeParams per group of whole
-// features that fits the parameter block (one group for up to 64 features and 256 slots).
+// Host side: the caller's features and slots are validated once, then packed into one UeParams per group that fits the
+// parameter block (one group for up to 64 features and 256 slots).
 static int ue_check(const tfrs_ue_feature* features, int n_features, const tfrs_ue_slot* slots, int n_slots, bool bwd,
                     const char* what) {
   TFRS_CHECK_ARG(features && slots && n_features > 0 && n_slots > 0, "%s: NULL argument or empty call", what);
   int total = 0;
   for (int k = 0; k < n_features; ++k) {
     const tfrs_ue_feature& f = features[k];
-    TFRS_CHECK_ARG(f.n_chunks > 0 && f.n_chunks <= UE_MAX_SLOTS, "%s: feature %d: n_chunks must be in [1, %d]", what, k,
-                   UE_MAX_SLOTS);
+    TFRS_CHECK_ARG(f.n_chunks > 0, "%s: feature %d: n_chunks must be positive", what, k);
     TFRS_CHECK_ARG(f.n >= 0 && f.n < (1ll << 38), "%s: feature %d: bad n", what, k);
     TFRS_CHECK_ARG(!f.row_splits || (f.n_bags >= 0 && f.combiner >= TFRS_COMBINER_SUM && f.combiner <= TFRS_COMBINER_SQRTN),
                    "%s: feature %d: bad n_bags / combiner", what, k);
@@ -221,7 +220,7 @@ static int ue_check(const tfrs_ue_feature* features, int n_features, const tfrs_
     if (!bwd)
       TFRS_CHECK_ARG(f.n == 0 || (f.values && (f.kind == TFRS_I32 || f.kind == TFRS_I64 || (f.kind == TFRS_BYTES && f.offsets))),
                      "%s: feature %d: NULL values, or kind not I32, I64 or BYTES with offsets", what, k);
-    TFRS_CHECK_ARG(total + f.n_chunks <= n_slots, "%s: the features have more chunks than the %d slots", what, n_slots);
+    TFRS_CHECK_ARG(f.n_chunks <= n_slots - total, "%s: the features have more chunks than the %d slots", what, n_slots);
     for (int c = total; c < total + f.n_chunks; ++c) {
       const tfrs_ue_slot& s = slots[c];
       TFRS_CHECK_ARG(s.dim > 0 && s.dim % 4 == 0 && s.col_off >= 0 && s.col_off % 4 == 0 && s.ld % 4 == 0 &&
@@ -245,36 +244,43 @@ static int ue_check(const tfrs_ue_feature* features, int n_features, const tfrs_
 }
 
 // Calls launch(params, features in the group, slots in the group) once per group; y_slot / y_feat start as the identity
-// map over the group's slots (the backward launch), the forward rewrites them for its pooling launch.
+// map over the group's slots (the backward launch), the forward rewrites them for its pooling launch.  A feature goes
+// whole into the current group, or into a fresh one when its chunks do not fit.  A feature of more than UE_MAX_SLOTS
+// chunks fills the current group and continues in fresh ones, one UeFeat entry per group over a disjoint range of its
+// chunks: every slot carries its own salt, table and columns, so the chunks of a feature are independent.
 template <typename Launch>
 static int ue_groups(const tfrs_ue_feature* features, int n_features, const tfrs_ue_slot* slots, bool bwd, Launch launch) {
   UeParams p;
   int nf = 0, ns = 0, slot0 = 0;
-  for (int k = 0; k <= n_features; ++k) {
-    if (nf > 0 && (k == n_features || nf == UE_MAX_FEATURES || ns + features[k].n_chunks > UE_MAX_SLOTS)) {
-      const int rc = launch(p, nf, ns);
-      if (rc != TFRS_OK) return rc;
-      nf = 0; ns = 0;
-    }
-    if (k == n_features) break;
+  for (int k = 0; k < n_features; ++k) {
     const tfrs_ue_feature& f = features[k];
-    UeFeat& d = p.f[nf];
-    d.values = f.values; d.offsets = f.offsets; d.splits = f.row_splits; d.n = f.n;
-    d.n_bags = f.row_splits ? f.n_bags : 0; d.first = ns; d.n_chunks = f.n_chunks; d.kind = f.kind;
-    d.combiner = f.combiner; d.copy = f.row_splits ? 0 : 1;
-    for (int c = 0; c < f.n_chunks; ++c) {
-      const tfrs_ue_slot& s = slots[slot0 + c];
-      UeSlot& o = p.s[ns + c];
-      o.table = s.table; o.grad = s.grad; o.out = bwd ? s.grad_rows : s.out;
-      o.ids = reinterpret_cast<long long*>(s.ids);
-      o.k0 = s.salt[0]; o.k1 = s.salt[1];
-      o.nbins = (unsigned long long)(s.rows > 0 ? s.rows : 1); o.magic = ~0ull / o.nbins;
-      o.ld = s.ld; o.col_off = s.col_off; o.dim = s.dim;
-      p.y_slot[ns + c] = (short)(ns + c); p.y_feat[ns + c] = (short)nf;
+    for (int c0 = 0; c0 < f.n_chunks;) {
+      if (nf > 0 && (nf == UE_MAX_FEATURES || ns == UE_MAX_SLOTS ||
+                     (f.n_chunks <= UE_MAX_SLOTS && ns + f.n_chunks > UE_MAX_SLOTS))) {
+        const int rc = launch(p, nf, ns);
+        if (rc != TFRS_OK) return rc;
+        nf = 0; ns = 0;
+      }
+      const int nc = min(f.n_chunks - c0, UE_MAX_SLOTS - ns);
+      UeFeat& d = p.f[nf];
+      d.values = f.values; d.offsets = f.offsets; d.splits = f.row_splits; d.n = f.n;
+      d.n_bags = f.row_splits ? f.n_bags : 0; d.first = ns; d.n_chunks = nc; d.kind = f.kind;
+      d.combiner = f.combiner; d.copy = f.row_splits ? 0 : 1;
+      for (int c = 0; c < nc; ++c) {
+        const tfrs_ue_slot& s = slots[slot0 + c0 + c];
+        UeSlot& o = p.s[ns + c];
+        o.table = s.table; o.grad = s.grad; o.out = bwd ? s.grad_rows : s.out;
+        o.ids = reinterpret_cast<long long*>(s.ids);
+        o.k0 = s.salt[0]; o.k1 = s.salt[1];
+        o.nbins = (unsigned long long)(s.rows > 0 ? s.rows : 1); o.magic = ~0ull / o.nbins;
+        o.ld = s.ld; o.col_off = s.col_off; o.dim = s.dim;
+        p.y_slot[ns + c] = (short)(ns + c); p.y_feat[ns + c] = (short)nf;
+      }
+      c0 += nc; ns += nc; ++nf;
     }
-    slot0 += f.n_chunks; ns += f.n_chunks; ++nf;
+    slot0 += f.n_chunks;
   }
-  return TFRS_OK;
+  return nf > 0 ? launch(p, nf, ns) : TFRS_OK;
 }
 
 }  // namespace tfrs
