@@ -179,10 +179,33 @@ def _out_rows(x: LookupInput) -> int:
   return x.n if x.row_splits is None else x.row_splits.numel() - 1
 
 
-def _check_2d(t: torch.Tensor, rows: int, what: str) -> None:
+def _check_2d(t: torch.Tensor, rows: int, what: str, op: str) -> None:
   require_cuda(t, what)
   if t.dtype != torch.float32 or t.dim() != 2 or t.shape[0] != rows or (t.stride(1) != 1 and t.numel() > 0):
-    raise ValueError(f"unified_lookup: {what} must be 2-D float32 [{rows}, >= width] with unit inner stride")
+    raise ValueError(f"{op}: {what} must be 2-D float32 [{rows}, >= width] with unit inner stride")
+
+
+def _view_ld(m: torch.Tensor, col_off: int, dim: int, what: str, op: str) -> int:
+  """The row stride (`ld`) the kernels use for columns [col_off, col_off + dim) of the 2-D view `m` (checked by
+  _check_2d): its stride(0), or its width when it has at most one row.  Columns past the view's width, and rows that
+  overlap (0 < stride(0) < width, or an expanded view with stride(0) == 0), raise: the kernel would read or write
+  outside the view, and past its storage on the last row."""
+  width = m.shape[1]
+  if col_off < 0 or col_off + dim > width:
+    raise ValueError(f"{op}: {what}: columns [{col_off}, {col_off + dim}) run outside its {width} columns")
+  if m.shape[0] <= 1:
+    return width
+  if m.stride(0) < width:
+    raise ValueError(f"{op}: {what}: rows overlap (row stride {m.stride(0)} < width {width}); pass a contiguous tensor")
+  return m.stride(0)
+
+
+def _check_splits(s: torch.Tensor, op: str) -> None:
+  require_cuda(s, "row_splits")
+  if s.dtype != torch.int64 or s.dim() != 1 or s.numel() < 1:
+    raise TypeError("row_splits must be a non-empty 1-D int64 tensor")
+  if not s.is_contiguous():
+    raise ValueError(f"{op}: row_splits must be contiguous")
 
 
 def _ue_structs(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], outs: Sequence[torch.Tensor]):
@@ -199,20 +222,18 @@ def _ue_structs(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], outs
     f.values, f.offsets = x.values.data_ptr(), (x.offsets.data_ptr() if x.offsets is not None else None)
     f.n, f.n_chunks = x.n, counts[k]
     if x.row_splits is not None:
-      require_cuda(x.row_splits, "row_splits")
-      if x.row_splits.dtype != torch.int64 or x.row_splits.dim() != 1 or x.row_splits.numel() < 1:
-        raise TypeError("row_splits must be a non-empty 1-D int64 tensor")
+      _check_splits(x.row_splits, "unified_lookup")
       f.row_splits, f.n_bags, f.combiner = x.row_splits.data_ptr(), x.row_splits.numel() - 1, COMBINERS[x.combiner]
   cs = (_UeSlot * len(slots))()
   for c, (s, o) in enumerate(zip(slots, outs)):
     require_cuda(s.table, "table")
     if s.table.dtype != torch.float32 or not s.table.is_contiguous() or s.table.dim() != 2:
       raise ValueError("unified_lookup: tables must be contiguous 2-D float32")
-    _check_2d(o, _out_rows(inputs[s.input]), "each output / gradient")
+    _check_2d(o, _out_rows(inputs[s.input]), "each output / gradient", "unified_lookup")
     d = cs[c]
     d.table, d.rows, d.dim = s.table.data_ptr(), s.table.shape[0], s.table.shape[1]
     d.salt[0], d.salt[1] = s.salt
-    d.ld, d.col_off = max(o.stride(0), o.shape[1]), s.col_off
+    d.ld, d.col_off = _view_ld(o, s.col_off, d.dim, "each output / gradient", "unified_lookup"), s.col_off
     if s.ids is not None:
       require_cuda(s.ids, "ids")
       if s.ids.dtype != torch.int64 or not s.ids.is_contiguous() or s.ids.numel() != inputs[s.input].n:
@@ -284,8 +305,9 @@ def bag_out_rows(f: BagFeature) -> int:
   return bags * f.max_sequence_length if f.max_sequence_length > 0 else bags
 
 
-def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor]):
-  """The C descriptors; `mats[k]` is the 2-D tensor feature k's columns live in (its output, or that output's gradient)."""
+def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor], op: str):
+  """The C descriptors; `mats[k]` is the 2-D tensor feature k's columns live in (its output, or that output's gradient).
+  `op` names the caller in error messages."""
   cs = (_BagFeature * len(features))()
   for k, (f, m) in enumerate(zip(features, mats)):
     d = cs[k]
@@ -298,9 +320,7 @@ def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor]):
       raise ValueError("embedding_bag: values must be contiguous")
     d.values, d.n = f.values.data_ptr(), f.values.numel()
     if f.row_splits is not None:
-      require_cuda(f.row_splits, "row_splits")
-      if f.row_splits.dtype != torch.int64 or f.row_splits.dim() != 1 or f.row_splits.numel() < 1:
-        raise TypeError("row_splits must be a non-empty 1-D int64 tensor")
+      _check_splits(f.row_splits, op)
       d.row_splits, d.n_bags = f.row_splits.data_ptr(), f.row_splits.numel() - 1
       d.combiner, d.max_seq_len = COMBINERS[f.combiner], int(f.max_sequence_length)
     if f.weights is not None:
@@ -308,14 +328,15 @@ def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor]):
       if f.weights.dtype != torch.float32 or not f.weights.is_contiguous() or f.weights.numel() != f.values.numel():
         raise ValueError("embedding_bag: weights must be contiguous float32 with one entry per value")
       d.weights = f.weights.data_ptr()
-    _check_2d(m, bag_out_rows(f), "each output / gradient")
-    d.ld, d.col_off = max(m.stride(0), m.shape[1]), f.col_off
+    _check_2d(m, bag_out_rows(f), "each output / gradient", op)
+    d.ld, d.col_off = _view_ld(m, f.col_off, d.dim, "each output / gradient", op), f.col_off
     if f.ids is not None:
       require_cuda(f.ids, "ids")
       if f.ids.dtype != torch.int64 or not f.ids.is_contiguous() or f.ids.numel() != f.values.numel():
         raise ValueError("embedding_bag: ids must be contiguous int64 with one entry per value")
       d.ids = f.ids.data_ptr()
     if f.denom is not None:
+      require_cuda(f.denom, "denom")
       if f.denom.dtype != torch.float32 or not f.denom.is_contiguous() or f.denom.numel() != d.n_bags:
         raise ValueError("embedding_bag: denom must be contiguous float32 with one entry per bag")
       d.denom = f.denom.data_ptr()
@@ -325,7 +346,7 @@ def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor]):
 def embedding_bag(features: Sequence[BagFeature]) -> None:
   """Every lookup of one call (tfrs_embedding_bag_fwd_f32): pooled bags, sequence positions and dense values written
   into each feature's `out`.  One launch for up to 128 features."""
-  cs = _bag_structs(features, [f.out for f in features])
+  cs = _bag_structs(features, [f.out for f in features], "embedding_bag")
   for k, f in enumerate(features):
     cs[k].out = f.out.data_ptr()
   check(lib().tfrs_embedding_bag_fwd_f32(cs, len(features), stream()), "embedding_bag")
@@ -337,7 +358,7 @@ def embedding_bag_bwd(features: Sequence[BagFeature], grads: Sequence[torch.Tens
   its 2-D output; `out` itself is not read) and the forward's `denom`.  One launch for up to 128 features."""
   if len(grads) != len(features) or len(grad_rows) != len(features):
     raise ValueError("embedding_bag_bwd: one gradient and one grad_rows tensor per feature")
-  cs = _bag_structs(features, grads)
+  cs = _bag_structs(features, grads, "embedding_bag_bwd")
   for k, (f, g, r) in enumerate(zip(features, grads, grad_rows)):
     require_cuda(r, "grad_rows")
     if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (f.values.numel(), cs[k].dim):
