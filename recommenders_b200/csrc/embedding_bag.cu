@@ -20,6 +20,7 @@
 //            backward: V*(id + weight) + V*dim*4 (rows written) + gradient rows read (each bag's gradient once per value,
 //            mostly from L2).  V = values, R = output rows.
 #include "common.cuh"
+#include "bags.cuh"
 
 namespace tfrs {
 
@@ -53,12 +54,6 @@ __device__ __forceinline__ long long bg_id(const BagFeat& f, long long v) {
 }
 
 __device__ __forceinline__ float bg_w(const BagFeat& f, long long v) { return f.weights ? __ldg(f.weights + v) : 1.f; }
-
-__device__ __forceinline__ void bg_bag(const BagFeat& f, long long b, long long* s0, long long* s1) {
-  const long long a = min(max((long long)__ldg(f.splits + b), 0ll), f.n);
-  *s0 = a;
-  *s1 = min(max((long long)__ldg(f.splits + b + 1), a), f.n);
-}
 
 // V = 4: float4 pieces; V = 1: single columns.  The arithmetic is per column and identical in both.
 template <int V> struct Vec;
@@ -100,14 +95,14 @@ __device__ __forceinline__ void bg_fwd_item(const BagFeat& f, long long r, int c
     const long long b = r / f.seq_len;
     const int j = (int)(r - b * f.seq_len);
     long long s0, s1;
-    bg_bag(f, b, &s0, &s1);
+    bag_range(f, b, &s0, &s1);
     if (s0 + j < s1) {
       const long long id = bg_id(f, s0 + j);
       if (id >= 0 && id < f.rows) acc = X::mul(X::load(f.table + id * f.dim + col), bg_w(f, s0 + j));
     }
   } else {                                                    // pooled
     long long s0, s1;
-    bg_bag(f, r, &s0, &s1);
+    bag_range(f, r, &s0, &s1);
     float den = 0.f;
     bool any = false;
     for (long long v0 = s0; v0 < s1; v0 += BG_BATCH) {
@@ -164,13 +159,9 @@ __device__ __forceinline__ typename Vec<V>::T bg_bwd_item(const BagFeat& f, long
   const long long id = bg_id(f, v);
   if (id < 0 || id >= f.rows) return X::zero();
   if (!f.splits) return X::load(f.grad + v * f.ld + f.col_off + col);
-  long long lo = 0, hi = f.n_bags;                           // the last bag whose first value is <= v
-  while (hi - lo > 1) {
-    const long long mid = (lo + hi) >> 1;
-    if (__ldg(f.splits + mid) <= v) lo = mid; else hi = mid;
-  }
+  const long long lo = bag_of(f, v);
   long long s0, s1;
-  bg_bag(f, lo, &s0, &s1);
+  bag_range(f, lo, &s0, &s1);
   if (v < s0 || v >= s1) return X::zero();
   const float w = bg_w(f, v);
   if (f.seq_len > 0) {

@@ -15,6 +15,7 @@
 // Bucket ids alone (tfrs_hash_bins) come from K18's hash-only kernel (hashing.cu).
 #include "common.cuh"
 #include "bucket.cuh"
+#include "bags.cuh"
 
 namespace tfrs {
 
@@ -128,12 +129,6 @@ __device__ __forceinline__ float4 combine(float4 a, int combiner, long long coun
   return make_float4(__fdiv_rn(a.x, d), __fdiv_rn(a.y, d), __fdiv_rn(a.z, d), __fdiv_rn(a.w, d));
 }
 
-__device__ __forceinline__ void bag_range(const UeFeat& f, long long b, long long* s0, long long* s1) {
-  const long long a = min(max((long long)f.splits[b], 0ll), f.n);
-  *s0 = a;
-  *s1 = min(max((long long)f.splits[b + 1], a), f.n);
-}
-
 // A group of dim/4 lanes per (bag, slot): the bag's rows summed in value order from +0, then the combiner.
 __global__ void __launch_bounds__(UE_THREADS)
 ue_pool_kernel(const __grid_constant__ UeParams P) {
@@ -169,6 +164,7 @@ ue_lookup_bwd_kernel(const __grid_constant__ UeParams P) {
   const int lshift = (L & (L - 1)) == 0 ? 31 - __clz(L) : -1;
   const long long total = f.n * L, ld4 = s.ld >> 2;
   const long long stride = (long long)gridDim.x * UE_THREADS;
+  // g4 is read with __ldg: beside bags.cuh's __ldg loads of the splits the compiler no longer picks the read-only path
   const float4* __restrict__ g4 = reinterpret_cast<const float4*>(s.grad + s.col_off);
   float4* __restrict__ rows = reinterpret_cast<float4*>(s.out);
   const bool pooled = f.splits != nullptr;
@@ -180,15 +176,12 @@ ue_lookup_bwd_kernel(const __grid_constant__ UeParams P) {
       if (w >= total) break;
       const long long i = lshift >= 0 ? w >> lshift : w / L;
       const int sub = (int)(w - i * L);
-      if (!pooled) { v[u] = g4[i * ld4 + sub]; continue; }
-      long long lo = 0, hi = f.n_bags;       // the last bag whose first value is <= i
-      while (hi - lo > 1) {
-        const long long mid = (lo + hi) >> 1;
-        if (f.splits[mid] <= i) lo = mid; else hi = mid;
-      }
+      if (!pooled) { v[u] = __ldg(g4 + i * ld4 + sub); continue; }
+      const long long lo = bag_of(f, i);
       long long a, z;
       bag_range(f, lo, &a, &z);
-      v[u] = (i >= a && i < z) ? combine(g4[lo * ld4 + sub], f.combiner, z - a) : make_float4(0.f, 0.f, 0.f, 0.f);
+      v[u] = (i >= a && i < z) ? combine(__ldg(g4 + lo * ld4 + sub), f.combiner, z - a)
+                               : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int u = 0; u < UE_BWD_ITEMS; ++u) {

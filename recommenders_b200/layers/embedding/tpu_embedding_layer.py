@@ -16,11 +16,10 @@ from __future__ import annotations
 
 from typing import Any, Dict, List, Optional
 
-import numpy as np
 import torch
 
 from ... import ops
-from . import Embedding
+from . import Embedding, _default_initializer, _ragged_splits, _record_sparse_grads, _sparse_grad_ids, _upload
 
 
 class TableConfig:
@@ -104,12 +103,6 @@ def pack_as(structure, leaves: List[Any]):
   return rec(structure)
 
 
-def _default_initializer(dim: int):
-  # TableConfig's default, shared with UnifiedEmbedding; imported here because that module imports this package
-  from ..feature_multiplexing.unified_embedding import _default_initializer as init
-  return init(dim)
-
-
 class _Input:
   """One feature's input after classification: flat CUDA ids, int64 row splits (None: dense), weights, output shape."""
 
@@ -128,15 +121,7 @@ class _Input:
         w = w.coalesce().values()
     elif isinstance(x, tuple) and len(x) == 2:
       self.values, splits = x
-      if isinstance(splits, torch.Tensor):
-        ops.require_cuda(splits, f"row_splits of '{name}'")
-        if splits.dtype != torch.int64 or splits.dim() != 1:
-          raise TypeError(f"row_splits of '{name}' must be a 1-D int64 tensor")
-        self.row_splits = splits.contiguous()
-      elif isinstance(splits, np.ndarray) and splits.dtype.kind in "iu" and splits.ndim == 1:
-        self.host_splits = splits.astype(np.int64)
-      else:
-        raise TypeError(f"row_splits of '{name}' must be an int64 CUDA tensor or a NumPy integer array")
+      self.row_splits, self.host_splits = _ragged_splits(name, splits)
       if isinstance(w, tuple):
         w = w[0]
       if isinstance(self.values, torch.Tensor) and self.values.dim() != 1:
@@ -166,19 +151,6 @@ class _Input:
     return s.shape[0] - 1
 
 
-def _upload_splits(inputs: List[_Input], device) -> None:
-  """Every NumPy row split of one call in ONE host-to-device copy."""
-  host = [x.host_splits for x in inputs if x.host_splits is not None]
-  if not host:
-    return
-  dev = torch.from_numpy(np.concatenate(host)).to(device)
-  pos = 0
-  for x in inputs:
-    if x.host_splits is not None:
-      k = x.host_splits.size
-      x.row_splits = dev[pos:pos + k]; pos += k
-
-
 class _BagFn(torch.autograd.Function):
 
   @staticmethod
@@ -193,17 +165,10 @@ class _BagFn(torch.autograd.Function):
 
   @staticmethod
   def backward(ctx, *grads):
-    rows = {t: torch.empty((ids.numel(), ctx.tables[t].output_dim), dtype=torch.float32, device=ids.device)
-            for t, ids in ctx.ids.items()}
-    used = {t: 0 for t in rows}
-    gs, grs = [], []
-    for f, t, g, shape in zip(ctx.feats, ctx.table_of, grads, ctx.out_shapes):
-      gs.append(g.contiguous() if g is not None else torch.zeros(shape, dtype=torch.float32, device=f.values.device))
-      n = f.values.numel()
-      grs.append(rows[t][used[t]:used[t] + n]); used[t] += n
-    ops.embedding_bag_bwd(ctx.feats, gs, grs)
-    for t, ids in ctx.ids.items():
-      ctx.tables[t]._sparse_grads.append((ids, rows[t]))
+    gs = [g.contiguous() if g is not None else torch.zeros(shape, dtype=torch.float32, device=f.values.device)
+          for f, g, shape in zip(ctx.feats, grads, ctx.out_shapes)]
+    _record_sparse_grads(ctx.tables, ctx.table_of, [f.values.numel() for f in ctx.feats], ctx.ids,
+                         lambda rows: ops.embedding_bag_bwd(ctx.feats, gs, rows))
     return (None,) * (4 + len(ctx.tables))
 
 
@@ -251,24 +216,20 @@ class TPUEmbedding(torch.nn.Module):
     names = [f.name or str(i) for i, f in enumerate(self._features)]
     inputs = [_Input(nm, x, w, fc.max_sequence_length) for nm, x, w, fc in zip(names, flat, flat_w, self._features)]
     dev = self._tables[0].weight.device
-    _upload_splits(inputs, dev)
+    host = [x for x in inputs if x.host_splits is not None]       # every NumPy row split of the call in one copy
+    for x, splits in zip(host, _upload([x.host_splits for x in host], dev)[0]):
+      x.row_splits = splits
     grad = torch.is_grad_enabled()
-    total: Dict[int, int] = {}
-    for x, t in zip(inputs, self._table_of):
-      total[t] = total.get(t, 0) + x.values.numel()
-    ids = {t: torch.empty(n, dtype=torch.int64, device=dev) for t, n in total.items()} if grad else {}
-    used = {t: 0 for t in ids}
+    ids, sids = (_sparse_grad_ids(self._table_of, [x.values.numel() for x in inputs], dev) if grad
+                 else ({}, [None] * len(inputs)))
     feats = []
-    for x, t, fc in zip(inputs, self._table_of, self._features):
+    for x, t, sid in zip(inputs, self._table_of, sids):
       cfg = self._table_configs[t]
       f = ops.BagFeature(self._tables[t].weight, x.values, None, x.row_splits, x.weights, cfg.combiner, x.seq_len)
       out = torch.empty((ops.bag_out_rows(f), cfg.dim), dtype=torch.float32, device=dev)
-      sid = denom = None
-      if grad:
-        n = x.values.numel()
-        sid = ids[t][used[t]:used[t] + n]; used[t] += n
-        if x.bagged and x.seq_len == 0 and cfg.combiner != "sum":
-          denom = torch.empty(x.n_bags, dtype=torch.float32, device=dev)
+      denom = None
+      if grad and x.bagged and x.seq_len == 0 and cfg.combiner != "sum":
+        denom = torch.empty(x.n_bags, dtype=torch.float32, device=dev)
       feats.append(f._replace(out=out, ids=sid, denom=denom))
     if grad:
       outs = _BagFn.apply(list(self._tables), feats, self._table_of, ids, *[t._anchor for t in self._tables])

@@ -19,7 +19,6 @@ Inputs, per feature name:
 """
 from __future__ import annotations
 
-import math
 from typing import Any, Dict, List, NamedTuple, Tuple
 
 import numpy as np
@@ -27,7 +26,7 @@ import torch
 
 from ... import ops
 from ..._strings import is_strings as _is_strings, pack_strings as _pack_strings
-from ..embedding import Embedding
+from ..embedding import Embedding, _default_initializer, _ragged_splits, _record_sparse_grads, _sparse_grad_ids, _upload
 
 
 class FeatureConfig(NamedTuple):
@@ -37,15 +36,6 @@ class FeatureConfig(NamedTuple):
 
 
 _TABLE_KWARGS = ("initializer", "combiner")
-
-
-def _default_initializer(dim: int):
-  """TableConfig's default: truncated normal, mean 0, std 1/sqrt(dim), cut at two standard deviations."""
-  std = 1.0 / math.sqrt(dim)
-
-  def init(shape, device):
-    return torch.nn.init.trunc_normal_(torch.empty(shape, device=device), 0.0, std, -2.0 * std, 2.0 * std)
-  return init
 
 
 class UnifiedEmbeddingConfig:
@@ -120,15 +110,7 @@ class _Feature:
     self.row_splits = self.host_splits = self.strings = self.values = None
     if isinstance(x, tuple) and len(x) == 2:
       values, splits = x
-      if isinstance(splits, torch.Tensor):
-        ops.require_cuda(splits, f"row_splits of '{name}'")
-        if splits.dtype != torch.int64 or splits.dim() != 1:
-          raise TypeError(f"row_splits of '{name}' must be a 1-D int64 tensor")
-        self.row_splits = splits.contiguous()
-      elif isinstance(splits, np.ndarray) and splits.dtype.kind in "iu" and splits.ndim == 1:
-        self.host_splits = splits.astype(np.int64)
-      else:
-        raise TypeError(f"row_splits of '{name}' must be an int64 CUDA tensor or a NumPy integer array")
+      self.row_splits, self.host_splits = _ragged_splits(name, splits)
       self.n_bags = (self.row_splits if self.row_splits is not None else self.host_splits).shape[0] - 1
     else:
       values = x
@@ -149,29 +131,6 @@ class _Feature:
     self.n = int(np.prod(self.shape, dtype=np.int64))
 
 
-def _upload(feats: List[_Feature], device) -> None:
-  """Every string buffer and NumPy row split of one call in ONE host-to-device copy: the int64 arrays first (8-byte
-  aligned), then the bytes."""
-  i64 = [a for f in feats for a in ((f.strings[1] if f.strings else None), f.host_splits) if a is not None]
-  data = [f.strings[0] for f in feats if f.strings]
-  if not i64:
-    return
-  n64 = sum(a.size for a in i64)
-  host = np.concatenate([np.concatenate(i64).view(np.uint8)] + data)
-  dev = torch.from_numpy(host).to(device)
-  words, pos, byte_pos = dev[:8 * n64].view(torch.int64), 0, 8 * n64
-  for f in feats:
-    if f.strings:
-      k = f.strings[1].size
-      offsets = words[pos:pos + k]; pos += k
-      nb = f.strings[0].size
-      f.values = (dev[byte_pos:byte_pos + max(nb, 1)] if nb else dev[:1]), offsets
-      byte_pos += nb
-    if f.host_splits is not None:
-      k = f.host_splits.size
-      f.row_splits = words[pos:pos + k]; pos += k
-
-
 class _UnifiedLookupFn(torch.autograd.Function):
 
   @staticmethod
@@ -186,16 +145,9 @@ class _UnifiedLookupFn(torch.autograd.Function):
   @staticmethod
   def backward(ctx, *grads):
     layer, slots = ctx.layer, ctx.slots
-    dim = layer._config._dim_per_table
-    rows = {t: torch.empty((ids.numel(), dim), dtype=torch.float32, device=ids.device) for t, ids in ctx.ids.items()}
-    slot_grads, slot_rows, used = [], [], {t: 0 for t in rows}
-    for s, t in zip(slots, layer._slot_tables):
-      slot_grads.append(grads[s.input].contiguous())
-      n = ctx.inputs[s.input].n
-      slot_rows.append(rows[t][used[t]:used[t] + n]); used[t] += n
-    ops.unified_lookup_bwd(ctx.inputs, slots, slot_grads, slot_rows)
-    for t, ids in ctx.ids.items():
-      layer._tables[t]._sparse_grads.append((ids, rows[t]))
+    slot_grads = [grads[s.input].contiguous() for s in slots]
+    _record_sparse_grads(layer._tables, layer._slot_tables, [ctx.inputs[s.input].n for s in slots], ctx.ids,
+                         lambda rows: ops.unified_lookup_bwd(ctx.inputs, slots, slot_grads, rows))
     return (None,) * (5 + len(layer._tables))
 
 
@@ -234,15 +186,23 @@ class UnifiedEmbedding(torch.nn.Module):
   def forward(self, features: Dict[str, Any]) -> List[torch.Tensor]:
     feats = [_Feature(name, features[name]) for name, _ in self._plan]
     dev = self._tables[0].weight.device
-    _upload(feats, dev)
+    # every string buffer (bytes and offsets) and NumPy row split of the call in one copy
+    words, data = _upload([a for f in feats for a in ((f.strings[1] if f.strings else None), f.host_splits)
+                           if a is not None], dev, [f.strings[0] for f in feats if f.strings])
+    words, data = iter(words), iter(data)
+    for f in feats:
+      if f.strings:
+        f.values = next(data), next(words)
+      if f.host_splits is not None:
+        f.row_splits = next(words)
     grad = torch.is_grad_enabled()
     dim = self._config._dim_per_table
-    total = {}
-    for f, (_, chunks) in zip(feats, self._plan):
-      for t, _, _ in chunks:
-        total[t] = total.get(t, 0) + f.n
-    ids = {t: torch.empty(n, dtype=torch.int64, device=dev) for t, n in total.items()} if grad else {}
-    used = {t: 0 for t in ids}
+    slot_feats = [f for f, (_, chunks) in zip(feats, self._plan) for _ in chunks]
+    if grad:
+      ids, sids = _sparse_grad_ids(self._slot_tables, [f.n for f in slot_feats], dev)
+    else:   # K8's pooling reads the bucket ids of pooled slots
+      ids, sids = {}, [torch.empty(f.n, dtype=torch.int64, device=dev) if f.pooled else None for f in slot_feats]
+    sids = iter(sids)
     inputs, slots, outs = [], [], []
     for k, (f, (_, chunks)) in enumerate(zip(feats, self._plan)):
       values, offsets = f.values if isinstance(f.values, tuple) else (f.values, None)
@@ -250,11 +210,7 @@ class UnifiedEmbedding(torch.nn.Module):
       out = torch.empty((f.n_bags if f.pooled else f.n, len(chunks) * dim), dtype=torch.float32, device=dev)
       outs.append(out)
       for t, key, pos in chunks:
-        if grad:
-          sid = ids[t][used[t]:used[t] + f.n]; used[t] += f.n
-        else:
-          sid = torch.empty(f.n, dtype=torch.int64, device=dev) if f.pooled else None
-        slots.append(ops.LookupSlot(k, self._tables[t].weight, key, out, pos * dim, sid))
+        slots.append(ops.LookupSlot(k, self._tables[t].weight, key, out, pos * dim, next(sids)))
     if grad:
       outs = _UnifiedLookupFn.apply(self, inputs, slots, outs, ids, *[t._anchor for t in self._tables])
     else:

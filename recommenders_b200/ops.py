@@ -208,6 +208,24 @@ def _check_splits(s: torch.Tensor, op: str) -> None:
     raise ValueError(f"{op}: row_splits must be contiguous")
 
 
+def _check_table(t: torch.Tensor, op: str) -> None:
+  require_cuda(t, "table")
+  if t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 2:
+    raise ValueError(f"{op}: tables must be contiguous 2-D float32")
+
+
+def _check_ids(ids: torch.Tensor, n: int, op: str) -> None:
+  require_cuda(ids, "ids")
+  if ids.dtype != torch.int64 or not ids.is_contiguous() or ids.numel() != n:
+    raise ValueError(f"{op}: ids must be contiguous int64 with one entry per value")
+
+
+def _check_grad_rows(r: torch.Tensor, n: int, dim: int, op: str) -> None:
+  require_cuda(r, "grad_rows")
+  if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (n, dim):
+    raise ValueError(f"{op}: grad_rows must be contiguous float32 [n, dim]")
+
+
 def _ue_structs(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], outs: Sequence[torch.Tensor]):
   """The C descriptors of one call; slots must come grouped by input, inputs in order.  `outs[c]` is the 2-D tensor
   slot c's columns live in: its output in the forward, the gradient of that output in the backward."""
@@ -226,18 +244,14 @@ def _ue_structs(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot], outs
       f.row_splits, f.n_bags, f.combiner = x.row_splits.data_ptr(), x.row_splits.numel() - 1, COMBINERS[x.combiner]
   cs = (_UeSlot * len(slots))()
   for c, (s, o) in enumerate(zip(slots, outs)):
-    require_cuda(s.table, "table")
-    if s.table.dtype != torch.float32 or not s.table.is_contiguous() or s.table.dim() != 2:
-      raise ValueError("unified_lookup: tables must be contiguous 2-D float32")
+    _check_table(s.table, "unified_lookup")
     _check_2d(o, _out_rows(inputs[s.input]), "each output / gradient", "unified_lookup")
     d = cs[c]
     d.table, d.rows, d.dim = s.table.data_ptr(), s.table.shape[0], s.table.shape[1]
     d.salt[0], d.salt[1] = s.salt
     d.ld, d.col_off = _view_ld(o, s.col_off, d.dim, "each output / gradient", "unified_lookup"), s.col_off
     if s.ids is not None:
-      require_cuda(s.ids, "ids")
-      if s.ids.dtype != torch.int64 or not s.ids.is_contiguous() or s.ids.numel() != inputs[s.input].n:
-        raise ValueError("unified_lookup: ids must be contiguous int64 with one entry per value")
+      _check_ids(s.ids, inputs[s.input].n, "unified_lookup")
       d.ids = s.ids.data_ptr()
   return feats, cs
 
@@ -260,9 +274,7 @@ def unified_lookup_bwd(inputs: Sequence[LookupInput], slots: Sequence[LookupSlot
     raise ValueError("unified_lookup_bwd: one gradient and one grad_rows tensor per slot")
   feats, cs = _ue_structs(inputs, slots, grads)
   for c, (g, r) in enumerate(zip(grads, grad_rows)):
-    require_cuda(r, "grad_rows")
-    if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (inputs[slots[c].input].n, cs[c].dim):
-      raise ValueError("unified_lookup_bwd: grad_rows must be contiguous float32 [n, dim]")
+    _check_grad_rows(r, inputs[slots[c].input].n, cs[c].dim, "unified_lookup_bwd")
     cs[c].grad, cs[c].grad_rows = g.data_ptr(), r.data_ptr()
   check(lib().tfrs_unified_lookup_bwd_f32(feats, len(inputs), cs, len(slots), stream()), "unified_lookup_bwd")
 
@@ -311,9 +323,7 @@ def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor], o
   cs = (_BagFeature * len(features))()
   for k, (f, m) in enumerate(zip(features, mats)):
     d = cs[k]
-    require_cuda(f.table, "table")
-    if f.table.dtype != torch.float32 or not f.table.is_contiguous() or f.table.dim() != 2:
-      raise ValueError("embedding_bag: tables must be contiguous 2-D float32")
+    _check_table(f.table, "embedding_bag")
     d.table, d.rows, d.dim = f.table.data_ptr(), f.table.shape[0], f.table.shape[1]
     d.kind = _ffi.ids_dtype_code(require_cuda(f.values, "values"))
     if not f.values.is_contiguous():
@@ -331,9 +341,7 @@ def _bag_structs(features: Sequence[BagFeature], mats: Sequence[torch.Tensor], o
     _check_2d(m, bag_out_rows(f), "each output / gradient", op)
     d.ld, d.col_off = _view_ld(m, f.col_off, d.dim, "each output / gradient", op), f.col_off
     if f.ids is not None:
-      require_cuda(f.ids, "ids")
-      if f.ids.dtype != torch.int64 or not f.ids.is_contiguous() or f.ids.numel() != f.values.numel():
-        raise ValueError("embedding_bag: ids must be contiguous int64 with one entry per value")
+      _check_ids(f.ids, f.values.numel(), "embedding_bag")
       d.ids = f.ids.data_ptr()
     if f.denom is not None:
       require_cuda(f.denom, "denom")
@@ -360,9 +368,7 @@ def embedding_bag_bwd(features: Sequence[BagFeature], grads: Sequence[torch.Tens
     raise ValueError("embedding_bag_bwd: one gradient and one grad_rows tensor per feature")
   cs = _bag_structs(features, grads, "embedding_bag_bwd")
   for k, (f, g, r) in enumerate(zip(features, grads, grad_rows)):
-    require_cuda(r, "grad_rows")
-    if r.dtype != torch.float32 or not r.is_contiguous() or r.shape != (f.values.numel(), cs[k].dim):
-      raise ValueError("embedding_bag_bwd: grad_rows must be contiguous float32 [n, dim]")
+    _check_grad_rows(r, f.values.numel(), cs[k].dim, "embedding_bag_bwd")
     cs[k].grad, cs[k].grad_rows = g.data_ptr(), r.data_ptr()
   check(lib().tfrs_embedding_bag_bwd_f32(cs, len(features), stream()), "embedding_bag_bwd")
 
