@@ -842,6 +842,37 @@ int tfrs_mean_pool_bwd(const float* g, int64_t B, int64_t T, int64_t d, const vo
 int tfrs_hashing(const void* values, const int64_t* offsets, int kind, int64_t n, const uint64_t* salt, int64_t num_bins,
                  int has_mask, int64_t mask, const uint8_t* mask_bytes, int64_t mask_len, int64_t* bins, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K19 GRU recurrence: tf.keras.layers.GRU(units, reset_after=True) as the reference's sequential retrieval tutorial
+ * builds its query tower (`Sequential([StringLookup, Embedding, GRU(32)])`).  Weights as Keras stores them, columns
+ * ordered (z, r, h): kernel W [D, 3u], recurrent_kernel U [u, 3u], bias [2, 3u] = (b_i, b_r).  The input projection
+ * gx = x.W + b_i ([B*T, 3u], row b*T + t) is the caller's, on K6 (tfrs_dense_fwd_f32 / tfrs_dense_bwd_f32).
+ *   gr = h_{t-1}.U + b_r (fmaf chain over k ascending from +0.0f, then + b_r);  z = sigmoid(gx_z + gr_z),
+ *   r = sigmoid(gx_r + gr_r),  hh = tanh(gx_h + r gr_h),  h_t = z h_{t-1} + (1 - z) hh;  sigmoid = 1 / (1 + expf(-x)).
+ * h_0 = h0 [B, u], or zeros when h0 is NULL.  mask [B, T] (TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero = kept, nullable):
+ * at a masked step h_t = h_{t-1} and nothing is computed.  1 <= units <= TFRS_GRU_MAX_UNITS, T >= 1, B < 2^31; B == 0
+ * writes nothing.
+ *   tfrs_gru_fwd_f32: h_last [B, u] = h_T; out_seq [B, T, u] = every h_t (nullable); gates [B, T, 4u] = (z, r, hh, gr_h)
+ *     and h_prev [B, T, u] = h_{t-1} (both or neither, for the backward; gates are not written at masked steps).
+ *     One launch.
+ *   tfrs_gru_bwd_f32: from the upstream gradients g_seq [B, T, u] (of out_seq) and g_last [B, u] (of h_last), either
+ *     nullable, in reverse t with dh carried:  dh += g_seq[t] (+ g_last at T-1);  dz = dh (h_{t-1} - hh) z (1 - z);
+ *     dn = dh (1 - z)(1 - hh^2);  dr = dn gr_h r (1 - r);  dgx = [dz | dr | dn];  dgr = [dz | dr | dn r];
+ *     dh <- dh z + dgr.U^T (fmaf chain over the 3u columns ascending).  A masked step passes dh through and writes zero
+ *     dgx rows.  Writes dgx [B*T, 3u] (the gradient of gx) and dh0 [B, u] (nullable) in one launch, then dU = h_prev^T .
+ *     dgr and db_r = colsum(dgr) (each nullable) with tfrs_dense_bwd_f32.  ws: tfrs_gru_bwd_workspace_bytes, 16-byte
+ *     aligned.  No float atomics.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_GRU_MAX_UNITS 2048
+
+int tfrs_gru_fwd_f32(const float* gx, const float* U, const float* b_r, const float* h0, const void* mask, int mask_kind,
+                     int64_t B, int64_t T, int units, float* out_seq, float* h_last, float* gates, float* h_prev,
+                     void* stream);
+size_t tfrs_gru_bwd_workspace_bytes(int64_t B, int64_t T, int units);
+int tfrs_gru_bwd_f32(const float* U, const float* gates, const float* h_prev, const void* mask, int mask_kind,
+                     const float* g_seq, const float* g_last, int64_t B, int64_t T, int units, float* dgx, float* dU,
+                     float* db_r, float* dh0, void* ws, size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

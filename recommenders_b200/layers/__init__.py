@@ -6,6 +6,8 @@ from . import feature_interaction
 from . import loss
 from . import pooling
 from . import preprocessing
+from . import recurrent
 from .feature_interaction import dcn
 from .pooling import GlobalAveragePooling1D
 from .preprocessing import Discretization, Hashing, IntegerLookup, Normalization, StringLookup, TextVectorization
+from .recurrent import GRU

@@ -1,6 +1,7 @@
 """Cross layer of DCN-v2: mirror of tensorflow_recommenders/layers/feature_interaction/dcn.py."""
 from __future__ import annotations
 
+import math
 from typing import Callable, Optional, Union
 
 import torch
@@ -16,9 +17,18 @@ _ACTIVATIONS = {
 
 def _init(name, shape, device):
   """Keras initializers by name: "truncated_normal" (mean 0, stddev 0.05, cut at 2 sigma), "zeros", "ones",
-  "glorot_uniform"; a callable(shape, device) is used as is."""
+  "glorot_uniform", "orthogonal" (gain 1); a callable(shape, device) is used as is."""
   if callable(name):
     return name(shape, device)
+  if name == "orthogonal":
+    # Keras's Orthogonal: q of the QR of a normal (max(rows, cols), min(rows, cols)) matrix, columns scaled by
+    # sign(diag(r)), transposed when rows < cols -- orthonormal rows or columns, whichever are fewer.  rows = the product
+    # of all dimensions but the last.  Drawn and factorised in float64 on the host from torch's seeded generator.
+    rows, cols = math.prod(shape[:-1]), shape[-1]
+    q, r = torch.linalg.qr(torch.randn((max(rows, cols), min(rows, cols)), dtype=torch.float64))
+    q = q * torch.sign(torch.diagonal(r))
+    q = q.T if rows < cols else q
+    return q.reshape(shape).to(device=device, dtype=torch.float32).contiguous()
   t = torch.empty(shape, dtype=torch.float32, device=device)
   if name == "truncated_normal":
     torch.nn.init.trunc_normal_(t, mean=0.0, std=0.05, a=-0.1, b=0.1)

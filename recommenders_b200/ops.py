@@ -2065,14 +2065,14 @@ def normalization_adapt(x: torch.Tensor, C: int, batch_rows: int, state: torch.T
         "normalization_adapt")
 
 
-def _mask_arg(mask: Optional[torch.Tensor], B: int, T: int):
+def _mask_arg(mask: Optional[torch.Tensor], B: int, T: int, op: str = "mean_pool"):
   if mask is None:
     return None, 0
   require_cuda(mask, "mask")
   if mask.dtype not in _MASK_KINDS:
-    raise TypeError(f"mean_pool: the mask must be bool, int32 or int64, got {mask.dtype}")
+    raise TypeError(f"{op}: the mask must be bool, int32 or int64, got {mask.dtype}")
   if tuple(mask.shape) != (B, T):
-    raise ValueError(f"mean_pool: the mask has shape {tuple(mask.shape)}, the input [{B}, {T}, d]")
+    raise ValueError(f"{op}: the mask has shape {tuple(mask.shape)}, the input [{B}, {T}, d]")
   return mask.contiguous(), _MASK_KINDS[mask.dtype]
 
 
@@ -2116,3 +2116,99 @@ def attached_mask(x: torch.Tensor) -> Optional[torch.Tensor]:
   if hint is not None and hint[1] == x._version and hint[2] == x.data_ptr() and tuple(hint[0].shape) == tuple(x.shape[:-1]):
     return hint[0]
   return None
+
+
+# ------------------------------------------------------------------------------------------------
+# K19 GRU recurrence: layers.GRU (reset_after=True); the input projection runs on K6
+# ------------------------------------------------------------------------------------------------
+GRU_MAX_UNITS = 2048   # TFRS_GRU_MAX_UNITS of include/tfrs_b200.h
+
+
+def _gru_fwd(gx, U, b_r, h0, m, mk, return_sequences: bool, save: bool):
+  B, T, u3 = gx.shape
+  u = u3 // 3
+  new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=gx.device)
+  seq = new(B, T, u) if return_sequences else None
+  h_last = new(B, u)
+  gates, h_prev = (new(B, T, 4 * u), new(B, T, u)) if save else (None, None)
+  check(lib().tfrs_gru_fwd_f32(ptr(gx), ptr(U), ptr(b_r), ptr(h0), ptr(m), mk, B, T, u, ptr(seq), ptr(h_last), ptr(gates),
+                               ptr(h_prev), stream()), "gru_fwd")
+  return seq, h_last, gates, h_prev
+
+
+class _GRURecurrence(torch.autograd.Function):
+  """(out_seq, h_T) with return_sequences, else h_T alone, from gx = x.W + b_i [B, T, 3u]; differentiable in gx, U, b_r
+  and h0."""
+
+  @staticmethod
+  def forward(ctx, gx, U, b_r, h0, m, mk, return_sequences):
+    seq, h_last, gates, h_prev = _gru_fwd(gx, U, b_r, h0, m, mk, return_sequences, True)
+    ctx.save_for_backward(U, gates, h_prev, m)
+    ctx.mk, ctx.return_sequences = mk, return_sequences
+    ctx.set_materialize_grads(False)
+    return (seq, h_last) if return_sequences else h_last
+
+  @staticmethod
+  def backward(ctx, *grads):
+    U, gates, h_prev, m = ctx.saved_tensors
+    g_seq, g_last = grads if ctx.return_sequences else (None, grads[0])
+    B, T, u = h_prev.shape
+    n_gx, n_U, n_br, n_h0 = ctx.needs_input_grad[:4]
+    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=U.device)
+    dgx = new(B, T, 3 * u)
+    dU = new(u, 3 * u) if n_U else None
+    db_r = new(3 * u) if n_br else None
+    dh0 = new(B, u) if n_h0 else None
+    if B == 0 or (g_seq is None and g_last is None):
+      for t in (dgx, dU, db_r, dh0):
+        if t is not None:
+          t.zero_()
+    else:
+      g_seq = None if g_seq is None else f32c(g_seq, "grad")
+      g_last = None if g_last is None else f32c(g_last, "grad")
+      ws = workspace(lib().tfrs_gru_bwd_workspace_bytes(B, T, u), U.device, "gru_bwd")
+      check(lib().tfrs_gru_bwd_f32(ptr(U), ptr(gates), ptr(h_prev), ptr(m), ctx.mk, ptr(g_seq), ptr(g_last), B, T, u,
+                                   ptr(dgx), ptr(dU), ptr(db_r), ptr(dh0), ptr(ws), ws.numel(), stream()), "gru_bwd")
+    return dgx if n_gx else None, dU, db_r, dh0, None, None, None
+
+
+def gru(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, bias: Optional[torch.Tensor] = None,
+        initial_state: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None,
+        return_sequences: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+  """tf.keras.layers.GRU(reset_after=True) over x [B, T, D]: returns (output, h_T), output = [B, T, u] every h_t with
+  `return_sequences`, else h_T [B, u].  kernel W [D, 3u], recurrent_kernel U [u, 3u] and bias [2, 3u] = (b_i, b_r) as
+  Keras stores them, columns (z, r, h); initial_state h_0 [B, u] (zeros when None); mask [B, T] bool / int32 / int64
+  (nonzero = kept): a masked step carries h unchanged.  gx = x.W + b_i is one K6 Dense call (ops.dense), the T steps are
+  one K19 launch; the backward is K19's reverse launch plus K6's backward for the projection and for dU, db_r.
+  Differentiable in x, all three weights and initial_state."""
+  require_cuda(x, "inputs")
+  if x.dim() != 3:
+    raise ValueError(f"gru: inputs must be [batch, timesteps, features], got shape {tuple(x.shape)}")
+  B, T, D = x.shape
+  if T == 0:
+    raise ValueError("gru: the inputs have no time steps (T = 0)")
+  require_cuda(recurrent_kernel, "recurrent_kernel")
+  u = recurrent_kernel.shape[0] if recurrent_kernel.dim() == 2 else 0
+  if recurrent_kernel.dim() != 2 or recurrent_kernel.shape[1] != 3 * u or u == 0:
+    raise ValueError(f"gru: recurrent_kernel must be [units, 3 * units], got {tuple(recurrent_kernel.shape)}")
+  if u > GRU_MAX_UNITS:
+    raise ValueError(f"gru: units = {u} is above the kernel's ceiling of {GRU_MAX_UNITS}")
+  if tuple(kernel.shape) != (D, 3 * u):
+    raise ValueError(f"gru: kernel must be [{D}, {3 * u}], got {tuple(kernel.shape)}")
+  if bias is not None and tuple(bias.shape) != (2, 3 * u):
+    raise ValueError(f"gru: bias must be [2, {3 * u}] (reset_after=True), got {tuple(bias.shape)}")
+  if initial_state is not None and tuple(initial_state.shape) != (B, u):
+    raise ValueError(f"gru: initial_state must be [{B}, {u}], got {tuple(initial_state.shape)}")
+  if mask is not None and return_sequences:
+    raise NotImplementedError("gru: a mask together with return_sequences=True is not supported")
+  m, mk = _mask_arg(mask, B, T, "gru")
+  gx = dense(x.reshape(B * T, D), kernel, None if bias is None else bias[0]).reshape(B, T, 3 * u)
+  U = f32c(recurrent_kernel, "recurrent_kernel")
+  b_r = None if bias is None else f32c(bias[1], "bias")
+  h0 = None if initial_state is None else f32c(initial_state, "initial_state")
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, b_r, h0)):
+    out = _GRURecurrence.apply(gx, U, b_r, h0, m, mk, bool(return_sequences))
+    return out if return_sequences else (out, out)
+  seq, h_last, _, _ = _gru_fwd(gx.detach(), U.detach(), None if b_r is None else b_r.detach(),
+                               None if h0 is None else h0.detach(), m, mk, bool(return_sequences), False)
+  return (seq if return_sequences else h_last), h_last
