@@ -873,6 +873,39 @@ int tfrs_gru_bwd_f32(const float* U, const float* gates, const float* h_prev, co
                      const float* g_seq, const float* g_last, int64_t B, int64_t T, int units, float* dgx, float* dU,
                      float* db_r, float* dh0, void* ws, size_t ws_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K20 LSTM recurrence: tf.keras.layers.LSTM(units) with the TF2 defaults (tanh / sigmoid, implementation=2), the cell
+ * users put in the sequential retrieval tutorial's query tower instead of the GRU.  Weights as Keras stores them,
+ * columns ordered (i, f, c, o): kernel W [D, 4u], recurrent_kernel U [u, 4u], bias b [4u].  The input projection
+ * gx = x.W + b ([B*T, 4u], row b*T + t) is the caller's, on K6 (tfrs_dense_fwd_f32 / tfrs_dense_bwd_f32).
+ *   z = gx + h_{t-1}.U (fmaf chain over k ascending from +0.0f, then added to gx);  i = sigmoid(z_i), f = sigmoid(z_f),
+ *   g = tanh(z_c), o = sigmoid(z_o);  c_t = f c_{t-1} + i g,  h_t = o tanh(c_t);  sigmoid = 1 / (1 + expf(-x)).
+ * h_0 = h0 [B, u] and c_0 = c0 [B, u], each zeros when NULL.  mask [B, T] (TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero =
+ * kept, nullable): at a masked step h_t = h_{t-1}, c_t = c_{t-1} and nothing is computed.  1 <= units <=
+ * TFRS_LSTM_MAX_UNITS, T >= 1, B < 2^31; B == 0 writes nothing.
+ *   tfrs_lstm_fwd_f32: h_last [B, u] = h_T and c_last [B, u] = c_T; out_seq [B, T, u] = every h_t (nullable); gates
+ *     [B, T, 4u] = (i, f, g, o), c_seq [B, T, u] = every c_t and h_prev [B, T, u] = h_{t-1} (all three or none, for the
+ *     backward; gates are not written at masked steps).  One launch.
+ *   tfrs_lstm_bwd_f32: from the upstream gradients g_seq [B, T, u] (of out_seq), g_h [B, u] (of h_last) and g_c [B, u]
+ *     (of c_last), each nullable, in reverse t with dh and dc carried:  dh += g_seq[t] (+ g_h at T-1), dc (+= g_c at
+ *     T-1);  do = dh tanh(c_t) o (1 - o);  dc += dh o (1 - tanh(c_t)^2);  di = dc g i (1 - i);  df = dc c_{t-1} f (1 - f);
+ *     dg = dc i (1 - g^2);  dz = [di | df | dg | do];  dh <- dz.U^T (fmaf chain over the 4u columns ascending);
+ *     dc <- dc f.  c0 is the forward's (nullable).  A masked step passes dh and dc through and writes zero dz rows.
+ *     Writes dz [B*T, 4u] (the gradient of gx), dh0 and dc0 [B, u] (each nullable) in one launch, then dU = h_prev^T .
+ *     dz (nullable; needs h_prev) with tfrs_dense_bwd_f32.  ws: tfrs_lstm_bwd_workspace_bytes, 16-byte aligned (only
+ *     read when dU is written).  No float atomics.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_LSTM_MAX_UNITS 2048
+
+int tfrs_lstm_fwd_f32(const float* gx, const float* U, const float* h0, const float* c0, const void* mask, int mask_kind,
+                      int64_t B, int64_t T, int units, float* out_seq, float* h_last, float* c_last, float* gates,
+                      float* c_seq, float* h_prev, void* stream);
+size_t tfrs_lstm_bwd_workspace_bytes(int64_t B, int64_t T, int units);
+int tfrs_lstm_bwd_f32(const float* U, const float* gates, const float* c_seq, const float* h_prev, const float* c0,
+                      const void* mask, int mask_kind, const float* g_seq, const float* g_h, const float* g_c, int64_t B,
+                      int64_t T, int units, float* dz, float* dU, float* dh0, float* dc0, void* ws, size_t ws_bytes,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -158,6 +158,10 @@ _SIGNATURES = {
     "tfrs_gru_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_l, c_l, c_i, c_p, c_p, c_p, c_p, c_p]),
     "tfrs_gru_bwd_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
     "tfrs_gru_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_l, c_l, c_i, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_lstm_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_i, c_l, c_l, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "tfrs_lstm_bwd_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
+    "tfrs_lstm_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_l, c_l, c_i, c_p, c_p, c_p, c_p, c_p,
+                                c_sz, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

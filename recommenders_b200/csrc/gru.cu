@@ -14,30 +14,9 @@
 //     one barrier per step), then dh <- dh z + dgr.U^T as the fmaf chain over the 3u columns ascending, U^T staged like U.
 //     The same C entry then runs K6's backward for dU = h_{t-1}^T . dgr and db_r = colsum(dgr).
 //   A masked step does no arithmetic: the forward carries h, the backward passes dh through and writes zero rows.
-#include "gru.cuh"
+#include "rnn.cuh"
 
 namespace tfrs {
-
-constexpr int GRU_THREADS = 256;
-constexpr int GRU_PAIRS = 8;                  // (row, unit) pairs per thread: R * JT = GRU_THREADS * GRU_PAIRS / UJ
-constexpr int GRU_SMEM_MAX = 227 * 1024;      // sm_90 opt-in dynamic shared memory per block
-constexpr int GRU_SLICE_BYTES = 64 * 1024;    // a streamed slice of U (or U^T) when the whole matrix does not fit
-
-struct GruTile {
-  int jt, g, uj, rj, rows;
-};
-
-static GruTile gru_tile(int u) {
-  GruTile t;
-  t.jt = 32;   // a power of two, so that the G = GRU_THREADS / JT row groups use every thread and no two alias a row
-  while (t.jt < u && t.jt < GRU_THREADS) t.jt *= 2;
-  t.g = GRU_THREADS / t.jt;
-  t.uj = 1;    // a power of two too, so that RJ = GRU_PAIRS / UJ is exact and names a kernel instance (gru_tiles)
-  while (t.uj * t.jt < u) t.uj *= 2;
-  t.rj = GRU_PAIRS / t.uj;
-  t.rows = t.g * t.rj;
-  return t;
-}
 
 struct GruFwdArgs {
   const float* gx; const float* U; const float* br; const float* h0; const void* mask;
@@ -51,28 +30,23 @@ struct GruBwdArgs {
   float* dgx; float* dgr; float* dh0;
 };
 
-template <typename M>
-__device__ __forceinline__ bool gru_keep(const void* mask, long long i) {
-  return mask == nullptr || static_cast<const M*>(mask)[i] != 0;
-}
-
 template <typename M, int UJ, int RJ>
-__global__ void __launch_bounds__(GRU_THREADS, 2)
+__global__ void __launch_bounds__(RNN_THREADS, 2)
 gru_fwd_kernel(const GruFwdArgs p) {
   extern __shared__ float sm[];
-  const int u = p.u, u3 = 3 * u, JT = p.jt, G = GRU_THREADS / JT, R = G * RJ;
+  const int u = p.u, u3 = 3 * u, JT = p.jt, G = RNN_THREADS / JT, R = G * RJ;
   const int j0 = threadIdx.x % JT, g = threadIdx.x / JT;
   const long long b0 = (long long)blockIdx.x * R;
   float* sU = sm + 2 * R * u;
   const bool resident = p.ks >= u;
 
-  for (int e = threadIdx.x; e < R * u; e += GRU_THREADS) {
+  for (int e = threadIdx.x; e < R * u; e += RNN_THREADS) {
     const long long b = b0 + e / u;
     sm[e] = (p.h0 && b < p.B) ? p.h0[b * u + e % u] : 0.f;
     sm[R * u + e] = 0.f;
   }
   if (resident)
-    for (int e = threadIdx.x; e < u * u3; e += GRU_THREADS) sU[e] = __ldg(p.U + e);
+    for (int e = threadIdx.x; e < u * u3; e += RNN_THREADS) sU[e] = __ldg(p.U + e);
   __syncthreads();
 
   int cur = 0;
@@ -90,7 +64,7 @@ gru_fwd_kernel(const GruFwdArgs p) {
       if (!resident) {
         __syncthreads();
         const float* src = p.U + (long long)k0 * u3;
-        for (int e = threadIdx.x; e < kn * u3; e += GRU_THREADS) sU[e] = __ldg(src + e);
+        for (int e = threadIdx.x; e < kn * u3; e += RNN_THREADS) sU[e] = __ldg(src + e);
         __syncthreads();
       }
       const float* w = resident ? sU + (long long)k0 * u3 : sU;
@@ -120,7 +94,7 @@ gru_fwd_kernel(const GruFwdArgs p) {
       const long long b = b0 + row;
       if (b >= p.B) continue;
       const long long o = b * p.T + t;
-      const bool keep = gru_keep<M>(p.mask, o);
+      const bool keep = rnn_keep<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;
@@ -131,9 +105,9 @@ gru_fwd_kernel(const GruFwdArgs p) {
           const float* gxr = p.gx + o * u3;
           float gz = acc[a][i][0], gr = acc[a][i][1], gh = acc[a][i][2];
           if (p.br) { gz += __ldg(p.br + j); gr += __ldg(p.br + u + j); gh += __ldg(p.br + 2 * u + j); }
-          const float z = gru_sigmoid(gxr[j] + gz);
-          const float r = gru_sigmoid(gxr[u + j] + gr);
-          const float hh = gru_tanh(gxr[2 * u + j] + r * gh);
+          const float z = rnn_sigmoid(gxr[j] + gz);
+          const float r = rnn_sigmoid(gxr[u + j] + gr);
+          const float hh = rnn_tanh(gxr[2 * u + j] + r * gh);
           h = z * hp + (1.f - z) * hh;
           if (p.gates) {
             float* gt = p.gates + o * 4 * u;
@@ -152,19 +126,19 @@ gru_fwd_kernel(const GruFwdArgs p) {
 }
 
 template <typename M, int UJ, int RJ>
-__global__ void __launch_bounds__(GRU_THREADS, 2)
+__global__ void __launch_bounds__(RNN_THREADS, 2)
 gru_bwd_kernel(const GruBwdArgs p) {
   extern __shared__ float sm[];
-  const int u = p.u, u3 = 3 * u, JT = p.jt, G = GRU_THREADS / JT, R = G * RJ;
+  const int u = p.u, u3 = 3 * u, JT = p.jt, G = RNN_THREADS / JT, R = G * RJ;
   const int j0 = threadIdx.x % JT, g = threadIdx.x / JT;
   const long long b0 = (long long)blockIdx.x * R;
   float* sUT = sm + 2 * R * u3;   // U^T slice: column c of U is row c of sUT, stride u + 1
   const int ld = u + 1;
   const bool resident = p.cs >= u3;
 
-  for (int e = threadIdx.x; e < 2 * R * u3; e += GRU_THREADS) sm[e] = 0.f;
+  for (int e = threadIdx.x; e < 2 * R * u3; e += RNN_THREADS) sm[e] = 0.f;
   if (resident)
-    for (long long e = threadIdx.x; e < (long long)u * u3; e += GRU_THREADS)
+    for (long long e = threadIdx.x; e < (long long)u * u3; e += RNN_THREADS)
       sUT[(e % u3) * ld + e / u3] = __ldg(p.U + e);
   __syncthreads();
 
@@ -184,7 +158,7 @@ gru_bwd_kernel(const GruBwdArgs p) {
       const long long b = b0 + row;
       const bool valid = b < p.B;
       const long long o = b * p.T + t;
-      keep[i] = valid && gru_keep<M>(p.mask, o);
+      keep[i] = valid && rnn_keep<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;
@@ -198,9 +172,9 @@ gru_bwd_kernel(const GruBwdArgs p) {
           const float* gt = p.gates + o * 4 * u;
           const float z = gt[j], r = gt[u + j], hh = gt[2 * u + j], grh = gt[3 * u + j];
           const float hp = p.h_prev[o * u + j];
-          dz = d * (hp - hh) * gru_sigmoid_grad(z);
-          dhp = d * (1.f - z) * gru_tanh_grad(hh);
-          dr = dhp * grh * gru_sigmoid_grad(r);
+          dz = d * (hp - hh) * rnn_sigmoid_grad(z);
+          dhp = d * (1.f - z) * rnn_tanh_grad(hh);
+          dr = dhp * grh * rnn_sigmoid_grad(r);
           dgh = dhp * r;
           carry[a][i] = d * z;
         } else {
@@ -224,7 +198,7 @@ gru_bwd_kernel(const GruBwdArgs p) {
       const int cn = min(p.cs, u3 - c0);
       if (!resident) {
         __syncthreads();
-        for (long long e = threadIdx.x; e < (long long)cn * u; e += GRU_THREADS) {
+        for (long long e = threadIdx.x; e < (long long)cn * u; e += RNN_THREADS) {
           const long long k = e / cn, cc = e % cn;
           sUT[cc * ld + k] = __ldg(p.U + k * u3 + c0 + cc);
         }
@@ -265,24 +239,11 @@ gru_bwd_kernel(const GruBwdArgs p) {
   }
 }
 
-// shared memory of one CTA: the fixed part plus U (forward) or U^T (backward) in slices of `per` floats per k (c) row
-static void gru_smem(int fixed_floats, int rows_total, int per, int* slice_rows, size_t* bytes) {
-  const size_t fixed = (size_t)fixed_floats * 4, whole = (size_t)rows_total * per * 4;
-  if (fixed + whole <= (size_t)GRU_SMEM_MAX) {
-    *slice_rows = rows_total;
-    *bytes = fixed + whole;
-    return;
-  }
-  int s = GRU_SLICE_BYTES / (per * 4);
-  *slice_rows = s < 1 ? 1 : s;
-  *bytes = fixed + (size_t)*slice_rows * per * 4;
-}
-
 template <typename M, int UJ, int RJ>
 struct GruFwdLaunch {
   static int run(const GruFwdArgs& a, unsigned grid, size_t smem, cudaStream_t st) {
-    TFRS_DYN_SMEM((gru_fwd_kernel<M, UJ, RJ>), GRU_SMEM_MAX);
-    gru_fwd_kernel<M, UJ, RJ><<<grid, GRU_THREADS, smem, st>>>(a);
+    TFRS_DYN_SMEM((gru_fwd_kernel<M, UJ, RJ>), RNN_SMEM_MAX);
+    gru_fwd_kernel<M, UJ, RJ><<<grid, RNN_THREADS, smem, st>>>(a);
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }
@@ -291,42 +252,12 @@ struct GruFwdLaunch {
 template <typename M, int UJ, int RJ>
 struct GruBwdLaunch {
   static int run(const GruBwdArgs& a, unsigned grid, size_t smem, cudaStream_t st) {
-    TFRS_DYN_SMEM((gru_bwd_kernel<M, UJ, RJ>), GRU_SMEM_MAX);
-    gru_bwd_kernel<M, UJ, RJ><<<grid, GRU_THREADS, smem, st>>>(a);
+    TFRS_DYN_SMEM((gru_bwd_kernel<M, UJ, RJ>), RNN_SMEM_MAX);
+    gru_bwd_kernel<M, UJ, RJ><<<grid, RNN_THREADS, smem, st>>>(a);
     TFRS_LAUNCH_CHECK();
     return TFRS_OK;
   }
 };
-
-// L<M, UJ, RJ>::run for the tile of u (UJ units per thread, RJ = GRU_PAIRS / UJ rows)
-template <template <typename, int, int> class L, typename M, typename A>
-static int gru_tiles(int uj, const A& a, unsigned grid, size_t smem, cudaStream_t st) {
-  switch (uj) {
-    case 1: return L<M, 1, 8>::run(a, grid, smem, st);
-    case 2: return L<M, 2, 4>::run(a, grid, smem, st);
-    case 4: return L<M, 4, 2>::run(a, grid, smem, st);
-    case 8: return L<M, 8, 1>::run(a, grid, smem, st);
-  }
-  set_error("gru: no kernel instance for %d units per thread", uj);
-  return TFRS_ERR_INVALID_ARG;
-}
-
-// ... and for the mask's element type (no mask runs the BOOL instance with a NULL mask)
-template <template <typename, int, int> class L, typename A>
-static int gru_dispatch(int mask_kind, int uj, const A& a, unsigned grid, size_t smem, cudaStream_t st) {
-  if (!a.mask || mask_kind == TFRS_BOOL) return gru_tiles<L, uint8_t>(uj, a, grid, smem, st);
-  if (mask_kind == TFRS_I32) return gru_tiles<L, int32_t>(uj, a, grid, smem, st);
-  return gru_tiles<L, long long>(uj, a, grid, smem, st);
-}
-
-static int gru_check(const char* what, int64_t B, int64_t T, int u, const void* mask, int mask_kind) {
-  TFRS_CHECK_ARG(B >= 0 && B < (1ll << 31) && T >= 1 && T < (1ll << 31) && u >= 1 && u <= TFRS_GRU_MAX_UNITS,
-                 "%s: bad shape B=%lld T=%lld units=%d (1 <= units <= %d, T >= 1)", what, (long long)B, (long long)T, u,
-                 TFRS_GRU_MAX_UNITS);
-  TFRS_CHECK_ARG(!mask || mask_kind == TFRS_I32 || mask_kind == TFRS_I64 || mask_kind == TFRS_BOOL,
-                 "%s: the mask must be I32, I64 or BOOL", what);
-  return TFRS_OK;
-}
 
 }  // namespace tfrs
 using namespace tfrs;
@@ -334,17 +265,17 @@ using namespace tfrs;
 extern "C" int tfrs_gru_fwd_f32(const float* gx, const float* U, const float* b_r, const float* h0, const void* mask,
                                 int mask_kind, int64_t B, int64_t T, int units, float* out_seq, float* h_last, float* gates,
                                 float* h_prev, void* stream) {
-  int rc = gru_check("gru_fwd", B, T, units, mask, mask_kind);
+  int rc = rnn_check("gru_fwd", B, T, units, TFRS_GRU_MAX_UNITS, mask, mask_kind);
   if (rc) return rc;
   if (B == 0) return TFRS_OK;
   TFRS_CHECK_ARG(gx && U && h_last, "gru_fwd: NULL pointer");
   TFRS_CHECK_ARG(!gates == !h_prev, "gru_fwd: gates and h_prev are saved together");
-  const GruTile tl = gru_tile(units);
+  const RnnTile tl = rnn_tile(units);
   GruFwdArgs a{gx, U, b_r, h0, mask, B, T, units, tl.jt, 0, out_seq, h_last, gates, h_prev};
   size_t smem;
-  gru_smem(2 * tl.rows * units, units, 3 * units, &a.ks, &smem);
+  rnn_smem(2 * tl.rows * units, units, 3 * units, &a.ks, &smem);
   const unsigned grid = (unsigned)ceil_div(B, tl.rows);
-  return gru_dispatch<GruFwdLaunch>(mask_kind, tl.uj, a, grid, smem, (cudaStream_t)stream);
+  return rnn_dispatch<GruFwdLaunch>("gru_fwd", mask_kind, tl.uj, a, grid, smem, (cudaStream_t)stream);
 }
 
 extern "C" size_t tfrs_gru_bwd_workspace_bytes(int64_t B, int64_t T, int units) {
@@ -356,7 +287,7 @@ extern "C" size_t tfrs_gru_bwd_workspace_bytes(int64_t B, int64_t T, int units) 
 extern "C" int tfrs_gru_bwd_f32(const float* U, const float* gates, const float* h_prev, const void* mask, int mask_kind,
                                 const float* g_seq, const float* g_last, int64_t B, int64_t T, int units, float* dgx,
                                 float* dU, float* db_r, float* dh0, void* ws, size_t ws_bytes, void* stream) {
-  int rc = gru_check("gru_bwd", B, T, units, mask, mask_kind);
+  int rc = rnn_check("gru_bwd", B, T, units, TFRS_GRU_MAX_UNITS, mask, mask_kind);
   if (rc) return rc;
   if (B == 0) return TFRS_OK;
   TFRS_CHECK_ARG(U && gates && h_prev && dgx, "gru_bwd: NULL pointer");
@@ -366,12 +297,12 @@ extern "C" int tfrs_gru_bwd_f32(const float* U, const float* gates, const float*
   const long long n = (long long)B * T;
   float* dgr = (float*)ws;
   unsigned char* kws = (unsigned char*)ws + align_up((size_t)n * 3 * units * 4, 1024);
-  const GruTile tl = gru_tile(units);
+  const RnnTile tl = rnn_tile(units);
   GruBwdArgs a{U, gates, h_prev, mask, g_seq, g_last, B, T, units, tl.jt, 0, dgx, dgr, dh0};
   size_t smem;
-  gru_smem(2 * tl.rows * 3 * units, 3 * units, units + 1, &a.cs, &smem);
+  rnn_smem(2 * tl.rows * 3 * units, 3 * units, units + 1, &a.cs, &smem);
   const unsigned grid = (unsigned)ceil_div(B, tl.rows);
-  rc = gru_dispatch<GruBwdLaunch>(mask_kind, tl.uj, a, grid, smem, (cudaStream_t)stream);
+  rc = rnn_dispatch<GruBwdLaunch>("gru_bwd", mask_kind, tl.uj, a, grid, smem, (cudaStream_t)stream);
   if (rc || (!dU && !db_r)) return rc;
   // dU = h_prev^T . dgr, db_r = colsum(dgr): K6's backward of a linear layer whose output gradient is dgr
   return tfrs_dense_bwd_f32(h_prev, U, dgr, dgr, nullptr, n, units, 3 * units, TFRS_ACT_LINEAR, nullptr, dU, db_r, kws,

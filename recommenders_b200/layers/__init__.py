@@ -10,4 +10,4 @@ from . import recurrent
 from .feature_interaction import dcn
 from .pooling import GlobalAveragePooling1D
 from .preprocessing import Discretization, Hashing, IntegerLookup, Normalization, StringLookup, TextVectorization
-from .recurrent import GRU
+from .recurrent import GRU, LSTM

@@ -2212,3 +2212,103 @@ def gru(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, b
   seq, h_last, _, _ = _gru_fwd(gx.detach(), U.detach(), None if b_r is None else b_r.detach(),
                                None if h0 is None else h0.detach(), m, mk, bool(return_sequences), False)
   return (seq if return_sequences else h_last), h_last
+
+
+# ------------------------------------------------------------------------------------------------
+# K20 LSTM recurrence: layers.LSTM; the input projection runs on K6
+# ------------------------------------------------------------------------------------------------
+LSTM_MAX_UNITS = 2048   # TFRS_LSTM_MAX_UNITS of include/tfrs_b200.h
+
+
+def _lstm_fwd(gx, U, h0, c0, m, mk, return_sequences: bool, save: bool):
+  B, T, u4 = gx.shape
+  u = u4 // 4
+  new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=gx.device)
+  seq = new(B, T, u) if return_sequences else None
+  h_last, c_last = new(B, u), new(B, u)
+  gates, c_seq, h_prev = (new(B, T, 4 * u), new(B, T, u), new(B, T, u)) if save else (None, None, None)
+  check(lib().tfrs_lstm_fwd_f32(ptr(gx), ptr(U), ptr(h0), ptr(c0), ptr(m), mk, B, T, u, ptr(seq), ptr(h_last),
+                                ptr(c_last), ptr(gates), ptr(c_seq), ptr(h_prev), stream()), "lstm_fwd")
+  return seq, h_last, c_last, gates, c_seq, h_prev
+
+
+class _LSTMRecurrence(torch.autograd.Function):
+  """(out_seq, h_T, c_T) with return_sequences, else (h_T, c_T), from gx = x.W + b [B, T, 4u]; differentiable in gx, U,
+  h0 and c0."""
+
+  @staticmethod
+  def forward(ctx, gx, U, h0, c0, m, mk, return_sequences):
+    seq, h_last, c_last, gates, c_seq, h_prev = _lstm_fwd(gx, U, h0, c0, m, mk, return_sequences, True)
+    ctx.save_for_backward(U, gates, c_seq, h_prev, c0, m)
+    ctx.mk, ctx.return_sequences = mk, return_sequences
+    ctx.set_materialize_grads(False)
+    return (seq, h_last, c_last) if return_sequences else (h_last, c_last)
+
+  @staticmethod
+  def backward(ctx, *grads):
+    U, gates, c_seq, h_prev, c0, m = ctx.saved_tensors
+    g_seq, g_h, g_c = grads if ctx.return_sequences else (None, *grads)
+    B, T, u = h_prev.shape
+    n_gx, n_U, n_h0, n_c0 = ctx.needs_input_grad[:4]
+    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=U.device)
+    dz = new(B, T, 4 * u)
+    dU = new(u, 4 * u) if n_U else None
+    dh0 = new(B, u) if n_h0 else None
+    dc0 = new(B, u) if n_c0 else None
+    if B == 0 or (g_seq is None and g_h is None and g_c is None):
+      for t in (dz, dU, dh0, dc0):
+        if t is not None:
+          t.zero_()
+    else:
+      g_seq, g_h, g_c = (None if g is None else f32c(g, "grad") for g in (g_seq, g_h, g_c))
+      ws = workspace(lib().tfrs_lstm_bwd_workspace_bytes(B, T, u), U.device, "lstm_bwd")
+      check(lib().tfrs_lstm_bwd_f32(ptr(U), ptr(gates), ptr(c_seq), ptr(h_prev), ptr(c0), ptr(m), ctx.mk, ptr(g_seq),
+                                    ptr(g_h), ptr(g_c), B, T, u, ptr(dz), ptr(dU), ptr(dh0), ptr(dc0), ptr(ws),
+                                    ws.numel(), stream()), "lstm_bwd")
+    return dz if n_gx else None, dU, dh0, dc0, None, None, None
+
+
+def lstm(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, bias: Optional[torch.Tensor] = None,
+         initial_state: Optional[Sequence[torch.Tensor]] = None, mask: Optional[torch.Tensor] = None,
+         return_sequences: bool = False) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+  """tf.keras.layers.LSTM over x [B, T, D]: returns (output, h_T, c_T), output = [B, T, u] every h_t with
+  `return_sequences`, else h_T [B, u].  kernel W [D, 4u], recurrent_kernel U [u, 4u] and bias [4u] as Keras stores them,
+  columns (i, f, c, o); initial_state (h_0, c_0), each [B, u] (zeros when None); mask [B, T] bool / int32 / int64
+  (nonzero = kept): a masked step carries h and c unchanged.  gx = x.W + b is one K6 Dense call (ops.dense), the T steps
+  are one K20 launch; the backward is K20's reverse launch plus K6's backward for the projection and for dU.
+  Differentiable in x, all three weights and both initial states."""
+  require_cuda(x, "inputs")
+  if x.dim() != 3:
+    raise ValueError(f"lstm: inputs must be [batch, timesteps, features], got shape {tuple(x.shape)}")
+  B, T, D = x.shape
+  if T == 0:
+    raise ValueError("lstm: the inputs have no time steps (T = 0)")
+  require_cuda(recurrent_kernel, "recurrent_kernel")
+  u = recurrent_kernel.shape[0] if recurrent_kernel.dim() == 2 else 0
+  if recurrent_kernel.dim() != 2 or recurrent_kernel.shape[1] != 4 * u or u == 0:
+    raise ValueError(f"lstm: recurrent_kernel must be [units, 4 * units], got {tuple(recurrent_kernel.shape)}")
+  if u > LSTM_MAX_UNITS:
+    raise ValueError(f"lstm: units = {u} is above the kernel's ceiling of {LSTM_MAX_UNITS}")
+  if tuple(kernel.shape) != (D, 4 * u):
+    raise ValueError(f"lstm: kernel must be [{D}, {4 * u}], got {tuple(kernel.shape)}")
+  if bias is not None and tuple(bias.shape) != (4 * u,):
+    raise ValueError(f"lstm: bias must be [{4 * u}], got {tuple(bias.shape)}")
+  h0 = c0 = None
+  if initial_state is not None:
+    if isinstance(initial_state, torch.Tensor) or len(initial_state) != 2:
+      raise ValueError("lstm: initial_state must be the pair (h_0, c_0)")
+    for name, s in zip(("h_0", "c_0"), initial_state):
+      if tuple(s.shape) != (B, u):
+        raise ValueError(f"lstm: initial_state {name} must be [{B}, {u}], got {tuple(s.shape)}")
+    h0, c0 = (f32c(s, "initial_state") for s in initial_state)
+  if mask is not None and return_sequences:
+    raise NotImplementedError("lstm: a mask together with return_sequences=True is not supported")
+  m, mk = _mask_arg(mask, B, T, "lstm")
+  gx = dense(x.reshape(B * T, D), kernel, bias).reshape(B, T, 4 * u)
+  U = f32c(recurrent_kernel, "recurrent_kernel")
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, h0, c0)):
+    out = _LSTMRecurrence.apply(gx, U, h0, c0, m, mk, bool(return_sequences))
+    return out if return_sequences else (out[0], out[0], out[1])
+  seq, h_last, c_last, _, _, _ = _lstm_fwd(gx.detach(), U.detach(), None if h0 is None else h0.detach(),
+                                           None if c0 is None else c0.detach(), m, mk, bool(return_sequences), False)
+  return (seq if return_sequences else h_last), h_last, c_last
