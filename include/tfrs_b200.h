@@ -906,6 +906,56 @@ int tfrs_lstm_bwd_f32(const float* U, const float* gates, const float* c_seq, co
                       int64_t T, int units, float* dz, float* dU, float* dh0, float* dc0, void* ws, size_t ws_bytes,
                       void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K21 attention core: tf.keras.layers.MultiHeadAttention between its projections (attention over the sequence axis, no
+ * dropout).  The caller projects with K6 (tfrs_dense_fwd_f32): Q [B, T, H*dk], K [B, S, H*dk], V [B, S, H*dv], head h
+ * in columns h*d .. h*d + d - 1, contiguous; they are read in place.  1 <= dk, dv <= TFRS_MHA_MAX_HEAD_DIM, T, S >= 1.
+ *   scores s = (Q_h * scale) . K_h^T with scale = (float)(1 / sqrt(dk)) applied to Q in fp32 (Keras's order); where the
+ *   combined mask drops (b, t, s), s += -1e9f (tf-keras Softmax), so a fully masked row is uniform; P = softmax over s;
+ *   O_h = P . V_h.  masks (nullable; each mask pointer nullable, nonzero = kept, kinds TFRS_I32 / TFRS_I64 / TFRS_BOOL):
+ *   query [B, T], value [B, S], key [B, S], attention [B, T, S], causal (keeps s <= t), combined by AND.
+ *   tfrs_mha_fwd_f32: O [B, T, H*dv]; stats [B, H, T, 2] = (row max m, row sum l of e^{s - m}) -- the log-sum-exp
+ *     m + log l, kept as two numbers because a fully masked row's m = -1e9 leaves no fp32 room for log l (nullable; the
+ *     backward needs it); P [B, H, T, S] = e^{s - m} / l (nullable).  One launch.
+ *   tfrs_mha_bwd_f32: from dO [B, T, H*dv] and the forward's O and stats: dQ, dK, dV (the gradients of the projected Q,
+ *     K, V).  Three launches: delta = rowsum(dO * O); dK, dV per key row (P recomputed from stats); dQ per query row.
+ *     ws: tfrs_mha_bwd_workspace_bytes, 16-byte aligned.  Fixed summation order, no float atomics.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_MHA_MAX_HEAD_DIM 128
+
+typedef struct TfrsMhaMasks {
+  const void* query; int query_kind;
+  const void* value; int value_kind;
+  const void* key; int key_kind;
+  const void* attention; int attention_kind;
+  int causal;
+} TfrsMhaMasks;
+
+int tfrs_mha_fwd_f32(const float* Q, const float* K, const float* V, const TfrsMhaMasks* masks, int64_t B, int64_t T,
+                     int64_t S, int H, int dk, int dv, float* O, float* stats, float* P, void* stream);
+size_t tfrs_mha_bwd_workspace_bytes(int64_t B, int64_t T, int H);
+int tfrs_mha_bwd_f32(const float* Q, const float* K, const float* V, const TfrsMhaMasks* masks, const float* O,
+                     const float* stats, const float* dO, int64_t B, int64_t T, int64_t S, int H, int dk, int dv,
+                     float* dQ, float* dK, float* dV, void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * K22 layer normalization: tf.keras.layers.LayerNormalization(axis=-1) over the rows of x [N, d] (d >= 1).
+ *   mean = hi + lo with hi = sum(x) / d and lo = sum(x - hi) / d; var = sum((x - hi)^2) / d - lo^2 (population
+ *   variance, corrected two-pass); rstd = 1 / sqrtf(var + eps); y = ((x - hi) - lo) * rstd * gamma + beta, gamma / beta
+ *   [d] nullable (scale / center off).  Keeping the mean as the pair (hi, lo) keeps x - mean exact where |mean| >> std.
+ *   tfrs_layer_norm_fwd_f32: y [N, d]; mean [N, 2] = (hi, lo) and rstd [N] (nullable together; the backward needs
+ *     them).  One launch.
+ *   tfrs_layer_norm_bwd_f32: from dy: dx [N, d] = rstd (g - mean(g) - xhat mean(g xhat)) with g = dy * gamma and
+ *     xhat = ((x - hi) - lo) rstd; dparams [2, d] = (sum_rows dy xhat, sum_rows dy) = (dgamma, dbeta) (nullable) from
+ *     per-CTA partials folded in fixed order by a second launch.  ws: tfrs_layer_norm_bwd_workspace_bytes, 16-byte
+ *     aligned.  No float atomics.
+ * ------------------------------------------------------------------------------------------- */
+int tfrs_layer_norm_fwd_f32(const float* x, const float* gamma, const float* beta, int64_t N, int64_t d, float eps,
+                            float* y, float* mean, float* rstd, void* stream);
+size_t tfrs_layer_norm_bwd_workspace_bytes(int64_t N, int64_t d);
+int tfrs_layer_norm_bwd_f32(const float* x, const float* gamma, const float* mean, const float* rstd, const float* dy,
+                            int64_t N, int64_t d, float* dx, float* dparams, void* ws, size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

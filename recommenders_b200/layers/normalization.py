@@ -1,0 +1,76 @@
+"""`LayerNormalization`, the normalization of Transformer blocks: tf.keras.layers.LayerNormalization over the last axis
+on K22.  DESIGN.md §2 (A25) pins its rule."""
+from __future__ import annotations
+
+from typing import Any, Dict
+
+import torch
+
+from .. import ops
+from .feature_interaction.dcn import _init
+
+
+class LayerNormalization(torch.nn.Module):
+  """`tf.keras.layers.LayerNormalization()`: y = (x - mean) * rsqrt(var + epsilon) * gamma + beta over the last axis of x
+  (float32), with the population variance.  gamma [d] ("ones") and beta [d] ("zeros") are created on the first call;
+  `scale=False` / `center=False` leave them out.  A mask attached to x (an `Embedding(mask_zero=True)` output) is
+  attached to y too.  Any axis but the last, regularizers and constraints raise NotImplementedError."""
+
+  def __init__(self, axis=-1, epsilon: float = 1e-3, center: bool = True, scale: bool = True,
+               beta_initializer="zeros", gamma_initializer="ones", beta_regularizer=None, gamma_regularizer=None,
+               beta_constraint=None, gamma_constraint=None, name=None, **kwargs):
+    super().__init__()
+    unsupported = {
+        "beta_regularizer": beta_regularizer is not None,
+        "gamma_regularizer": gamma_regularizer is not None,
+        "beta_constraint": beta_constraint is not None,
+        "gamma_constraint": gamma_constraint is not None,
+    }
+    for arg, bad in unsupported.items():
+      if bad:
+        raise NotImplementedError(f"LayerNormalization: {arg}={locals()[arg]!r} is not supported")
+    self.axis = list(axis) if isinstance(axis, (list, tuple)) else axis
+    if isinstance(self.axis, list) and len(self.axis) != 1:
+      raise NotImplementedError(f"LayerNormalization: axis={axis!r} is not supported (the last axis only)")
+    self.epsilon, self.center, self.scale = float(epsilon), bool(center), bool(scale)
+    self._beta_initializer, self._gamma_initializer = beta_initializer, gamma_initializer
+    self.name = name
+    self.built = False
+
+  def _check_axis(self, rank: int) -> None:
+    a = self.axis[0] if isinstance(self.axis, list) else self.axis
+    if a not in (-1, rank - 1):
+      raise NotImplementedError(f"LayerNormalization: axis={self.axis!r} is not supported (the last axis only)")
+
+  def build(self, input_shape, device=None):
+    self._check_axis(len(input_shape))
+    d = int(input_shape[-1])
+    device = device or torch.device("cuda", torch.cuda.current_device())
+    self.gamma = torch.nn.Parameter(_init(self._gamma_initializer, (d,), device)) if self.scale else None
+    self.beta = torch.nn.Parameter(_init(self._beta_initializer, (d,), device)) if self.center else None
+    self.built = True
+
+  def call(self, inputs: torch.Tensor, training=None):
+    if not isinstance(inputs, torch.Tensor):
+      raise TypeError(f"LayerNormalization: inputs must be a torch.Tensor, got {type(inputs)}")
+    if not self.built:
+      self.build(inputs.shape, inputs.device)
+    self._check_axis(inputs.dim())
+    mask = ops.attached_mask(inputs)
+    y = ops.layer_norm(inputs, self.gamma, self.beta, self.epsilon)
+    if mask is not None:
+      y._tfrs_mask = (mask, y._version, y.data_ptr())
+    return y
+
+  def forward(self, inputs, training=None):
+    return self.call(inputs, training=training)
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"axis": self.axis, "epsilon": self.epsilon, "center": self.center, "scale": self.scale,
+            "beta_initializer": self._beta_initializer, "gamma_initializer": self._gamma_initializer,
+            "beta_regularizer": None, "gamma_regularizer": None, "beta_constraint": None, "gamma_constraint": None,
+            "name": self.name}
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)

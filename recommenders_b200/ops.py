@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _ffi
-from ._ffi import c_f, c_i, c_l, c_sz, check, f32c, lib, ptr, require_cuda, stream, workspace
+from ._ffi import c_f, c_i, c_l, c_p, c_sz, check, f32c, lib, ptr, require_cuda, stream, workspace
 
 # Corpora at least this large go through the tensor-core screening path when an index image exists.
 TC_MIN_N = 16384
@@ -2312,3 +2312,216 @@ def lstm(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, 
   seq, h_last, c_last, _, _, _ = _lstm_fwd(gx.detach(), U.detach(), None if h0 is None else h0.detach(),
                                            None if c0 is None else c0.detach(), m, mk, bool(return_sequences), False)
   return (seq if return_sequences else h_last), h_last, c_last
+
+
+# ------------------------------------------------------------------------------------------------
+# K21 attention core: layers.MultiHeadAttention; the four projections run on K6
+# ------------------------------------------------------------------------------------------------
+MHA_MAX_HEAD_DIM = 128   # TFRS_MHA_MAX_HEAD_DIM of include/tfrs_b200.h
+
+
+class _MhaMasks(ctypes.Structure):
+  _fields_ = [("query", c_p), ("query_kind", c_i), ("value", c_p), ("value_kind", c_i), ("key", c_p), ("key_kind", c_i),
+              ("attention", c_p), ("attention_kind", c_i), ("causal", c_i)]
+
+
+def _mha_mask(mask, shape, name: str):
+  if mask is None:
+    return None
+  require_cuda(mask, name)
+  if mask.dtype not in _MASK_KINDS:
+    raise TypeError(f"attention: {name} must be bool, int32 or int64, got {mask.dtype}")
+  if tuple(mask.shape) != tuple(shape):
+    raise ValueError(f"attention: {name} has shape {tuple(mask.shape)}, expected {list(shape)}")
+  return mask.contiguous()
+
+
+def _mha_masks(masks, causal: bool) -> _MhaMasks:
+  s = _MhaMasks()
+  for name, m in zip(("query", "value", "key", "attention"), masks):
+    setattr(s, name, None if m is None else m.data_ptr())
+    setattr(s, name + "_kind", _MASK_KINDS[m.dtype] if m is not None else 0)
+  s.causal = int(bool(causal))
+  return s
+
+
+def _attention_fwd(Q, K, V, H, dk, dv, masks, causal, want_p, save):
+  B, T, S = Q.shape[0], Q.shape[1], K.shape[1]
+  O = torch.empty((B, T, H * dv), dtype=torch.float32, device=Q.device)
+  stats = torch.empty((B, H, T, 2), dtype=torch.float32, device=Q.device) if save else None
+  P = torch.empty((B, H, T, S), dtype=torch.float32, device=Q.device) if want_p else None
+  m = _mha_masks(masks, causal)
+  check(lib().tfrs_mha_fwd_f32(ptr(Q), ptr(K), ptr(V), ctypes.byref(m), B, T, S, H, dk, dv, ptr(O), ptr(stats), ptr(P),
+                               stream()), "mha_fwd")
+  return O, stats, P
+
+
+class _AttentionCore(torch.autograd.Function):
+  """(O [B, T, H*dv], P [B, H, T, S] or an empty tensor) from the projected Q, K, V; differentiable in Q, K and V.  P is
+  not differentiable."""
+
+  @staticmethod
+  def forward(ctx, Q, K, V, H, dk, dv, qm, vm, km, am, causal, want_p):
+    O, stats, P = _attention_fwd(Q, K, V, H, dk, dv, (qm, vm, km, am), causal, want_p, True)
+    P = P if want_p else torch.empty((0,), dtype=torch.float32, device=Q.device)
+    ctx.save_for_backward(Q, K, V, O, stats, qm, vm, km, am)
+    ctx.shape, ctx.causal = (H, dk, dv), causal
+    ctx.mark_non_differentiable(P)
+    ctx.set_materialize_grads(False)
+    return O, P
+
+  @staticmethod
+  def backward(ctx, dO, _dP):
+    Q, K, V, O, stats, qm, vm, km, am = ctx.saved_tensors
+    H, dk, dv = ctx.shape
+    B, T, S = Q.shape[0], Q.shape[1], K.shape[1]
+    dQ, dK, dV = torch.empty_like(Q), torch.empty_like(K), torch.empty_like(V)
+    if dO is None or B == 0:
+      for t in (dQ, dK, dV):
+        t.zero_()
+    else:
+      dO = f32c(dO, "grad")
+      m = _mha_masks((qm, vm, km, am), ctx.causal)
+      ws = workspace(lib().tfrs_mha_bwd_workspace_bytes(B, T, H), Q.device, "mha_bwd")
+      check(lib().tfrs_mha_bwd_f32(ptr(Q), ptr(K), ptr(V), ctypes.byref(m), ptr(O), ptr(stats), ptr(dO), B, T, S, H, dk,
+                                   dv, ptr(dQ), ptr(dK), ptr(dV), ptr(ws), ws.numel(), stream()), "mha_bwd")
+    n = ctx.needs_input_grad
+    return (dQ if n[0] else None, dK if n[1] else None, dV if n[2] else None) + (None,) * 9
+
+
+def attention_core(Q: torch.Tensor, K: torch.Tensor, V: torch.Tensor, num_heads: int, query_mask=None, value_mask=None,
+                   key_mask=None, attention_mask=None, causal: bool = False, return_scores: bool = False):
+  """K21 on projected tensors: Q [B, T, H*dk], K [B, S, H*dk], V [B, S, H*dv] (float32, CUDA) -> (O [B, T, H*dv],
+  P [B, H, T, S] with `return_scores`, else None).  scores = (Q_h * (1/sqrt(dk))) . K_h^T; where the combined mask
+  (query_mask [B, T] & value_mask [B, S] & key_mask [B, S] & the causal triangle s <= t & attention_mask [B, T, S];
+  bool / int32 / int64, nonzero = kept) drops a score, -1e9 is added in fp32, as tf-keras's Softmax does.  One launch
+  forward, three backward.  Differentiable in Q, K and V; P is returned detached (non-differentiable)."""
+  for t, name in ((Q, "query"), (K, "key"), (V, "value")):
+    require_cuda(t, name)
+    if t.dim() != 3:
+      raise ValueError(f"attention: the projected {name} must be [batch, length, heads * dim], got {tuple(t.shape)}")
+  H = int(num_heads)
+  B, T, S = Q.shape[0], Q.shape[1], K.shape[1]
+  if H < 1 or Q.shape[2] % H or V.shape[2] % H:
+    raise ValueError(f"attention: {H} heads do not divide the widths {Q.shape[2]} and {V.shape[2]}")
+  dk, dv = Q.shape[2] // H, V.shape[2] // H
+  if tuple(K.shape) != (B, S, H * dk) or V.shape[:2] != (B, S):
+    raise ValueError(f"attention: key {tuple(K.shape)} and value {tuple(V.shape)} do not fit query {tuple(Q.shape)}")
+  if T == 0 or S == 0:
+    raise ValueError("attention: the query and key sequences must not be empty")
+  if not 1 <= dk <= MHA_MAX_HEAD_DIM or not 1 <= dv <= MHA_MAX_HEAD_DIM:
+    raise ValueError(f"attention: key_dim = {dk} and value_dim = {dv} must be in 1 .. {MHA_MAX_HEAD_DIM}")
+  masks = (_mha_mask(query_mask, (B, T), "query_mask"), _mha_mask(value_mask, (B, S), "value_mask"),
+           _mha_mask(key_mask, (B, S), "key_mask"), _mha_mask(attention_mask, (B, T, S), "attention_mask"))
+  Q, K, V = f32c(Q, "query"), f32c(K, "key"), f32c(V, "value")
+  if torch.is_grad_enabled() and any(t.requires_grad for t in (Q, K, V)):
+    O, P = _AttentionCore.apply(Q, K, V, H, dk, dv, *masks, bool(causal), bool(return_scores))
+    return O, (P if return_scores else None)
+  O, _, P = _attention_fwd(Q.detach(), K.detach(), V.detach(), H, dk, dv, masks, bool(causal), bool(return_scores),
+                           False)
+  return O, P
+
+
+def attention(query: torch.Tensor, value: torch.Tensor, key: Optional[torch.Tensor], query_kernel: torch.Tensor,
+              key_kernel: torch.Tensor, value_kernel: torch.Tensor, output_kernel: torch.Tensor, query_bias=None,
+              key_bias=None, value_bias=None, output_bias=None, query_mask=None, value_mask=None, key_mask=None,
+              attention_mask=None, causal: bool = False, return_scores: bool = False):
+  """tf.keras.layers.MultiHeadAttention's call on query [B, T, D_q], value [B, S, D_v] and key [B, S, D_k] (key = value
+  when None), with the weights as Keras stores them: query_kernel [D_q, H, dk], key_kernel [D_k, H, dk], value_kernel
+  [D_v, H, dv], output_kernel [H, dv, D_out], biases [H, dk] / [H, dk] / [H, dv] / [D_out] (each nullable).  Returns
+  (output [B, T, D_out], scores [B, H, T, S] with `return_scores`, else None).  The four projections are K6 Dense calls
+  on the kernels viewed as 2-D (no copies); the attention core is K21 (attention_core).  Differentiable in the three
+  inputs and all eight weights."""
+  key = value if key is None else key
+  for t, name in ((query, "query"), (value, "value"), (key, "key")):
+    require_cuda(t, name)
+    if t.dim() != 3:
+      raise NotImplementedError(f"attention: {name} must have rank 3 [batch, length, features], got {tuple(t.shape)}")
+  if query_kernel.dim() != 3 or key_kernel.dim() != 3 or value_kernel.dim() != 3 or output_kernel.dim() != 3:
+    raise ValueError("attention: the query / key / value / output kernels must be 3-D")
+  _, H, dk = query_kernel.shape
+  dv = value_kernel.shape[2]
+  checks = ((query_kernel, (query.shape[2], H, dk)), (key_kernel, (key.shape[2], H, dk)),
+            (value_kernel, (value.shape[2], H, dv)), (output_kernel, (H, dv, output_kernel.shape[2])))
+  for w, shape in checks:
+    if tuple(w.shape) != tuple(shape):
+      raise ValueError(f"attention: a kernel has shape {tuple(w.shape)}, expected {list(shape)}")
+  if key.shape[:2] != value.shape[:2] or key.shape[0] != query.shape[0]:
+    raise ValueError(f"attention: query {tuple(query.shape)}, value {tuple(value.shape)} and key {tuple(key.shape)} "
+                     "must share the batch, and key and value the length")
+  B, T, S = query.shape[0], query.shape[1], value.shape[1]
+  flat = lambda w, rows: w.reshape(rows, -1)
+  vec = lambda b: None if b is None else b.reshape(-1)
+  Q = dense(query.reshape(B * T, -1), flat(query_kernel, query.shape[2]), vec(query_bias)).reshape(B, T, H * dk)
+  K = dense(key.reshape(B * S, -1), flat(key_kernel, key.shape[2]), vec(key_bias)).reshape(B, S, H * dk)
+  V = dense(value.reshape(B * S, -1), flat(value_kernel, value.shape[2]), vec(value_bias)).reshape(B, S, H * dv)
+  O, P = attention_core(Q, K, V, H, query_mask, value_mask, key_mask, attention_mask, causal, return_scores)
+  out = dense(O.reshape(B * T, H * dv), flat(output_kernel, H * dv), output_bias).reshape(B, T, -1)
+  return out, P
+
+
+# ------------------------------------------------------------------------------------------------
+# K22 layer normalization: layers.LayerNormalization over the last axis
+# ------------------------------------------------------------------------------------------------
+def _layer_norm_fwd(x2, gamma, beta, eps, save):
+  N, d = x2.shape
+  y = torch.empty_like(x2)
+  mean = torch.empty((N, 2), dtype=torch.float32, device=x2.device) if save else None    # the pair (hi, lo)
+  rstd = torch.empty((N,), dtype=torch.float32, device=x2.device) if save else None
+  check(lib().tfrs_layer_norm_fwd_f32(ptr(x2), ptr(gamma), ptr(beta), N, d, float(eps), ptr(y), ptr(mean), ptr(rstd),
+                                      stream()), "layer_norm_fwd")
+  return y, mean, rstd
+
+
+class _LayerNorm(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, x2, gamma, beta, eps):
+    y, mean, rstd = _layer_norm_fwd(x2, gamma, beta, eps, True)
+    ctx.save_for_backward(x2, gamma, mean, rstd)
+    ctx.set_materialize_grads(False)
+    return y
+
+  @staticmethod
+  def backward(ctx, dy):
+    x2, gamma, mean, rstd = ctx.saved_tensors
+    N, d = x2.shape
+    n_x, n_g, n_b = ctx.needs_input_grad[:3]
+    dx = torch.empty_like(x2) if n_x else None
+    dparams = torch.empty((2, d), dtype=torch.float32, device=x2.device) if (n_g or n_b) else None
+    if dy is None:
+      for t in (dx, dparams):
+        if t is not None:
+          t.zero_()
+    else:
+      dy = f32c(dy, "grad")
+      ws = workspace(lib().tfrs_layer_norm_bwd_workspace_bytes(N, d), x2.device, "layer_norm_bwd")
+      check(lib().tfrs_layer_norm_bwd_f32(ptr(x2), ptr(gamma), ptr(mean), ptr(rstd), ptr(dy), N, d, ptr(dx),
+                                          ptr(dparams), ptr(ws), ws.numel(), stream()), "layer_norm_bwd")
+    return (dx, dparams[0] if n_g else None, dparams[1] if n_b else None, None)
+
+
+def layer_norm(x: torch.Tensor, gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None,
+               epsilon: float = 1e-3) -> torch.Tensor:
+  """tf.keras.layers.LayerNormalization(axis=-1): y = (x - mean) * rsqrt(var + epsilon) * gamma + beta over the last
+  axis of x (float32, CUDA), population variance, two passes, the mean kept as an fp32 pair so that x - mean stays exact
+  where |mean| >> std; gamma / beta [d] or None (scale / center off).  One K22
+  launch forward; the backward is one launch for dx and the per-CTA dgamma / dbeta partials plus a fixed-order fold.
+  Differentiable in x, gamma and beta."""
+  require_cuda(x, "inputs")
+  if x.dim() == 0:
+    raise ValueError("layer_norm: the input must have at least one axis")
+  d = x.shape[-1]
+  if d == 0:
+    raise ValueError("layer_norm: the normalized axis is empty")
+  for p, name in ((gamma, "gamma"), (beta, "beta")):
+    if p is not None and tuple(p.shape) != (d,):
+      raise ValueError(f"layer_norm: {name} must be [{d}], got {tuple(p.shape)}")
+  x2 = f32c(x, "inputs").reshape(-1, d)
+  g = None if gamma is None else f32c(gamma, "gamma")
+  b = None if beta is None else f32c(beta, "beta")
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x2, g, b)):
+    return _LayerNorm.apply(x2, g, b, float(epsilon)).reshape(x.shape)
+  y, _, _ = _layer_norm_fwd(x2.detach(), None if g is None else g.detach(), None if b is None else b.detach(), epsilon,
+                            False)
+  return y.reshape(x.shape)
