@@ -110,3 +110,50 @@ def test_constructor_checks():
   assert ftk.TreeAH().is_exact() is False
   with pytest.raises(ImportError):
     ftk.ScaNN()
+
+
+def test_plan_mirrors_at_hand_computed_points():
+  """The slice, chunk and merge-route mirrors at points worked out by hand on a 132-SM H100."""
+  assert tao.slices(1, 1, 20000, 1, 132) == 64             # min(ceil(264 / 1), 78) capped at 64
+  assert tao.slices(5, 1, 20000, 1, 132) == 53             # ceil(264 / 5)
+  assert tao.slices(1, 5, 17000, 5, 132) == 13             # 3400 rows per leaf / 256
+  assert tao.slices(1, 1, 1200, 2, 132) == 2
+  assert tao.slices(1, 3, 20000, 10, 132) == 7             # test_gpu_tree_ah's sliced leaves
+  assert tao.slices(300, 1, 20000, 1, 132) == 1 and tao.slices(1, 1, 100, 100, 132) == 1
+  # 4096 queries x 10 probes x 2048 candidates: 10*2048*12 + 2048*12 + 2*128 + 4 + 10*12 + 10*12 + 10*24 B per query
+  assert tao.query_chunk(4096, 10, 1, 16, 10, 2048, True) == (512 << 20) // 271076 == 1980
+  assert tao.query_chunk(3, 10, 1, 16, 10, 2048, True) == 3
+  assert tao.merge_region(64, 106, 106) == 6784 and tao.tree_merge(64, 106, 106)       # 162,816 B
+  assert tao.merge_region(64, 107, 107) == 6848 and not tao.tree_merge(64, 107, 107)   # 164,352 B
+  assert tao.tree_merge(4, 1706, 1706) and not tao.tree_merge(4, 1707, 1707)           # 163,776 / 163,872 B
+  assert tao.tree_merge(64, 1, 1) and not tao.tree_merge(65, 1, 1)
+  assert tao.merge_region(5, 10, 30) == 60                  # levels of 3 x 20, then 2 x 30 entries
+
+
+def test_update_steps_keep_empty_members_and_signed_zero():
+  xt = np.array([[-0.0, 1e8], [-0.0, 1.0], [2.0, -1e8], [-0.0, 0.5]], np.float32)
+  cent = np.full((3, 2), 7.25, np.float32)
+  got = tao.update_centroids(xt, np.array([0, 0, 2, 0]), cent)
+  assert got[0].tobytes() == np.array([-0.0, np.float32((1e8 + 1.0 + 0.5) / 3)], np.float32).tobytes()
+  assert got[1].tobytes() == cent[1].tobytes() and got[2].tobytes() == xt[2].tobytes()
+  cb = np.full((2, 16, 2), 3.0, np.float32)
+  cb[1, :, 1] = 0.0                                           # d = 3, dpb = 2: the last block's unused dim
+  rt = np.array([[-0.0, -0.0, 1.0], [-0.0, -0.0, 2.0]], np.float32)
+  got = tao.update_codebooks(rt, np.array([[5, 9], [5, 9]]), cb, 2)
+  assert got[0, 5].tobytes() == np.array([-0.0, -0.0], np.float32).tobytes()
+  assert np.array_equal(got[1, 9], [1.5, 0.0]) and np.all(np.delete(got[0], 5, 0) == 3.0)
+  assert np.all(got[1, :, 1] == 0.0) and np.all(np.delete(got[1, :, 0], 9) == 3.0)
+
+
+@pytest.mark.parametrize("dpb", [1, 3, 8])
+def test_half_tie_queries_hit_half_integers(built, dpb):
+  x = _data(400, 20, seed=dpb)
+  cb = tao.build(x, num_leaves=4, training_iterations=1, dpb=dpb)["codebooks"]
+  for t in (1.5, 2.5, -3.5, 126.5):
+    q = tao.half_tie_query(cb, 20, dpb, t)
+    assert q is not None, t
+    T, s = tao.table(q[None], cb, dpb)
+    assert s[0] == 1.0 and np.abs(T).max() == 127.0 and np.count_nonzero(T == np.float32(t)) >= 1
+    T8, _ = tao.lut(q[None], cb, dpb)
+    assert np.all(T8[T == np.float32(t)] == np.rint(t))      # half to even: 2, 2, -4, 126
+  assert tao.half_tie_query(cb[:1], dpb, dpb, 1.5) is None
