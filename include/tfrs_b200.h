@@ -956,6 +956,52 @@ size_t tfrs_layer_norm_bwd_workspace_bytes(int64_t N, int64_t d);
 int tfrs_layer_norm_bwd_f32(const float* x, const float* gamma, const float* mean, const float* rstd, const float* dy,
                             int64_t N, int64_t d, float* dx, float* dparams, void* ws, size_t ws_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * K23 dropout: tf.keras.layers.Dropout's training-mode output over x (contiguous float32, `rank` axes of `shape`):
+ *   y[i] = keep(m(i)) ? x[i] * scale : +0.0f.  The same call on dy is the backward (the mask is regenerated, never
+ *   stored).  A dropped element is +0 whatever x[i] is, so a dropped NaN or inf does not propagate.
+ *   noise_shape [rank] (nullable = shape): each entry is 1 (one mask value broadcast along that axis) or shape[a].  Mask
+ *   element j counts row-major over the noise shape; m(i) is the mask element of output element i.
+ *   Philox4x32-10 (M = 0xD2511F53, 0xCD9E8D57; W = 0x9E3779B9, 0xBB67AE85) at key (seed lo, seed hi) and counter
+ *   (g lo, g hi, call lo, call hi) with g = j / 4; element j takes output word j % 4.
+ *   keep <=> (word >> 8) >= thr, thr = ceil(rate * 2^24) in float64;  scale = (float)(1 / (1 - rate)) from float64.
+ *   0 <= rate < 1; 1 <= rank <= TFRS_DROPOUT_MAX_RANK (TFRS_ERR_UNSUPPORTED otherwise).  `call` is the caller's per-layer
+ *   counter, advanced once per training call.  An empty x writes nothing.  One launch.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_DROPOUT_MAX_RANK 4
+
+int tfrs_dropout_f32(const float* x, int rank, const int64_t* shape, const int64_t* noise_shape, double rate,
+                     uint64_t seed, uint64_t call, float* y, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * K24 batch normalization: tf.keras.layers.BatchNormalization(axis=-1) over the rows of x [N, d] (N >= 1, d >= 1; the
+ * statistics are per column).  gamma / beta [d] nullable (scale / center off).  mask [N] (TFRS_I32 / TFRS_I64 /
+ * TFRS_BOOL, nonzero = kept, nullable) restricts the batch moments to the kept rows (weighted moments, n = sum w); n = 0
+ * gives mean 0 and variance 0.  Every sum runs in a fixed order over a row chunking that depends on (N, d) only: no
+ * float atomics, bitwise reproducible.
+ *   training: the batch mean as the fp32 pair hi = f32(mean), lo = f32(mean - hi) (per-chunk shifted sums folded in
+ *     fp64), the population variance var, rstd = 1 / sqrtf(var + eps), y = ((x - hi) - lo) rstd gamma + beta; the
+ *     moving statistics updated in place with decay = f32(1 - momentum): mm = mm - (mm - f32(hi + lo)) decay, mv = mv
+ *     - (mv - var) decay (plain fp32, no contraction).
+ *   inference: y = (x - mm) rstd_mv gamma + beta with rstd_mv = 1 / sqrtf(mv + eps); nothing is updated.
+ *   tfrs_batch_norm_fwd_f32: y [N, d]; saved [3 d + 1] = (hi [d], lo [d], rstd [d], n) for the backward (nullable; at
+ *     inference hi = mm, lo = 0, rstd = rstd_mv).  Training: three launches (chunk sums, fold + moving update,
+ *     normalize); ws: tfrs_batch_norm_fwd_workspace_bytes, 16-byte aligned.  Inference: one launch, no workspace.
+ *   tfrs_batch_norm_bwd_f32: from dy and the forward's saved: dparams [2, d] = (dgamma, dbeta) = (sum_rows dy xhat,
+ *     sum_rows dy) over all rows, xhat = ((x - hi) - lo) rstd; dx [N, d] (nullable) = gamma rstd (dy - w (S1 + xhat S2)
+ *     / n) in training (S1 = dbeta, S2 = dgamma), dy gamma rstd_mv at inference.  Training: three launches (chunk
+ *     partials, fold, dx); inference: two (chunk partials with dx, fold).  ws: tfrs_batch_norm_bwd_workspace_bytes,
+ *     16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_batch_norm_fwd_workspace_bytes(int64_t N, int64_t d);
+int tfrs_batch_norm_fwd_f32(const float* x, const void* mask, int mask_kind, const float* gamma, const float* beta,
+                            int64_t N, int64_t d, int training, double momentum, float eps, float* moving_mean,
+                            float* moving_var, float* y, float* saved, void* ws, size_t ws_bytes, void* stream);
+size_t tfrs_batch_norm_bwd_workspace_bytes(int64_t N, int64_t d);
+int tfrs_batch_norm_bwd_f32(const float* x, const void* mask, int mask_kind, const float* gamma, const float* saved,
+                            const float* dy, int64_t N, int64_t d, int training, float* dx, float* dparams, void* ws,
+                            size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

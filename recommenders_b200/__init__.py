@@ -10,6 +10,7 @@ ranking hot path behind the reference's own API surface:
 (namespace per tensorflow_recommenders/__init__.py:51-61 and layers/__init__.py:18-23).  Tensors are CUDA
 torch tensors; all arithmetic on the path runs in libtfrs_b200.so (include/tfrs_b200.h).  No CPU fallback.
 """
+from . import backend
 from . import data
 from . import examples
 from . import layers

@@ -24,6 +24,8 @@ c_l = ctypes.c_int64
 c_f = ctypes.c_float
 c_sz = ctypes.c_size_t
 c_u32 = ctypes.c_uint32
+c_u64 = ctypes.c_uint64
+c_d = ctypes.c_double
 
 _SIGNATURES = {
     "tfrs_version": (c_i, []),
@@ -169,6 +171,11 @@ _SIGNATURES = {
     "tfrs_layer_norm_fwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_l, c_f, c_p, c_p, c_p, c_p]),
     "tfrs_layer_norm_bwd_workspace_bytes": (c_sz, [c_l, c_l]),
     "tfrs_layer_norm_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_l, c_l, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_dropout_f32": (c_i, [c_p, c_i, c_p, c_p, c_d, c_u64, c_u64, c_p, c_p]),
+    "tfrs_batch_norm_fwd_workspace_bytes": (c_sz, [c_l, c_l]),
+    "tfrs_batch_norm_fwd_f32": (c_i, [c_p, c_p, c_i, c_p, c_p, c_l, c_l, c_i, c_d, c_f, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "tfrs_batch_norm_bwd_workspace_bytes": (c_sz, [c_l, c_l]),
+    "tfrs_batch_norm_bwd_f32": (c_i, [c_p, c_p, c_i, c_p, c_p, c_p, c_l, c_l, c_i, c_p, c_p, c_p, c_sz, c_p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

@@ -9,9 +9,11 @@ from . import normalization
 from . import pooling
 from . import preprocessing
 from . import recurrent
+from . import regularization
 from .attention import MultiHeadAttention
 from .feature_interaction import dcn
-from .normalization import LayerNormalization
+from .normalization import BatchNormalization, LayerNormalization
 from .pooling import GlobalAveragePooling1D
 from .preprocessing import Discretization, Hashing, IntegerLookup, Normalization, StringLookup, TextVectorization
 from .recurrent import GRU, LSTM
+from .regularization import Dropout, SpatialDropout1D

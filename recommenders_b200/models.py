@@ -7,6 +7,7 @@ from typing import Dict, Iterable, List
 import torch
 
 from . import optimizers as _opt
+from .backend import learning_phase_scope
 
 
 class Model(torch.nn.Module):
@@ -57,11 +58,13 @@ class Model(torch.nn.Module):
     return torch.stack([l.sum() for l in losses]).sum()
 
   def train_step(self, inputs) -> Dict[str, object]:
-    """Custom train step using the `compute_loss` method (base.py:64-85)."""
+    """Custom train step using the `compute_loss` method (base.py:64-85).  `compute_loss` runs in a training learning
+    phase (backend.py), so Dropout and BatchNormalization in the towers train without `training` forwarded to them."""
     if self.optimizer is None:
       raise RuntimeError("call compile(optimizer) before train_step")
     self.optimizer.zero_grad()
-    loss = self.compute_loss(inputs, training=True)
+    with learning_phase_scope(True):
+      loss = self.compute_loss(inputs, training=True)
     regularization_loss = self._regularization_loss(loss)
     total_loss = loss + regularization_loss
     total_loss.backward()
@@ -75,7 +78,8 @@ class Model(torch.nn.Module):
   @torch.no_grad()
   def test_step(self, inputs) -> Dict[str, object]:
     """Custom test step using the `compute_loss` method (base.py:87-104)."""
-    loss = self.compute_loss(inputs, training=False)
+    with learning_phase_scope(False):
+      loss = self.compute_loss(inputs, training=False)
     regularization_loss = self._regularization_loss(loss)
     total_loss = loss + regularization_loss
     metrics = {metric.name: metric.result() for metric in self.metrics}

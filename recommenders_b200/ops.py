@@ -2525,3 +2525,154 @@ def layer_norm(x: torch.Tensor, gamma: Optional[torch.Tensor] = None, beta: Opti
   y, _, _ = _layer_norm_fwd(x2.detach(), None if g is None else g.detach(), None if b is None else b.detach(), epsilon,
                             False)
   return y.reshape(x.shape)
+
+
+# ------------------------------------------------------------------------------------------------
+# K23 dropout: layers.Dropout / SpatialDropout1D in training, one counter-based Philox kernel both ways
+# ------------------------------------------------------------------------------------------------
+DROPOUT_MAX_RANK = 4   # TFRS_DROPOUT_MAX_RANK of include/tfrs_b200.h
+
+
+def dropout_noise_shape(shape, noise_shape) -> Tuple[int, ...]:
+  """Keras's noise shape for an input of `shape`: a None entry takes the input's size, and every entry must be 1 (one
+  mask value broadcast along that axis) or the input's size."""
+  shape = tuple(int(s) for s in shape)
+  if noise_shape is None:
+    return shape
+  if len(noise_shape) != len(shape):
+    raise ValueError(f"dropout: noise_shape {tuple(noise_shape)} does not broadcast to the input's shape {shape}")
+  noise = tuple(shape[a] if s is None else int(s) for a, s in enumerate(noise_shape))
+  if any(n not in (1, s) for n, s in zip(noise, shape)):
+    raise ValueError(f"dropout: noise_shape {tuple(noise_shape)} does not broadcast to the input's shape {shape}")
+  return noise
+
+
+def _dropout_launch(x, rate, key, call, noise):
+  y = torch.empty_like(x, memory_format=torch.contiguous_format)
+  arr = lambda v: ctypes.cast((ctypes.c_int64 * len(v))(*v), c_p)
+  check(lib().tfrs_dropout_f32(ptr(x), x.dim(), arr(x.shape), arr(noise), float(rate), key, call, ptr(y), stream()),
+        "dropout")
+  return y
+
+
+class _Dropout(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, x, rate, key, call, noise):
+    ctx.args = (rate, key, call, noise)
+    return _dropout_launch(x, rate, key, call, noise)
+
+  @staticmethod
+  def backward(ctx, dy):
+    return _dropout_launch(f32c(dy, "grad"), *ctx.args), None, None, None, None
+
+
+def dropout(x: torch.Tensor, rate: float, key: int, call: int, noise_shape=None) -> torch.Tensor:
+  """tf.keras.layers.Dropout in training: y = keep ? x * f32(1 / (1 - rate)) : +0 over x (float32, CUDA, rank 1 to
+  DROPOUT_MAX_RANK).  The mask is Philox4x32-10 at the 64-bit `key` and the 64-bit counter `call` (include/tfrs_b200.h,
+  K23); `noise_shape` follows Keras.  Differentiable in x: the backward regenerates the mask from (key, call), nothing is
+  stored.  One launch each way, also at rate 0 (the layers skip that call)."""
+  require_cuda(x, "inputs")
+  if x.dtype != torch.float32:
+    raise TypeError(f"dropout: inputs must be float32, got {x.dtype}")
+  if not 1 <= x.dim() <= DROPOUT_MAX_RANK:
+    raise NotImplementedError(f"dropout: an input of rank {x.dim()} is not supported (rank 1 to {DROPOUT_MAX_RANK})")
+  if not 0.0 <= float(rate) < 1.0:
+    raise ValueError(f"dropout: rate must be in [0, 1), got {rate}")
+  noise = dropout_noise_shape(x.shape, noise_shape)
+  key, call = int(key) & (2**64 - 1), int(call) & (2**64 - 1)
+  xc = x.contiguous()
+  if torch.is_grad_enabled() and x.requires_grad:
+    return _Dropout.apply(xc, float(rate), key, call, noise)
+  return _dropout_launch(xc.detach(), float(rate), key, call, noise)
+
+
+# ------------------------------------------------------------------------------------------------
+# K24 batch normalization: layers.BatchNormalization over the last axis
+# ------------------------------------------------------------------------------------------------
+def _bn_fwd(x2, m, mk, gamma, beta, mm, mv, training, momentum, eps, save):
+  N, d = x2.shape
+  y = torch.empty_like(x2)
+  saved = torch.empty((3 * d + 1,), dtype=torch.float32, device=x2.device) if save else None   # (hi, lo, rstd, n)
+  nb = lib().tfrs_batch_norm_fwd_workspace_bytes(N, d) if training else 0
+  ws = workspace(nb, x2.device, "batch_norm_fwd") if training else None
+  check(lib().tfrs_batch_norm_fwd_f32(ptr(x2), ptr(m), mk, ptr(gamma), ptr(beta), N, d, int(training), float(momentum),
+                                      float(eps), ptr(mm), ptr(mv), ptr(y), ptr(saved), ptr(ws),
+                                      0 if ws is None else ws.numel(), stream()), "batch_norm_fwd")
+  if training:   # the kernel wrote the moving statistics through raw pointers; tell autograd they changed
+    torch.autograd.graph.increment_version(mm)
+    torch.autograd.graph.increment_version(mv)
+  return y, saved
+
+
+class _BatchNorm(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, x2, gamma, beta, m, mk, moving, training, momentum, eps):
+    y, saved = _bn_fwd(x2, m, mk, gamma, beta, *moving, training, momentum, eps, True)
+    ctx.save_for_backward(x2, gamma, saved, m)
+    ctx.mk, ctx.training = mk, training
+    ctx.set_materialize_grads(False)
+    return y
+
+  @staticmethod
+  def backward(ctx, dy):
+    x2, gamma, saved, m = ctx.saved_tensors
+    N, d = x2.shape
+    n_x, n_g, n_b = ctx.needs_input_grad[:3]
+    dx = torch.empty_like(x2) if n_x else None
+    dparams = torch.empty((2, d), dtype=torch.float32, device=x2.device)
+    if dy is None:
+      dparams.zero_()
+      if dx is not None:
+        dx.zero_()
+    else:
+      dy = f32c(dy, "grad")
+      ws = workspace(lib().tfrs_batch_norm_bwd_workspace_bytes(N, d), x2.device, "batch_norm_bwd")
+      check(lib().tfrs_batch_norm_bwd_f32(ptr(x2), ptr(m), ctx.mk, ptr(gamma), ptr(saved), ptr(dy), N, d,
+                                          int(ctx.training), ptr(dx), ptr(dparams), ptr(ws), ws.numel(), stream()),
+            "batch_norm_bwd")
+    return (dx, dparams[0] if n_g else None, dparams[1] if n_b else None) + (None,) * 6
+
+
+def batch_norm(x: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor], moving_mean: torch.Tensor,
+               moving_variance: torch.Tensor, training: bool, momentum: float = 0.99, epsilon: float = 1e-3,
+               mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+  """tf.keras.layers.BatchNormalization(axis=-1) over x (float32, CUDA, rank >= 2; the statistics are per last-axis
+  column over all other axes).  In training: the batch mean (an fp32 pair) and population variance, restricted to the
+  rows `mask` (x.shape[:-1], bool / int32 / int64, nonzero = kept) keeps; y = (x - mean) rsqrt(var + epsilon) gamma +
+  beta; moving_mean / moving_variance (float32 [d], contiguous) are updated in place with decay f32(1 - momentum), also
+  under no_grad, and their autograd version counters move as after any in-place update.  At inference: y = (x - moving_mean) rsqrt(moving_variance + epsilon) gamma + beta.  gamma / beta [d]
+  or None (scale / center off).  Differentiable in x, gamma and beta in both modes; under no_grad nothing is saved.
+  K24: three launches forward in training, one at inference; three backward in training, two at inference."""
+  require_cuda(x, "inputs")
+  if x.dim() < 2:
+    raise ValueError(f"batch_norm: the input must have at least two axes, got {tuple(x.shape)}")
+  d = x.shape[-1]
+  N = x.numel() // d if d else 0
+  if d == 0 or N == 0:
+    raise ValueError(f"batch_norm: the input {tuple(x.shape)} is empty")
+  for p, name in ((gamma, "gamma"), (beta, "beta"), (moving_mean, "moving_mean"), (moving_variance, "moving_variance")):
+    if p is not None and tuple(p.shape) != (d,):
+      raise ValueError(f"batch_norm: {name} must be [{d}], got {tuple(p.shape)}")
+  for p, name in ((moving_mean, "moving_mean"), (moving_variance, "moving_variance")):
+    require_cuda(p, name)
+    if p.dtype != torch.float32 or not p.is_contiguous():
+      raise TypeError(f"batch_norm: {name} must be a contiguous float32 tensor (it is updated in place)")
+  m, mk = None, 0
+  if mask is not None:
+    require_cuda(mask, "mask")
+    if mask.dtype not in _MASK_KINDS:
+      raise TypeError(f"batch_norm: the mask must be bool, int32 or int64, got {mask.dtype}")
+    if tuple(mask.shape) != tuple(x.shape[:-1]):
+      raise ValueError(f"batch_norm: the mask has shape {tuple(mask.shape)}, the input {tuple(x.shape)}")
+    m, mk = mask.contiguous().reshape(N), _MASK_KINDS[mask.dtype]
+  x2 = f32c(x, "inputs").reshape(N, d)
+  g = None if gamma is None else f32c(gamma, "gamma")
+  b = None if beta is None else f32c(beta, "beta")
+  moving = (moving_mean.detach(), moving_variance.detach())
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x2, g, b)):
+    return _BatchNorm.apply(x2, g, b, m, mk, moving, bool(training), float(momentum), float(epsilon)).reshape(x.shape)
+  y, _ = _bn_fwd(x2.detach(), m, mk, None if g is None else g.detach(), None if b is None else b.detach(), *moving,
+                 bool(training), momentum, epsilon, False)
+  return y.reshape(x.shape)
