@@ -939,6 +939,50 @@ int tfrs_mha_bwd_f32(const float* Q, const float* K, const float* V, const TfrsM
                      float* dQ, float* dK, float* dV, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Dense attention (K21 dot scores, K25 tanh scores): tf.keras.layers.Attention and AdditiveAttention on query Q [B, Tq,
+ * dim], key K [B, Tv, dim] and value V [B, Tv, dv] (float32, contiguous; 1 <= dim, dv <= TFRS_MHA_MAX_HEAD_DIM, Tq, Tv
+ * >= 1), run as one head over the B * Tq query rows.  Scores in fp32:
+ *   TFRS_DENSE_DOT:      s = scale * (q . k)                        (scale [1], NULL = 1)
+ *   TFRS_DENSE_CONCAT:   s = wc * sum_d tanhf(scale (q_d + k_d))    (scale [1], NULL = 1; concat_weight wc [1])
+ *   TFRS_DENSE_ADDITIVE: s = sum_d scale_d tanhf(q_d + k_d)         (scale [dim], NULL = 1)
+ *   The weights are device pointers, read by the kernels.  keep(b, i, j) = value_mask[b, j] & (j <= i if causal); a
+ *   dropped score gets s -= 1e9 in fp32, then P = softmax over j (a fully masked row is uniform).  With rate > 0 (a
+ *   training call) the weights are dropped as K23 drops a [B, Tq, Tv] tensor: element e = (b Tq + i) Tv + j takes word
+ *   e % 4 of Philox4x32-10 at counter (e/4 lo, e/4 hi, call lo, call hi) and key (seed lo, seed hi); keep <=> (word >>
+ *   8) >= ceil(rate * 2^24); W = keep ? P * (float)(1 / (1 - rate)) : +0; else W = P.  O[b, i] = query_mask[b, i] *
+ *   sum_j W_ij v_j.  Masks [B, Tq] / [B, Tv] nullable, kinds TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero = kept.
+ *   tfrs_dense_attention_fwd_f32: O [B, Tq, dv]; stats [B, Tq, 2] = (row max, row sum of e^{s - max}) (nullable; the
+ *     backward needs it); P [B, Tq, Tv] = W (nullable).  One launch.
+ *   tfrs_dense_attention_bwd_f32: from dO and the forward's O and stats: dQ, dK [B, Tv, dim], dV; dscale ([1], or [dim]
+ *     for ADDITIVE; nullable) and dconcat_weight ([1], CONCAT only; nullable).  Three launches (delta, dK / dV per key
+ *     row, dQ and the per-row partials of the weights' gradients per query row) and one fixed-order fold per weight
+ *     gradient asked for.  ws: tfrs_dense_attention_bwd_workspace_bytes, 16-byte aligned.  No float atomics: bitwise
+ *     reproducible.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_DENSE_DOT 0
+#define TFRS_DENSE_CONCAT 1
+#define TFRS_DENSE_ADDITIVE 2
+
+typedef struct TfrsDenseAttention {
+  int mode;
+  const float* scale;
+  const float* concat_weight;
+  const void* query_mask; int query_mask_kind;
+  const void* value_mask; int value_mask_kind;
+  int causal;
+  double rate; uint64_t seed; uint64_t call;
+} TfrsDenseAttention;
+
+int tfrs_dense_attention_fwd_f32(const float* Q, const float* K, const float* V, const TfrsDenseAttention* desc,
+                                 int64_t B, int64_t Tq, int64_t Tv, int dim, int dv, float* O, float* stats, float* P,
+                                 void* stream);
+size_t tfrs_dense_attention_bwd_workspace_bytes(int mode, int64_t B, int64_t Tq, int dim);
+int tfrs_dense_attention_bwd_f32(const float* Q, const float* K, const float* V, const TfrsDenseAttention* desc,
+                                 const float* O, const float* stats, const float* dO, int64_t B, int64_t Tq, int64_t Tv,
+                                 int dim, int dv, float* dQ, float* dK, float* dV, float* dscale, float* dconcat_weight,
+                                 void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K22 layer normalization: tf.keras.layers.LayerNormalization(axis=-1) over the rows of x [N, d] (d >= 1).
  *   mean = hi + lo with hi = sum(x) / d and lo = sum(x - hi) / d; var = sum((x - hi)^2) / d - lo^2 (population
  *   variance, corrected two-pass); rstd = 1 / sqrtf(var + eps); y = ((x - hi) - lo) * rstd * gamma + beta, gamma / beta

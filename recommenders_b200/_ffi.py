@@ -168,6 +168,10 @@ _SIGNATURES = {
     "tfrs_mha_bwd_workspace_bytes": (c_sz, [c_l, c_l, c_i]),
     "tfrs_mha_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_l, c_l, c_l, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz,
                                c_p]),
+    "tfrs_dense_attention_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_l, c_l, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "tfrs_dense_attention_bwd_workspace_bytes": (c_sz, [c_i, c_l, c_l, c_i]),
+    "tfrs_dense_attention_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_l, c_l, c_l, c_i, c_i, c_p, c_p, c_p, c_p,
+                                           c_p, c_p, c_sz, c_p]),
     "tfrs_layer_norm_fwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_l, c_f, c_p, c_p, c_p, c_p]),
     "tfrs_layer_norm_bwd_workspace_bytes": (c_sz, [c_l, c_l]),
     "tfrs_layer_norm_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_l, c_l, c_p, c_p, c_p, c_sz, c_p]),

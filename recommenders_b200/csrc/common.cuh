@@ -69,6 +69,8 @@ static inline unsigned elementwise_grid(long long n) {
 int reduce_parts(const float* partial, long long M, long long N, int parts, float* out, long long ld, cudaStream_t st);
 // loss[0] = sum_i v[i * stride] over i < n, in fp64 and a fixed order
 int reduce_loss(const float* v, long long n, long long stride, float* loss, cudaStream_t st);
+// out[c] = sum_i v[i * cols + c] over i < n, for each c < cols: one CTA per column, fp64, the order of reduce_loss
+int reduce_columns(const float* v, long long n, long long cols, float* out, cudaStream_t st);
 
 // Hook of the sharded scan (topk_tc.cu <-> comm.cu): all device pointers; thr[q] = L_q - margin_q in the shard's screening
 // units (scores scaled by 2^(*exp_corpus + qexp[q])), cut[q] = 2 eps_q.  The hook may raise thr[].

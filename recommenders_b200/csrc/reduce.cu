@@ -1,5 +1,5 @@
 // reduce.cu -- the fixed-order reductions shared by the layers: the fp32 sum of split-K / chunk / part partials and the fp64
-// sum of a loss vector.  The summation order is fixed, so every result is bitwise reproducible; there are no float atomics.
+// sum of a loss vector or of each column of a row-major matrix.  The summation order is fixed, so every result is bitwise reproducible; there are no float atomics.
 #include "common.cuh"
 
 namespace tfrs {
@@ -20,10 +20,13 @@ int reduce_parts(const float* partial, long long M, long long N, int parts, floa
   return TFRS_OK;
 }
 
-// loss[0] = sum_i v[i * stride], i < n: fp64 per-thread sums (thread t takes i = t, t + 1024, ...), then a fixed tree
+// loss[c] = sum_i v[i * stride + c], i < n, c = blockIdx.x: fp64 per-thread sums (thread t takes i = t, t + 1024, ...),
+// then a fixed tree
 __global__ void __launch_bounds__(1024)
 reduce_loss_kernel(const float* __restrict__ v, long long n, long long stride, float* __restrict__ loss) {
   __shared__ double red[1024];
+  v += blockIdx.x;
+  loss += blockIdx.x;
   double a = 0.0;
   for (long long i = threadIdx.x; i < n; i += 1024) a += (double)v[i * stride];
   red[threadIdx.x] = a;
@@ -34,6 +37,12 @@ reduce_loss_kernel(const float* __restrict__ v, long long n, long long stride, f
 
 int reduce_loss(const float* v, long long n, long long stride, float* loss, cudaStream_t st) {
   reduce_loss_kernel<<<1, 1024, 0, st>>>(v, n, stride, loss);
+  TFRS_LAUNCH_CHECK();
+  return TFRS_OK;
+}
+
+int reduce_columns(const float* v, long long n, long long cols, float* out, cudaStream_t st) {
+  reduce_loss_kernel<<<(unsigned)cols, 1024, 0, st>>>(v, n, cols, out);
   TFRS_LAUNCH_CHECK();
   return TFRS_OK;
 }

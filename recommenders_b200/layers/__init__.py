@@ -10,7 +10,7 @@ from . import pooling
 from . import preprocessing
 from . import recurrent
 from . import regularization
-from .attention import MultiHeadAttention
+from .attention import AdditiveAttention, Attention, MultiHeadAttention
 from .feature_interaction import dcn
 from .normalization import BatchNormalization, LayerNormalization
 from .pooling import GlobalAveragePooling1D

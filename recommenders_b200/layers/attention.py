@@ -1,6 +1,8 @@
-"""`MultiHeadAttention`, the self-attention block of SASRec-style query towers and of the Transformer title encoders the
-featurization tutorial points to: tf.keras.layers.MultiHeadAttention on K6 (the four projections) and K21 (the
-attention core).  DESIGN.md §2 (A25) pins its rules."""
+"""`MultiHeadAttention`, `Attention` and `AdditiveAttention`.  MultiHeadAttention is the self-attention block of
+SASRec-style query towers and of the Transformer title encoders the featurization tutorial points to:
+tf.keras.layers.MultiHeadAttention on K6 (the four projections) and K21 (the attention core), DESIGN.md §2 (A25).  Attention and AdditiveAttention are the target attention of DIN / BST-style
+ranking models (a candidate attending over a user's history): tf.keras's dense attention layers on K21's dot scores and
+K25's tanh scores, DESIGN.md §2 (A27)."""
 from __future__ import annotations
 
 import math
@@ -10,6 +12,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from ..backend import resolve_training
 from .feature_interaction.dcn import _init
 
 
@@ -158,3 +161,130 @@ class MultiHeadAttention(torch.nn.Module):
   @classmethod
   def from_config(cls, config: Dict[str, Any]):
     return cls(**config)
+
+
+class _BaseDenseAttention(torch.nn.Module):
+  """tf-keras's BaseDenseAttention: `layer([query, value])` or `layer([query, value, key])` on ops.dense_attention.
+  DESIGN.md §2 (A27) pins its rules."""
+
+  def __init__(self, dropout: float = 0.0, seed=None, causal: bool = False, name=None, kwargs=None):
+    super().__init__()
+    cls = type(self).__name__
+    for key, val in (kwargs or {}).items():   # Keras's base-layer arguments; anything else is a mistake
+      if (key == "dtype" and val in (None, "float32", torch.float32)) or (key == "trainable" and val is True):
+        continue
+      if key in ("dtype", "trainable"):
+        raise NotImplementedError(f"{cls}: {key}={val!r} is not supported")
+      raise TypeError(f"{cls}: keyword argument not understood: {key!r}")
+    if isinstance(dropout, bool) or not isinstance(dropout, (int, float)) or not 0 <= dropout < 1:
+      raise ValueError(f"{type(self).__name__}: dropout must be a float in [0, 1), got {dropout!r}")
+    self.dropout, self.seed, self.causal, self.name = float(dropout), seed, bool(causal), name
+    self._key = 0
+    if self.dropout > 0:
+      if seed is None:       # drawn only when it is used, so a dropout-free layer leaves torch's RNG alone
+        lo, hi = torch.randint(0, 2**32, (2,), dtype=torch.int64).tolist()
+        self._key = lo | (hi << 32)
+      else:
+        self._key = int(seed) & (2**64 - 1)
+    self._calls = 0
+    self.built = False
+
+  def _score_args(self):
+    raise NotImplementedError
+
+  def call(self, inputs, mask=None, training=None, return_attention_scores: bool = False,
+           use_causal_mask: bool = False):
+    cls = type(self).__name__
+    if not isinstance(inputs, (list, tuple)) or len(inputs) not in (2, 3):
+      raise ValueError(f"{cls} layer must be called on a list of inputs, namely [query, value] or [query, value, key]. "
+                       f"Received: {inputs!r}")
+    if mask is not None and (not isinstance(mask, (list, tuple)) or not 2 <= len(mask) <= len(inputs)):
+      raise ValueError(f"{cls} layer mask must be a list of length 2, namely [query_mask, value_mask]. Received: "
+                       f"{mask!r}")
+    query, value = inputs[0], inputs[1]
+    key = inputs[2] if len(inputs) == 3 else value
+    for t, name in ((query, "query"), (value, "value"), (key, "key")):
+      if not isinstance(t, torch.Tensor) or t.dim() != 3:
+        raise ValueError(f"{cls}: {name} must be a 3-D tensor [batch, length, dim], got "
+                         f"{tuple(t.shape) if isinstance(t, torch.Tensor) else type(t)}")
+    if not self.built:
+      self.build(int(query.shape[-1]), query.device)
+    dev = query.device
+    q_mask, v_mask = (None, None) if mask is None else (mask[0], mask[1])
+    q_mask = ops.attached_mask(query) if q_mask is None else _as_mask(q_mask, dev)
+    v_mask = ops.attached_mask(value) if v_mask is None else _as_mask(v_mask, dev)
+    rate, call = 0.0, 0
+    if self.dropout > 0 and resolve_training(training):
+      rate, call = self.dropout, self._calls
+      self._calls += 1
+    mode, scale, cw = self._score_args()
+    out, weights = ops.dense_attention(query, key, value, mode, scale, cw, query_mask=q_mask, value_mask=v_mask,
+                                       causal=self.causal or bool(use_causal_mask), rate=rate, seed=self._key,
+                                       call=call, return_scores=bool(return_attention_scores))
+    if q_mask is not None:
+      out._tfrs_mask = (q_mask, out._version, out.data_ptr())
+    return (out, weights) if return_attention_scores else out
+
+  def forward(self, inputs, mask=None, training=None, return_attention_scores: bool = False,
+              use_causal_mask: bool = False):
+    return self.call(inputs, mask=mask, training=training, return_attention_scores=return_attention_scores,
+                     use_causal_mask=use_causal_mask)
+
+  @classmethod
+  def from_config(cls, config: Dict[str, Any]):
+    return cls(**config)
+
+
+class Attention(_BaseDenseAttention):
+  """`tf.keras.layers.Attention(use_scale=False, score_mode="dot", dropout=0.0, seed=None)`, Luong-style attention:
+  `layer([query, value, key], mask=[query_mask, value_mask], training=None, return_attention_scores=False,
+  use_causal_mask=False)` with query [B, Tq, dim], value [B, Tv, dv], key [B, Tv, dim] (key = value when omitted) ->
+  [B, Tq, dv], and with `return_attention_scores` also the weights [B, Tq, Tv] value was multiplied by (after dropout),
+  detached.  Scores: "dot" (q . k) * scale; "concat" concat_score_weight * sum_d tanh(scale (q_d + k_d)).  Weights,
+  created on the first call: `scale` (a scalar, 1) with use_scale and `concat_score_weight` (a scalar, 1) with
+  "concat".  A mask not passed is taken from the input an `Embedding(mask_zero=True)` produced; the value mask and the
+  causal triangle (`use_causal_mask`, or the deprecated `causal=True`) drop scores before the softmax, the query mask
+  zeroes output rows, and the output carries it.  Dropout on the weights in training only (`backend.resolve_training`),
+  with Dropout's seed and call-counter rules.  dim and dv go up to 128 (ops.MHA_MAX_HEAD_DIM)."""
+
+  def __init__(self, use_scale: bool = False, score_mode: str = "dot", dropout: float = 0.0, seed=None, causal=False,
+               name=None, **kwargs):
+    if score_mode not in ("dot", "concat"):
+      raise ValueError(f"Invalid value for argument score_mode. Expected one of {{'dot', 'concat'}}. Received: "
+                       f"score_mode={score_mode}")
+    super().__init__(dropout, seed, causal, name, kwargs)
+    self.use_scale, self.score_mode = bool(use_scale), score_mode
+
+  def build(self, dim: int, device):
+    one = lambda: torch.nn.Parameter(torch.ones((), dtype=torch.float32, device=device))
+    self.scale = one() if self.use_scale else None
+    self.concat_score_weight = one() if self.score_mode == "concat" else None
+    self.built = True
+
+  def _score_args(self):
+    return self.score_mode, self.scale, self.concat_score_weight
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"use_scale": self.use_scale, "score_mode": self.score_mode, "dropout": self.dropout, "seed": self.seed,
+            "causal": self.causal, "name": self.name}
+
+
+class AdditiveAttention(_BaseDenseAttention):
+  """`tf.keras.layers.AdditiveAttention(use_scale=True, dropout=0.0, seed=None)`, Bahdanau-style attention: scores
+  sum_d scale_d tanh(q_d + k_d), with `scale` [dim] (glorot_uniform with Keras's fans, created on the first call) when
+  use_scale, else sum_d tanh(q_d + k_d).  Call, masks, dropout and the returned weights as `Attention`."""
+
+  def __init__(self, use_scale: bool = True, dropout: float = 0.0, seed=None, causal=False, name=None, **kwargs):
+    super().__init__(dropout, seed, causal, name, kwargs)
+    self.use_scale = bool(use_scale)
+
+  def build(self, dim: int, device):
+    self.scale = torch.nn.Parameter(_kernel_init("glorot_uniform", (dim,), device)) if self.use_scale else None
+    self.built = True
+
+  def _score_args(self):
+    return "additive", self.scale, None
+
+  def get_config(self) -> Dict[str, Any]:
+    return {"use_scale": self.use_scale, "dropout": self.dropout, "seed": self.seed, "causal": self.causal,
+            "name": self.name}

@@ -2461,6 +2461,136 @@ def attention(query: torch.Tensor, value: torch.Tensor, key: Optional[torch.Tens
 
 
 # ------------------------------------------------------------------------------------------------
+# Dense attention: layers.Attention (K21 dot scores, K25 concat scores) and layers.AdditiveAttention (K25)
+# ------------------------------------------------------------------------------------------------
+DENSE_SCORE_MODES = {"dot": 0, "concat": 1, "additive": 2}   # TFRS_DENSE_* of include/tfrs_b200.h
+
+
+class _DenseAttentionDesc(ctypes.Structure):
+  _fields_ = [("mode", c_i), ("scale", c_p), ("concat_weight", c_p), ("query_mask", c_p), ("query_mask_kind", c_i),
+              ("value_mask", c_p), ("value_mask_kind", c_i), ("causal", c_i), ("rate", _ffi.c_d), ("seed", _ffi.c_u64),
+              ("call", _ffi.c_u64)]
+
+
+def _dense_desc(mode, scale, cw, qm, vm, causal, rate, seed, call) -> _DenseAttentionDesc:
+  s = _DenseAttentionDesc()
+  s.mode, s.scale, s.concat_weight = mode, ptr(scale), ptr(cw)
+  s.query_mask, s.query_mask_kind = ptr(qm), _MASK_KINDS[qm.dtype] if qm is not None else 0
+  s.value_mask, s.value_mask_kind = ptr(vm), _MASK_KINDS[vm.dtype] if vm is not None else 0
+  s.causal, s.rate, s.seed, s.call = int(causal), float(rate), seed, call
+  return s
+
+
+def _dense_attention_fwd(q, k, v, args, want_p, save):
+  B, Tq, dim = q.shape
+  Tv, dv = v.shape[1], v.shape[2]
+  O = torch.empty((B, Tq, dv), dtype=torch.float32, device=q.device)
+  stats = torch.empty((B, Tq, 2), dtype=torch.float32, device=q.device) if save else None
+  P = torch.empty((B, Tq, Tv), dtype=torch.float32, device=q.device) if want_p else None
+  d = _dense_desc(*args)
+  check(lib().tfrs_dense_attention_fwd_f32(ptr(q), ptr(k), ptr(v), ctypes.byref(d), B, Tq, Tv, dim, dv, ptr(O),
+                                           ptr(stats), ptr(P), stream()), "dense_attention_fwd")
+  return O, stats, P
+
+
+class _DenseAttention(torch.autograd.Function):
+  """(O, P or an empty tensor); differentiable in q, k, v, scale and concat_weight.  P is not differentiable."""
+
+  @staticmethod
+  def forward(ctx, q, k, v, scale, cw, qm, vm, mode, causal, rate, seed, call, want_p):
+    args = (mode, scale, cw, qm, vm, causal, rate, seed, call)
+    O, stats, P = _dense_attention_fwd(q, k, v, args, want_p, True)
+    P = P if want_p else torch.empty((0,), dtype=torch.float32, device=q.device)
+    ctx.save_for_backward(q, k, v, scale, cw, qm, vm, O, stats)
+    ctx.args = (mode, causal, rate, seed, call)
+    ctx.mark_non_differentiable(P)
+    ctx.set_materialize_grads(False)
+    return O, P
+
+  @staticmethod
+  def backward(ctx, dO, _dP):
+    q, k, v, scale, cw, qm, vm, O, stats = ctx.saved_tensors
+    mode, causal, rate, seed, call = ctx.args
+    n = ctx.needs_input_grad
+    B, Tq, dim = q.shape
+    Tv, dv = v.shape[1], v.shape[2]
+    dq, dk, dv_ = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    dscale = torch.empty_like(scale) if n[3] else None
+    dcw = torch.empty_like(cw) if n[4] else None
+    if dO is None or B == 0:
+      for t in (dq, dk, dv_, dscale, dcw):
+        if t is not None:
+          t.zero_()
+    else:
+      dO = f32c(dO, "grad")
+      d = _dense_desc(mode, scale, cw, qm, vm, causal, rate, seed, call)
+      ws = workspace(lib().tfrs_dense_attention_bwd_workspace_bytes(mode, B, Tq, dim), q.device, "dense_attention_bwd")
+      check(lib().tfrs_dense_attention_bwd_f32(ptr(q), ptr(k), ptr(v), ctypes.byref(d), ptr(O), ptr(stats), ptr(dO), B,
+                                               Tq, Tv, dim, dv, ptr(dq), ptr(dk), ptr(dv_), ptr(dscale), ptr(dcw),
+                                               ptr(ws), ws.numel(), stream()), "dense_attention_bwd")
+    return (dq if n[0] else None, dk if n[1] else None, dv_ if n[2] else None, dscale, dcw) + (None,) * 8
+
+
+def dense_attention(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, score_mode: str = "dot", scale=None,
+                    concat_weight=None, query_mask=None, value_mask=None, causal: bool = False, rate: float = 0.0,
+                    seed: int = 0, call: int = 0, return_scores: bool = False):
+  """tf-keras's BaseDenseAttention core on query [B, Tq, dim], key [B, Tv, dim] and value [B, Tv, dv] (float32, CUDA;
+  dim, dv <= MHA_MAX_HEAD_DIM) -> (out [B, Tq, dv], weights [B, Tq, Tv] with `return_scores`, else None).  Scores:
+  "dot" (q . k) * scale; "concat" concat_weight * sum_d tanh(scale (q_d + k_d)); "additive" sum_d scale_d tanh(q_d +
+  k_d); scale None = 1 (a scalar tensor for dot / concat, [dim] for additive).  A score the value mask [B, Tv] or the
+  causal triangle drops gets -1e9, then softmax over Tv; with rate > 0 the weights are dropped by Philox4x32-10 at
+  (seed, call) as K23 drops a [B, Tq, Tv] tensor and the kept ones scaled by 1 / (1 - rate); out = weights . value,
+  zeroed on the rows query_mask [B, Tq] drops.  Masks are bool / int32 / int64, nonzero = kept.  The weights returned
+  are the ones value was multiplied by, detached.  One launch forward; three backward plus one fixed-order fold per
+  weight gradient.  Differentiable in query, key, value, scale and concat_weight."""
+  if score_mode not in DENSE_SCORE_MODES:
+    raise ValueError(f"dense_attention: score_mode must be 'dot', 'concat' or 'additive', got {score_mode!r}")
+  mode = DENSE_SCORE_MODES[score_mode]
+  for t, name in ((query, "query"), (key, "key"), (value, "value")):
+    require_cuda(t, name)
+    if t.dim() != 3:
+      raise ValueError(f"dense_attention: {name} must be [batch, length, dim], got {tuple(t.shape)}")
+  B, Tq, dim = query.shape
+  Tv, dv = value.shape[1], value.shape[2]
+  if tuple(key.shape) != (B, Tv, dim) or value.shape[0] != B:
+    raise ValueError(f"dense_attention: key {tuple(key.shape)} and value {tuple(value.shape)} do not fit query "
+                     f"{tuple(query.shape)}")
+  if Tq == 0 or Tv == 0:
+    raise ValueError("dense_attention: the query and value sequences must not be empty")
+  if not 1 <= dim <= MHA_MAX_HEAD_DIM or not 1 <= dv <= MHA_MAX_HEAD_DIM:
+    raise ValueError(f"dense_attention: dim = {dim} and value dim = {dv} must be in 1 .. {MHA_MAX_HEAD_DIM}, the "
+                     "kernels' ceiling")
+  if not 0.0 <= float(rate) < 1.0:
+    raise ValueError(f"dense_attention: rate must be in [0, 1), got {rate}")
+  want = (dim,) if mode == DENSE_SCORE_MODES["additive"] else (1,)
+  if scale is not None:
+    require_cuda(scale, "scale")
+    if scale.numel() != want[0] or (mode == DENSE_SCORE_MODES["additive"] and scale.dim() != 1):
+      raise ValueError(f"dense_attention: scale must have {want[0]} element(s), got shape {tuple(scale.shape)}")
+    scale = f32c(scale, "scale")
+  if mode == DENSE_SCORE_MODES["concat"]:
+    if concat_weight is None or concat_weight.numel() != 1:
+      raise ValueError("dense_attention: concat scores need a one-element concat_weight")
+    require_cuda(concat_weight, "concat_weight")
+    concat_weight = f32c(concat_weight, "concat_weight")
+  else:
+    concat_weight = None
+  qm = _mha_mask(query_mask, (B, Tq), "query_mask")
+  vm = _mha_mask(value_mask, (B, Tv), "value_mask")
+  q, k, v = f32c(query, "query"), f32c(key, "key"), f32c(value, "value")
+  seed, call = int(seed) & (2**64 - 1), int(call) & (2**64 - 1)
+  diff = (q, k, v, scale, concat_weight)
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in diff):
+    O, P = _DenseAttention.apply(q, k, v, scale, concat_weight, qm, vm, mode, bool(causal), float(rate), seed, call,
+                                 bool(return_scores))
+    return O, (P if return_scores else None)
+  det = lambda t: None if t is None else t.detach()
+  args = (mode, det(scale), det(concat_weight), qm, vm, bool(causal), float(rate), seed, call)
+  O, _, P = _dense_attention_fwd(q.detach(), k.detach(), v.detach(), args, bool(return_scores), False)
+  return O, P
+
+
+# ------------------------------------------------------------------------------------------------
 # K22 layer normalization: layers.LayerNormalization over the last axis
 # ------------------------------------------------------------------------------------------------
 def _layer_norm_fwd(x2, gamma, beta, eps, save):
