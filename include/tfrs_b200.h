@@ -811,9 +811,12 @@ int tfrs_text_spans(const uint8_t* scratch, const int64_t* offsets, int64_t n, c
  *     batch's moments, then one fold per channel); ws is tfrs_normalization_adapt_workspace_bytes bytes.
  *   tfrs_mean_pool_fwd: out [B, d] = sum_t x[b,t,:]*m[b,t] / sum_t m[b,t] (products and the sum in float32, t ascending
  *     from +0.0f; an all-masked row is 0/0), or without a mask sum_t x[b,t,:] / T.  x is addressed by element strides;
- *     mask [B, T] contiguous of mask_kind TFRS_I32 / TFRS_I64 / TFRS_BOOL (nonzero = kept), or NULL.  One launch.
+ *     mask [B, T] (a Keras mask, see TFRS_BOOL).  One launch.
  *   tfrs_mean_pool_bwd: dx [B, T, d] contiguous = f32(g[b,:] / sum_t m[b,t]) * m[b,t], or g[b,:] / T.  One launch.
  * ------------------------------------------------------------------------------------------- */
+/* A Keras mask crosses the ABI as (const void* mask, int mask_kind): a device array of kind TFRS_BOOL (one byte per
+ * element), TFRS_I32 or TFRS_I64, contiguous and row-major over the shape the entry names; nonzero = kept.  NULL keeps
+ * every element.  A non-NULL mask of another kind is TFRS_ERR_INVALID_ARG. */
 enum { TFRS_F32 = 3, TFRS_F64 = 4, TFRS_BOOL = 5 };
 
 int tfrs_bucketize(const void* x, int kind, int64_t n, const float* bounds, int64_t nb, int64_t* out, void* stream);
@@ -849,9 +852,8 @@ int tfrs_hashing(const void* values, const int64_t* offsets, int kind, int64_t n
  * gx = x.W + b_i ([B*T, 3u], row b*T + t) is the caller's, on K6 (tfrs_dense_fwd_f32 / tfrs_dense_bwd_f32).
  *   gr = h_{t-1}.U + b_r (fmaf chain over k ascending from +0.0f, then + b_r);  z = sigmoid(gx_z + gr_z),
  *   r = sigmoid(gx_r + gr_r),  hh = tanh(gx_h + r gr_h),  h_t = z h_{t-1} + (1 - z) hh;  sigmoid = 1 / (1 + expf(-x)).
- * h_0 = h0 [B, u], or zeros when h0 is NULL.  mask [B, T] (TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero = kept, nullable):
- * at a masked step h_t = h_{t-1} and nothing is computed.  1 <= units <= TFRS_GRU_MAX_UNITS, T >= 1, B < 2^31; B == 0
- * writes nothing.
+ * h_0 = h0 [B, u], or zeros when h0 is NULL.  mask [B, T] (a Keras mask, see TFRS_BOOL): at a masked step h_t = h_{t-1}
+ * and nothing is computed.  1 <= units <= TFRS_GRU_MAX_UNITS, T >= 1, B < 2^31; B == 0 writes nothing.
  *   tfrs_gru_fwd_f32: h_last [B, u] = h_T; out_seq [B, T, u] = every h_t (nullable); gates [B, T, 4u] = (z, r, hh, gr_h)
  *     and h_prev [B, T, u] = h_{t-1} (both or neither, for the backward; gates are not written at masked steps).
  *     One launch.
@@ -880,9 +882,9 @@ int tfrs_gru_bwd_f32(const float* U, const float* gates, const float* h_prev, co
  * gx = x.W + b ([B*T, 4u], row b*T + t) is the caller's, on K6 (tfrs_dense_fwd_f32 / tfrs_dense_bwd_f32).
  *   z = gx + h_{t-1}.U (fmaf chain over k ascending from +0.0f, then added to gx);  i = sigmoid(z_i), f = sigmoid(z_f),
  *   g = tanh(z_c), o = sigmoid(z_o);  c_t = f c_{t-1} + i g,  h_t = o tanh(c_t);  sigmoid = 1 / (1 + expf(-x)).
- * h_0 = h0 [B, u] and c_0 = c0 [B, u], each zeros when NULL.  mask [B, T] (TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero =
- * kept, nullable): at a masked step h_t = h_{t-1}, c_t = c_{t-1} and nothing is computed.  1 <= units <=
- * TFRS_LSTM_MAX_UNITS, T >= 1, B < 2^31; B == 0 writes nothing.
+ * h_0 = h0 [B, u] and c_0 = c0 [B, u], each zeros when NULL.  mask [B, T] (a Keras mask, see TFRS_BOOL): at a masked
+ * step h_t = h_{t-1}, c_t = c_{t-1} and nothing is computed.  1 <= units <= TFRS_LSTM_MAX_UNITS, T >= 1, B < 2^31;
+ * B == 0 writes nothing.
  *   tfrs_lstm_fwd_f32: h_last [B, u] = h_T and c_last [B, u] = c_T; out_seq [B, T, u] = every h_t (nullable); gates
  *     [B, T, 4u] = (i, f, g, o), c_seq [B, T, u] = every c_t and h_prev [B, T, u] = h_{t-1} (all three or none, for the
  *     backward; gates are not written at masked steps).  One launch.
@@ -912,8 +914,8 @@ int tfrs_lstm_bwd_f32(const float* U, const float* gates, const float* c_seq, co
  * in columns h*d .. h*d + d - 1, contiguous; they are read in place.  1 <= dk, dv <= TFRS_MHA_MAX_HEAD_DIM, T, S >= 1.
  *   scores s = (Q_h * scale) . K_h^T with scale = (float)(1 / sqrt(dk)) applied to Q in fp32 (Keras's order); where the
  *   combined mask drops (b, t, s), s += -1e9f (tf-keras Softmax), so a fully masked row is uniform; P = softmax over s;
- *   O_h = P . V_h.  masks (nullable; each mask pointer nullable, nonzero = kept, kinds TFRS_I32 / TFRS_I64 / TFRS_BOOL):
- *   query [B, T], value [B, S], key [B, S], attention [B, T, S], causal (keeps s <= t), combined by AND.
+ *   O_h = P . V_h.  masks (nullable; each a Keras mask, see TFRS_BOOL): query [B, T], value [B, S], key [B, S],
+ *   attention [B, T, S], causal (keeps s <= t), combined by AND.
  *   tfrs_mha_fwd_f32: O [B, T, H*dv]; stats [B, H, T, 2] = (row max m, row sum l of e^{s - m}) -- the log-sum-exp
  *     m + log l, kept as two numbers because a fully masked row's m = -1e9 leaves no fp32 room for log l (nullable; the
  *     backward needs it); P [B, H, T, S] = e^{s - m} / l (nullable).  One launch.
@@ -950,7 +952,7 @@ int tfrs_mha_bwd_f32(const float* Q, const float* K, const float* V, const TfrsM
  *   training call) the weights are dropped as K23 drops a [B, Tq, Tv] tensor: element e = (b Tq + i) Tv + j takes word
  *   e % 4 of Philox4x32-10 at counter (e/4 lo, e/4 hi, call lo, call hi) and key (seed lo, seed hi); keep <=> (word >>
  *   8) >= ceil(rate * 2^24); W = keep ? P * (float)(1 / (1 - rate)) : +0; else W = P.  O[b, i] = query_mask[b, i] *
- *   sum_j W_ij v_j.  Masks [B, Tq] / [B, Tv] nullable, kinds TFRS_I32 / TFRS_I64 / TFRS_BOOL, nonzero = kept.
+ *   sum_j W_ij v_j.  query_mask [B, Tq] and value_mask [B, Tv] (Keras masks, see TFRS_BOOL).
  *   tfrs_dense_attention_fwd_f32: O [B, Tq, dv]; stats [B, Tq, 2] = (row max, row sum of e^{s - max}) (nullable; the
  *     backward needs it); P [B, Tq, Tv] = W (nullable).  One launch.
  *   tfrs_dense_attention_bwd_f32: from dO and the forward's O and stats: dQ, dK [B, Tv, dim], dV; dscale ([1], or [dim]
@@ -1019,10 +1021,9 @@ int tfrs_dropout_f32(const float* x, int rank, const int64_t* shape, const int64
 
 /* ---------------------------------------------------------------------------------------------
  * K24 batch normalization: tf.keras.layers.BatchNormalization(axis=-1) over the rows of x [N, d] (N >= 1, d >= 1; the
- * statistics are per column).  gamma / beta [d] nullable (scale / center off).  mask [N] (TFRS_I32 / TFRS_I64 /
- * TFRS_BOOL, nonzero = kept, nullable) restricts the batch moments to the kept rows (weighted moments, n = sum w); n = 0
- * gives mean 0 and variance 0.  Every sum runs in a fixed order over a row chunking that depends on (N, d) only: no
- * float atomics, bitwise reproducible.
+ * statistics are per column).  gamma / beta [d] nullable (scale / center off).  mask [N] (a Keras mask, see TFRS_BOOL)
+ * restricts the batch moments to the kept rows (weighted moments, n = sum w); n = 0 gives mean 0 and variance 0.  Every
+ * sum runs in a fixed order over a row chunking that depends on (N, d) only: no float atomics, bitwise reproducible.
  *   training: the batch mean as the fp32 pair hi = f32(mean), lo = f32(mean - hi) (per-chunk shifted sums folded in
  *     fp64), the population variance var, rstd = 1 / sqrtf(var + eps), y = ((x - hi) - lo) rstd gamma + beta; the
  *     moving statistics updated in place with decay = f32(1 - momentum): mm = mm - (mm - f32(hi + lo)) decay, mv = mv

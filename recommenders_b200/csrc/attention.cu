@@ -16,9 +16,7 @@ static int mha_check(const char* what, int64_t B, int64_t T, int64_t S, int H, i
   if (m) {
     const void* ps[4] = {m->query, m->value, m->key, m->attention};
     const int ks[4] = {m->query_kind, m->value_kind, m->key_kind, m->attention_kind};
-    for (int i = 0; i < 4; ++i)
-      TFRS_CHECK_ARG(!ps[i] || ks[i] == TFRS_I32 || ks[i] == TFRS_I64 || ks[i] == TFRS_BOOL,
-                     "%s: a mask must be I32, I64 or BOOL", what);
+    for (int i = 0; i < 4; ++i) TFRS_CHECK_MASK(what, ps[i], ks[i]);
   }
   return TFRS_OK;
 }

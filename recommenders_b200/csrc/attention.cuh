@@ -57,26 +57,20 @@ struct MhaArgs {
   float* part;                                            // per query row: the score weights' gradient partials
 };
 
-__device__ __forceinline__ bool mha_mask_at(const void* m, int kind, long long i) {
-  if (kind == TFRS_BOOL) return static_cast<const uint8_t*>(m)[i] != 0;
-  if (kind == TFRS_I32) return static_cast<const int32_t*>(m)[i] != 0;
-  return static_cast<const long long*>(m)[i] != 0;
-}
-
 // score (b, t, s) kept by every mask present (tf-keras _compute_attention_mask: query & value & key & causal & attention)
 __device__ __forceinline__ bool mha_keep(const MhaArgs& a, long long b, int t, int s) {
   const TfrsMhaMasks& m = a.m;
-  if (m.query && !mha_mask_at(m.query, m.query_kind, b * a.T + t)) return false;
-  if (m.value && !mha_mask_at(m.value, m.value_kind, b * a.S + s)) return false;
-  if (m.key && !mha_mask_at(m.key, m.key_kind, b * a.S + s)) return false;
+  if (m.query && !mask_kept(m.query, m.query_kind, b * a.T + t)) return false;
+  if (m.value && !mask_kept(m.value, m.value_kind, b * a.S + s)) return false;
+  if (m.key && !mask_kept(m.key, m.key_kind, b * a.S + s)) return false;
   if (m.causal && s > t) return false;
-  if (m.attention && !mha_mask_at(m.attention, m.attention_kind, (b * a.T + t) * a.S + s)) return false;
+  if (m.attention && !mask_kept(m.attention, m.attention_kind, (b * a.T + t) * a.S + s)) return false;
   return true;
 }
 
 // the dense modes: query row r = b * T + t keeps its output
 __device__ __forceinline__ bool dense_out_kept(const MhaArgs& a, long long r) {
-  return !a.omask || mha_mask_at(a.omask, a.omask_kind, r);
+  return !a.omask || mask_kept(a.omask, a.omask_kind, r);
 }
 
 // the sum of x over the team's 8 lanes, in every lane (fixed butterfly order)

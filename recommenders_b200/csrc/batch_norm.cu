@@ -22,13 +22,6 @@ constexpr int BN_WARPS = BN_THREADS / 32;
 constexpr long long BN_MIN_CHUNK = 32;      // rows per CTA, at least
 constexpr long long BN_TARGET_CTAS = 2048;  // row chunks x column tiles, about two waves of 8 CTAs per SM on an H100
 
-__device__ __forceinline__ bool bn_kept(const void* m, int kind, long long r) {
-  if (!m) return true;
-  if (kind == TFRS_BOOL) return static_cast<const uint8_t*>(m)[r] != 0;
-  if (kind == TFRS_I32) return static_cast<const int32_t*>(m)[r] != 0;
-  return static_cast<const long long*>(m)[r] != 0;
-}
-
 struct BnRows {
   long long c, r0, r1;
   int warp, lane;
@@ -71,7 +64,7 @@ bn_stats_kernel(const float* __restrict__ x, const void* __restrict__ mask, int 
     rk = b.r1;
     for (long long base = b.r0; base < b.r1; base += BN_THREADS) {
       const long long r = base + threadIdx.x;
-      const int kept = r < b.r1 && bn_kept(mask, mk, r);
+      const int kept = r < b.r1 && mask_kept(mask, mk, r);
       if (__syncthreads_or(kept)) {
         if (kept) atomicMin(&first, (int)threadIdx.x);
         __syncthreads();
@@ -85,7 +78,7 @@ bn_stats_kernel(const float* __restrict__ x, const void* __restrict__ mask, int 
     K = x[rk * d + b.c];
 #pragma unroll 4
     for (long long r = b.r0 + b.warp; r < b.r1; r += BN_WARPS) {
-      if (bn_kept(mask, mk, r)) {
+      if (!mask || mask_kept(mask, mk, r)) {
         const float t = x[r * d + b.c] - K;
         s1 += t;
         s2 = fmaf(t, t, s2);
@@ -240,7 +233,7 @@ bn_bwd_dx_kernel(const float* __restrict__ x, const void* __restrict__ mask, int
 #pragma unroll 4
   for (long long r = b.r0 + b.warp; r < b.r1; r += BN_WARPS) {
     const float g = dy[r * d + b.c];
-    const float u = bn_kept(mask, mk, r) ? g - (s1n + ((x[r * d + b.c] - hi) - lo) * rs * s2n) : g;
+    const float u = !mask || mask_kept(mask, mk, r) ? g - (s1n + ((x[r * d + b.c] - hi) - lo) * rs * s2n) : g;
     dx[r * d + b.c] = k * u;
   }
 }
@@ -273,8 +266,7 @@ extern "C" int tfrs_batch_norm_fwd_f32(const float* x, const void* mask, int mas
                                        size_t ws_bytes, void* stream) {
   TFRS_CHECK_ARG(bn_shape_ok(N, d), "batch_norm_fwd: bad shape N=%lld d=%lld", (long long)N, (long long)d);
   TFRS_CHECK_ARG(x && y && moving_mean && moving_var, "batch_norm_fwd: NULL pointer");
-  TFRS_CHECK_ARG(!mask || mask_kind == TFRS_I32 || mask_kind == TFRS_I64 || mask_kind == TFRS_BOOL,
-                 "batch_norm_fwd: the mask must be I32, I64 or BOOL");
+  TFRS_CHECK_MASK("batch_norm_fwd", mask, mask_kind);
   TFRS_CHECK_ARG(eps >= 0.f, "batch_norm_fwd: epsilon must be >= 0");
   cudaStream_t st = (cudaStream_t)stream;
   long long chunk, parts;
@@ -321,8 +313,7 @@ extern "C" int tfrs_batch_norm_bwd_f32(const float* x, const void* mask, int mas
                                        float* dx, float* dparams, void* ws, size_t ws_bytes, void* stream) {
   TFRS_CHECK_ARG(bn_shape_ok(N, d), "batch_norm_bwd: bad shape N=%lld d=%lld", (long long)N, (long long)d);
   TFRS_CHECK_ARG(x && saved && dy && dparams, "batch_norm_bwd: NULL pointer");
-  TFRS_CHECK_ARG(!mask || mask_kind == TFRS_I32 || mask_kind == TFRS_I64 || mask_kind == TFRS_BOOL,
-                 "batch_norm_bwd: the mask must be I32, I64 or BOOL");
+  TFRS_CHECK_MASK("batch_norm_bwd", mask, mask_kind);
   if (!ws || ws_bytes < tfrs_batch_norm_bwd_workspace_bytes(N, d)) {
     set_error("batch_norm_bwd: workspace too small");
     return TFRS_ERR_WORKSPACE_TOO_SMALL;

@@ -40,6 +40,33 @@ void count_launch(int n = 1);
     }                                                                                            \
   } while (0)
 
+// ---- Keras masks (include/tfrs_b200.h): kind TFRS_BOOL / TFRS_I32 / TFRS_I64, nonzero = kept, NULL keeps everything
+#define TFRS_CHECK_MASK(what, mask, kind)                                                     \
+  TFRS_CHECK_ARG(!(mask) || (kind) == TFRS_I32 || (kind) == TFRS_I64 || (kind) == TFRS_BOOL, \
+                 "%s: a mask must be I32, I64 or BOOL", what)
+
+// element i of a mask of element type M (uint8_t for BOOL, int32_t, long long), true for a NULL mask
+template <typename M>
+__device__ __forceinline__ bool mask_kept(const void* m, long long i) {
+  return m == nullptr || static_cast<const M*>(m)[i] != 0;
+}
+
+// element i of a non-NULL mask of a runtime kind.  Callers test for NULL themselves: folding that test in here changes
+// the code of the K21 and K25 kernels.
+__device__ __forceinline__ bool mask_kept(const void* m, int kind, long long i) {
+  if (kind == TFRS_BOOL) return static_cast<const uint8_t*>(m)[i] != 0;
+  if (kind == TFRS_I32) return static_cast<const int32_t*>(m)[i] != 0;
+  return static_cast<const long long*>(m)[i] != 0;
+}
+
+// f(M{}) with M the element type of a checked mask; no mask runs the uint8_t instance
+template <typename F>
+static int mask_dispatch(const void* mask, int kind, F f) {
+  if (!mask || kind == TFRS_BOOL) return f(uint8_t{});
+  if (kind == TFRS_I32) return f(int32_t{});
+  return f((long long)0);
+}
+
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -149,9 +149,6 @@ ft_update_kernel(const T* __restrict__ x, long long N, long long R, long long C,
 
 // ---- masked mean pooling --------------------------------------------------------------------------------------------
 template <typename M>
-__device__ __forceinline__ float ft_keep(const M* mask, long long i) { return mask[i] != 0 ? 1.f : 0.f; }
-
-template <typename M>
 __global__ void __launch_bounds__(FT_THREADS)
 ft_pool_fwd_kernel(const float* __restrict__ x, long long B, long long T, long long d, long long sb, long long st,
                    long long sd, const M* __restrict__ mask, float* __restrict__ out) {
@@ -162,7 +159,7 @@ ft_pool_fwd_kernel(const float* __restrict__ x, long long B, long long T, long l
   float s = 0.f, c = 0.f;
   for (long long t = 0; t < T; ++t) {
     if (mask) {
-      const float m = ft_keep(mask, b * T + t);
+      const float m = mask_kept<M>(mask, b * T + t) ? 1.f : 0.f;
       s = __fadd_rn(s, __fmul_rn(__ldg(xp + t * st), m));
       c = __fadd_rn(c, m);
     } else {
@@ -182,11 +179,11 @@ ft_pool_bwd_kernel(const float* __restrict__ g, long long B, long long T, long l
   float c = (float)T;
   if (mask) {
     c = 0.f;
-    for (long long t = 0; t < T; ++t) c = __fadd_rn(c, ft_keep(mask, b * T + t));
+    for (long long t = 0; t < T; ++t) c = __fadd_rn(c, mask_kept<M>(mask, b * T + t) ? 1.f : 0.f);
   }
   const float q = __fdiv_rn(g[i], c);
   float* dp = dx + b * T * d + k;
-  for (long long t = 0; t < T; ++t) dp[t * d] = mask ? __fmul_rn(q, ft_keep(mask, b * T + t)) : q;
+  for (long long t = 0; t < T; ++t) dp[t * d] = mask ? __fmul_rn(q, mask_kept<M>(mask, b * T + t) ? 1.f : 0.f) : q;
 }
 
 template <typename M>
@@ -204,14 +201,12 @@ static int ft_pool_any(const float* x, long long B, long long T, long long d, lo
   const char* what = bwd ? "mean_pool_bwd" : "mean_pool_fwd";
   TFRS_CHECK_ARG(B >= 0 && T >= 0 && d >= 0 && B * d < (1ll << 40) && B * T < (1ll << 40) && B * T * d < (1ll << 46),
                  "%s: bad shape [%lld, %lld, %lld]", what, B, T, d);
-  TFRS_CHECK_ARG(!mask || mask_kind == TFRS_I32 || mask_kind == TFRS_I64 || mask_kind == TFRS_BOOL,
-                 "%s: the mask must be I32, I64 or BOOL", what);
+  TFRS_CHECK_MASK(what, mask, mask_kind);
   if (B * d == 0) return TFRS_OK;
   // an empty time axis leaves x (forward) or dx (backward) empty, and possibly NULL
   TFRS_CHECK_ARG(bwd ? x && (out || T == 0) : out && (x || T == 0), "%s: NULL input or output", what);
-  if (!mask || mask_kind == TFRS_BOOL) return ft_pool<uint8_t>(x, B, T, d, sb, st, sd, mask, out, bwd, s);
-  if (mask_kind == TFRS_I32) return ft_pool<int32_t>(x, B, T, d, sb, st, sd, mask, out, bwd, s);
-  return ft_pool<long long>(x, B, T, d, sb, st, sd, mask, out, bwd, s);
+  return mask_dispatch(mask, mask_kind,
+                       [&](auto m) { return ft_pool<decltype(m)>(x, B, T, d, sb, st, sd, mask, out, bwd, s); });
 }
 
 static bool ft_kind(int kind) { return kind == TFRS_I32 || kind == TFRS_I64 || kind == TFRS_F32 || kind == TFRS_F64; }

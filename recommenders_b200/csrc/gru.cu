@@ -94,7 +94,7 @@ gru_fwd_kernel(const GruFwdArgs p) {
       const long long b = b0 + row;
       if (b >= p.B) continue;
       const long long o = b * p.T + t;
-      const bool keep = rnn_keep<M>(p.mask, o);
+      const bool keep = mask_kept<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;
@@ -158,7 +158,7 @@ gru_bwd_kernel(const GruBwdArgs p) {
       const long long b = b0 + row;
       const bool valid = b < p.B;
       const long long o = b * p.T + t;
-      keep[i] = valid && rnn_keep<M>(p.mask, o);
+      keep[i] = valid && mask_kept<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;

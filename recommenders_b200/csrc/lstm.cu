@@ -108,7 +108,7 @@ lstm_fwd_kernel(const LstmFwdArgs p) {
       const long long b = b0 + row;
       if (b >= p.B) continue;
       const long long o = b * p.T + t;
-      const bool keep = rnn_keep<M>(p.mask, o);
+      const bool keep = mask_kept<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;
@@ -177,7 +177,7 @@ lstm_bwd_kernel(const LstmBwdArgs p) {
       const long long b = b0 + row;
       const bool valid = b < p.B;
       const long long o = b * p.T + t;
-      keep[i] = valid && rnn_keep<M>(p.mask, o);
+      keep[i] = valid && mask_kept<M>(p.mask, o);
 #pragma unroll
       for (int a = 0; a < UJ; ++a) {
         const int j = j0 + JT * a;

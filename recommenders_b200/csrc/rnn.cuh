@@ -1,7 +1,7 @@
 // rnn.cuh -- what the recurrence kernels K19 (gru.cu) and K20 (lstm.cu) share: the gate arithmetic, the plan of a
-// CTA's (row, unit) pairs, the mask test, the shared-memory budget and the choice of kernel instance.  Nothing here
-// depends on the cell; each file brings its own kernels.  The gate derivatives are taken from the saved gate OUTPUTS,
-// as TF's SigmoidGrad / TanhGrad do.
+// CTA's (row, unit) pairs, the shared-memory budget and the choice of kernel instance.  Nothing here depends on the
+// cell; each file brings its own kernels.  The gate derivatives are taken from the saved gate OUTPUTS, as TF's
+// SigmoidGrad / TanhGrad do.
 #pragma once
 #include "dense.cuh"
 
@@ -36,12 +36,6 @@ static inline RnnTile rnn_tile(int u) {
   return t;
 }
 
-// step i of the [B, T] mask is kept (no mask keeps every step)
-template <typename M>
-__device__ __forceinline__ bool rnn_keep(const void* mask, long long i) {
-  return mask == nullptr || static_cast<const M*>(mask)[i] != 0;
-}
-
 // shared memory of one CTA: the fixed part plus a weight matrix of `rows_total` rows of `per` floats, whole when it
 // fits in the 227 KB, otherwise in slices of RNN_SLICE_BYTES (*slice_rows rows)
 static inline void rnn_smem(int fixed_floats, int rows_total, int per, int* slice_rows, size_t* bytes) {
@@ -69,13 +63,12 @@ static int rnn_tiles(const char* what, int uj, const A& a, unsigned grid, size_t
   return TFRS_ERR_INVALID_ARG;
 }
 
-// ... and for the mask's element type (no mask runs the BOOL instance with a NULL mask)
+// ... and for the mask's element type
 template <template <typename, int, int> class L, typename A>
 static int rnn_dispatch(const char* what, int mask_kind, int uj, const A& a, unsigned grid, size_t smem,
                         cudaStream_t st) {
-  if (!a.mask || mask_kind == TFRS_BOOL) return rnn_tiles<L, uint8_t>(what, uj, a, grid, smem, st);
-  if (mask_kind == TFRS_I32) return rnn_tiles<L, int32_t>(what, uj, a, grid, smem, st);
-  return rnn_tiles<L, long long>(what, uj, a, grid, smem, st);
+  return mask_dispatch(a.mask, mask_kind,
+                       [&](auto m) { return rnn_tiles<L, decltype(m)>(what, uj, a, grid, smem, st); });
 }
 
 static inline int rnn_check(const char* what, int64_t B, int64_t T, int u, int max_units, const void* mask,
@@ -83,8 +76,7 @@ static inline int rnn_check(const char* what, int64_t B, int64_t T, int u, int m
   TFRS_CHECK_ARG(B >= 0 && B < (1ll << 31) && T >= 1 && T < (1ll << 31) && u >= 1 && u <= max_units,
                  "%s: bad shape B=%lld T=%lld units=%d (1 <= units <= %d, T >= 1)", what, (long long)B, (long long)T, u,
                  max_units);
-  TFRS_CHECK_ARG(!mask || mask_kind == TFRS_I32 || mask_kind == TFRS_I64 || mask_kind == TFRS_BOOL,
-                 "%s: the mask must be I32, I64 or BOOL", what);
+  TFRS_CHECK_MASK(what, mask, mask_kind);
   return TFRS_OK;
 }
 

@@ -44,12 +44,6 @@ class _Projection(torch.nn.Module):
     self.bias = None if bias is None else torch.nn.Parameter(bias)
 
 
-def _as_mask(mask, device):
-  if mask is None or isinstance(mask, torch.Tensor):
-    return mask
-  return torch.from_numpy(np.ascontiguousarray(mask)).to(device)
-
-
 class MultiHeadAttention(torch.nn.Module):
   """`tf.keras.layers.MultiHeadAttention(num_heads, key_dim)`: `layer(query, value, key=None)` with query [B, T, D_q],
   value [B, S, D_v], key [B, S, D_k] (key = value when None) -> [B, T, D_out] (D_out = D_q unless `output_shape`), and
@@ -130,19 +124,17 @@ class MultiHeadAttention(torch.nn.Module):
         raise NotImplementedError(f"MultiHeadAttention: {name} of rank {rank} is not supported (rank 3 only)")
     if not self.built:
       self.build(query.shape, value.shape, None if key is None else key.shape, query.device)
-    dev = query.device
-    query_mask = ops.attached_mask(query) if query_mask is None else _as_mask(query_mask, dev)
-    value_mask = ops.attached_mask(value) if value_mask is None else _as_mask(value_mask, dev)
-    if key_mask is None and key is not None:
-      key_mask = ops.attached_mask(key)
-    key_mask = _as_mask(key_mask, dev)
-    attention_mask = _as_mask(attention_mask, dev)
+    query_mask = ops.layer_mask(query, query_mask)
+    value_mask = ops.layer_mask(value, value_mask)
+    if key is not None or key_mask is not None:   # no key: value_mask already holds the mask attached to value
+      key_mask = ops.layer_mask(value if key is None else key, key_mask)
+    if attention_mask is not None:
+      attention_mask = ops.layer_mask(query, attention_mask)
     p = (self.query, self.key, self.value, self.attention_output)
     out, scores = ops.attention(query, value, key, *(w.kernel for w in p), *(w.bias for w in p), query_mask=query_mask,
                                 value_mask=value_mask, key_mask=key_mask, attention_mask=attention_mask,
                                 causal=bool(use_causal_mask), return_scores=bool(return_attention_scores))
-    if query_mask is not None:
-      out._tfrs_mask = (query_mask, out._version, out.data_ptr())
+    ops.attach_mask(out, query_mask)
     return (out, scores) if return_attention_scores else out
 
   def forward(self, query, value, key=None, attention_mask=None, return_attention_scores: bool = False, training=None,
@@ -209,10 +201,8 @@ class _BaseDenseAttention(torch.nn.Module):
                          f"{tuple(t.shape) if isinstance(t, torch.Tensor) else type(t)}")
     if not self.built:
       self.build(int(query.shape[-1]), query.device)
-    dev = query.device
     q_mask, v_mask = (None, None) if mask is None else (mask[0], mask[1])
-    q_mask = ops.attached_mask(query) if q_mask is None else _as_mask(q_mask, dev)
-    v_mask = ops.attached_mask(value) if v_mask is None else _as_mask(v_mask, dev)
+    q_mask, v_mask = ops.layer_mask(query, q_mask), ops.layer_mask(value, v_mask)
     rate, call = 0.0, 0
     if self.dropout > 0 and resolve_training(training):
       rate, call = self.dropout, self._calls
@@ -221,8 +211,7 @@ class _BaseDenseAttention(torch.nn.Module):
     out, weights = ops.dense_attention(query, key, value, mode, scale, cw, query_mask=q_mask, value_mask=v_mask,
                                        causal=self.causal or bool(use_causal_mask), rate=rate, seed=self._key,
                                        call=call, return_scores=bool(return_attention_scores))
-    if q_mask is not None:
-      out._tfrs_mask = (q_mask, out._version, out.data_ptr())
+    ops.attach_mask(out, q_mask)
     return (out, weights) if return_attention_scores else out
 
   def forward(self, inputs, mask=None, training=None, return_attention_scores: bool = False,

@@ -69,9 +69,7 @@ class Embedding(torch.nn.Module):
     else:
       out = ops.gather([self.weight], [flat])
     out = out.reshape(*shape, self.output_dim)
-    if self.mask_zero:
-      out._tfrs_mask = (ids, out._version, out.data_ptr())     # the ids themselves: nonzero = kept
-    return out
+    return ops.attach_mask(out, ids if self.mask_zero else None)     # the ids themselves: nonzero = kept
 
   def pop_sparse_grads(self):
     g, self._sparse_grads = self._sparse_grads, []

@@ -58,10 +58,7 @@ class LayerNormalization(torch.nn.Module):
       self.build(inputs.shape, inputs.device)
     self._check_axis(inputs.dim())
     mask = ops.attached_mask(inputs)
-    y = ops.layer_norm(inputs, self.gamma, self.beta, self.epsilon)
-    if mask is not None:
-      y._tfrs_mask = (mask, y._version, y.data_ptr())
-    return y
+    return ops.attach_mask(ops.layer_norm(inputs, self.gamma, self.beta, self.epsilon), mask)
 
   def forward(self, inputs, training=None):
     return self.call(inputs, training=training)
@@ -146,15 +143,10 @@ class BatchNormalization(torch.nn.Module):
     if not self.built:
       self.build(inputs.shape, inputs.device)
     self._check_axis(inputs.dim())
-    if mask is None:
-      mask = ops.attached_mask(inputs)
-    elif not isinstance(mask, torch.Tensor):
-      mask = torch.as_tensor(mask, device=inputs.device)
+    mask = ops.layer_mask(inputs, mask)
     y = ops.batch_norm(inputs, self.gamma, self.beta, self.moving_mean, self.moving_variance,
                        resolve_training(training), self.momentum, self.epsilon, mask)
-    if mask is not None:
-      y._tfrs_mask = (mask, y._version, y.data_ptr())
-    return y
+    return ops.attach_mask(y, mask)
 
   def forward(self, inputs, training=None, mask=None):
     return self.call(inputs, training=training, mask=mask)

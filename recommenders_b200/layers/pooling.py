@@ -5,7 +5,6 @@ from __future__ import annotations
 
 from typing import Any, Dict
 
-import numpy as np
 import torch
 
 from .. import ops
@@ -26,11 +25,7 @@ class GlobalAveragePooling1D(torch.nn.Module):
     self.data_format, self.keepdims, self.name = data_format, bool(keepdims), name
 
   def forward(self, inputs: torch.Tensor, mask=None) -> torch.Tensor:
-    if mask is None:
-      mask = ops.attached_mask(inputs)
-    elif not isinstance(mask, torch.Tensor):
-      mask = torch.from_numpy(np.ascontiguousarray(mask)).to(inputs.device)
-    out = ops.mean_pool(inputs, mask)
+    out = ops.mean_pool(inputs, ops.layer_mask(inputs, mask))
     return out.unsqueeze(1) if self.keepdims else out
 
   def get_config(self) -> Dict[str, Any]:

@@ -68,10 +68,7 @@ class GRU(torch.nn.Module):
   def call(self, inputs: torch.Tensor, mask=None, training=None, initial_state=None):
     if not self.built:
       self.build(inputs.shape, inputs.device if isinstance(inputs, torch.Tensor) else None)
-    if mask is None:
-      mask = ops.attached_mask(inputs)
-    elif not isinstance(mask, torch.Tensor):
-      mask = torch.from_numpy(np.ascontiguousarray(mask)).to(inputs.device)
+    mask = ops.layer_mask(inputs, mask)
     if isinstance(initial_state, (list, tuple)):
       if len(initial_state) != 1:
         raise ValueError(f"GRU: expected one initial state, got {len(initial_state)}")
@@ -159,10 +156,7 @@ class LSTM(torch.nn.Module):
   def call(self, inputs: torch.Tensor, mask=None, training=None, initial_state=None):
     if not self.built:
       self.build(inputs.shape, inputs.device if isinstance(inputs, torch.Tensor) else None)
-    if mask is None:
-      mask = ops.attached_mask(inputs)
-    elif not isinstance(mask, torch.Tensor):
-      mask = torch.from_numpy(np.ascontiguousarray(mask)).to(inputs.device)
+    mask = ops.layer_mask(inputs, mask)
     if initial_state is not None and (isinstance(initial_state, torch.Tensor) or len(initial_state) != 2):
       n = 1 if isinstance(initial_state, torch.Tensor) else len(initial_state)
       raise ValueError(f"LSTM: expected two initial states [h_0, c_0], got {n}")

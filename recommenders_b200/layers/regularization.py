@@ -49,10 +49,7 @@ class Dropout(torch.nn.Module):
     mask = ops.attached_mask(inputs)
     call = self._calls
     self._calls += 1
-    y = ops.dropout(inputs, self.rate, self._key, call, noise)
-    if mask is not None:
-      y._tfrs_mask = (mask, y._version, y.data_ptr())
-    return y
+    return ops.attach_mask(ops.dropout(inputs, self.rate, self._key, call, noise), mask)
 
   def forward(self, inputs, training=None):
     return self.call(inputs, training=training)

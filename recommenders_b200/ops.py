@@ -1620,6 +1620,19 @@ def dense_uses_tc(B: int, K: int, N: int) -> bool:
   return bool(lib().tfrs_dense_uses_tc(B, K, N))
 
 
+def _attach(y: torch.Tensor, attr: str, value: torch.Tensor) -> None:
+  """Hangs `value` on `y` as `attr`, valid while `y` is that very tensor, unmodified (its `_version` and `data_ptr`)."""
+  setattr(y, attr, (value, y._version, y.data_ptr()))
+
+
+def _attached(x: torch.Tensor, attr: str, shape) -> Optional[torch.Tensor]:
+  """The value `_attach` hung on `x` as `attr`, if it is still valid and has `shape`."""
+  hint = getattr(x, attr, None)
+  if hint is not None and hint[1] == x._version and hint[2] == x.data_ptr() and tuple(hint[0].shape) == tuple(shape):
+    return hint[0]
+  return None
+
+
 def dense(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor] = None, activation: Optional[str] = None) -> torch.Tensor:
   """act(x @ W + bias), W [in, out] (tf.keras.layers.Dense); activation None / "linear" / "relu" / "sigmoid" run fused.
 
@@ -1636,16 +1649,13 @@ def dense(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor] = None,
     y = y.reshape(*lead, y.shape[-1])
     z = z.reshape(*lead, z.shape[-1]) if act == ACT_SIGMOID else z
   if act == ACT_SIGMOID:
-    y._tfrs_logits = (z, y._version, y.data_ptr())
+    _attach(y, "_tfrs_logits", z)
   return y
 
 
 def attached_logits(pred: torch.Tensor) -> Optional[torch.Tensor]:
   """The logits a fused sigmoid Dense attached to `pred`, if `pred` is that very tensor, unmodified."""
-  hint = getattr(pred, "_tfrs_logits", None)
-  if hint is not None and hint[1] == pred._version and hint[2] == pred.data_ptr() and hint[0].shape == pred.shape:
-    return hint[0]
-  return None
+  return _attached(pred, "_tfrs_logits", pred.shape)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -2065,14 +2075,16 @@ def normalization_adapt(x: torch.Tensor, C: int, batch_rows: int, state: torch.T
         "normalization_adapt")
 
 
-def _mask_arg(mask: Optional[torch.Tensor], B: int, T: int, op: str = "mean_pool"):
+def _mask_arg(mask: Optional[torch.Tensor], shape, op: str, name: str = "the mask"):
+  """(mask, kind) for a kernel's (const void* mask, int mask_kind): a Keras mask (bool / int32 / int64, CUDA, nonzero =
+  kept) of exactly `shape`, made contiguous; (None, 0) for no mask."""
   if mask is None:
     return None, 0
-  require_cuda(mask, "mask")
+  require_cuda(mask, name)
   if mask.dtype not in _MASK_KINDS:
-    raise TypeError(f"{op}: the mask must be bool, int32 or int64, got {mask.dtype}")
-  if tuple(mask.shape) != (B, T):
-    raise ValueError(f"{op}: the mask has shape {tuple(mask.shape)}, the input [{B}, {T}, d]")
+    raise TypeError(f"{op}: {name} must be bool, int32 or int64, got {mask.dtype}")
+  if tuple(mask.shape) != tuple(shape):
+    raise ValueError(f"{op}: {name} has shape {tuple(mask.shape)}, expected {tuple(shape)}")
   return mask.contiguous(), _MASK_KINDS[mask.dtype]
 
 
@@ -2081,7 +2093,7 @@ class _MeanPool(torch.autograd.Function):
   @staticmethod
   def forward(ctx, x, mask):
     B, T, d = x.shape
-    m, mk = _mask_arg(mask, B, T)
+    m, mk = _mask_arg(mask, (B, T), "mean_pool")
     out = torch.empty((B, d), dtype=torch.float32, device=x.device)
     check(lib().tfrs_mean_pool_fwd(ptr(x), B, T, d, x.stride(0), x.stride(1), x.stride(2), ptr(m), mk, ptr(out),
                                    stream()), "mean_pool_fwd")
@@ -2112,10 +2124,25 @@ def mean_pool(x: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Ten
 def attached_mask(x: torch.Tensor) -> Optional[torch.Tensor]:
   """The mask (the ids, nonzero = kept) an Embedding with mask_zero=True attached to its output `x`, if `x` is that very
   tensor, unmodified."""
-  hint = getattr(x, "_tfrs_mask", None)
-  if hint is not None and hint[1] == x._version and hint[2] == x.data_ptr() and tuple(hint[0].shape) == tuple(x.shape[:-1]):
-    return hint[0]
-  return None
+  return _attached(x, "_tfrs_mask", x.shape[:-1])
+
+
+def attach_mask(y: torch.Tensor, mask: Optional[torch.Tensor]) -> torch.Tensor:
+  """Attaches `mask` (y.shape[:-1], nonzero = kept) to a layer's output `y` for `attached_mask`; None attaches nothing.
+  Returns `y`."""
+  if mask is not None:
+    _attach(y, "_tfrs_mask", mask)
+  return y
+
+
+def layer_mask(x: torch.Tensor, mask=None) -> Optional[torch.Tensor]:
+  """The mask a layer applies to its input `x`: `mask` when one is passed (an array or list becomes a tensor on x's
+  device), else the mask attached to `x`, if any."""
+  if mask is None:
+    return attached_mask(x)
+  if isinstance(mask, torch.Tensor):
+    return mask
+  return torch.from_numpy(np.ascontiguousarray(mask)).to(x.device)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -2201,7 +2228,7 @@ def gru(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, b
     raise ValueError(f"gru: initial_state must be [{B}, {u}], got {tuple(initial_state.shape)}")
   if mask is not None and return_sequences:
     raise NotImplementedError("gru: a mask together with return_sequences=True is not supported")
-  m, mk = _mask_arg(mask, B, T, "gru")
+  m, mk = _mask_arg(mask, (B, T), "gru")
   gx = dense(x.reshape(B * T, D), kernel, None if bias is None else bias[0]).reshape(B, T, 3 * u)
   U = f32c(recurrent_kernel, "recurrent_kernel")
   b_r = None if bias is None else f32c(bias[1], "bias")
@@ -2303,7 +2330,7 @@ def lstm(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, 
     h0, c0 = (f32c(s, "initial_state") for s in initial_state)
   if mask is not None and return_sequences:
     raise NotImplementedError("lstm: a mask together with return_sequences=True is not supported")
-  m, mk = _mask_arg(mask, B, T, "lstm")
+  m, mk = _mask_arg(mask, (B, T), "lstm")
   gx = dense(x.reshape(B * T, D), kernel, bias).reshape(B, T, 4 * u)
   U = f32c(recurrent_kernel, "recurrent_kernel")
   if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, h0, c0)):
@@ -2325,22 +2352,12 @@ class _MhaMasks(ctypes.Structure):
               ("attention", c_p), ("attention_kind", c_i), ("causal", c_i)]
 
 
-def _mha_mask(mask, shape, name: str):
-  if mask is None:
-    return None
-  require_cuda(mask, name)
-  if mask.dtype not in _MASK_KINDS:
-    raise TypeError(f"attention: {name} must be bool, int32 or int64, got {mask.dtype}")
-  if tuple(mask.shape) != tuple(shape):
-    raise ValueError(f"attention: {name} has shape {tuple(mask.shape)}, expected {list(shape)}")
-  return mask.contiguous()
-
-
 def _mha_masks(masks, causal: bool) -> _MhaMasks:
+  """masks: the query, value, key and attention masks as _mask_arg's (mask, kind) pairs."""
   s = _MhaMasks()
-  for name, m in zip(("query", "value", "key", "attention"), masks):
-    setattr(s, name, None if m is None else m.data_ptr())
-    setattr(s, name + "_kind", _MASK_KINDS[m.dtype] if m is not None else 0)
+  for name, (m, kind) in zip(("query", "value", "key", "attention"), masks):
+    setattr(s, name, ptr(m))
+    setattr(s, name + "_kind", kind)
   s.causal = int(bool(causal))
   return s
 
@@ -2361,18 +2378,18 @@ class _AttentionCore(torch.autograd.Function):
   not differentiable."""
 
   @staticmethod
-  def forward(ctx, Q, K, V, H, dk, dv, qm, vm, km, am, causal, want_p):
-    O, stats, P = _attention_fwd(Q, K, V, H, dk, dv, (qm, vm, km, am), causal, want_p, True)
+  def forward(ctx, Q, K, V, H, dk, dv, masks, causal, want_p):
+    O, stats, P = _attention_fwd(Q, K, V, H, dk, dv, masks, causal, want_p, True)
     P = P if want_p else torch.empty((0,), dtype=torch.float32, device=Q.device)
-    ctx.save_for_backward(Q, K, V, O, stats, qm, vm, km, am)
-    ctx.shape, ctx.causal = (H, dk, dv), causal
+    ctx.save_for_backward(Q, K, V, O, stats, *(m for m, _ in masks))
+    ctx.shape, ctx.causal, ctx.kinds = (H, dk, dv), causal, [kind for _, kind in masks]
     ctx.mark_non_differentiable(P)
     ctx.set_materialize_grads(False)
     return O, P
 
   @staticmethod
   def backward(ctx, dO, _dP):
-    Q, K, V, O, stats, qm, vm, km, am = ctx.saved_tensors
+    Q, K, V, O, stats, *masks = ctx.saved_tensors
     H, dk, dv = ctx.shape
     B, T, S = Q.shape[0], Q.shape[1], K.shape[1]
     dQ, dK, dV = torch.empty_like(Q), torch.empty_like(K), torch.empty_like(V)
@@ -2381,12 +2398,12 @@ class _AttentionCore(torch.autograd.Function):
         t.zero_()
     else:
       dO = f32c(dO, "grad")
-      m = _mha_masks((qm, vm, km, am), ctx.causal)
+      m = _mha_masks(zip(masks, ctx.kinds), ctx.causal)
       ws = workspace(lib().tfrs_mha_bwd_workspace_bytes(B, T, H), Q.device, "mha_bwd")
       check(lib().tfrs_mha_bwd_f32(ptr(Q), ptr(K), ptr(V), ctypes.byref(m), ptr(O), ptr(stats), ptr(dO), B, T, S, H, dk,
                                    dv, ptr(dQ), ptr(dK), ptr(dV), ptr(ws), ws.numel(), stream()), "mha_bwd")
     n = ctx.needs_input_grad
-    return (dQ if n[0] else None, dK if n[1] else None, dV if n[2] else None) + (None,) * 9
+    return (dQ if n[0] else None, dK if n[1] else None, dV if n[2] else None) + (None,) * 6
 
 
 def attention_core(Q: torch.Tensor, K: torch.Tensor, V: torch.Tensor, num_heads: int, query_mask=None, value_mask=None,
@@ -2411,11 +2428,13 @@ def attention_core(Q: torch.Tensor, K: torch.Tensor, V: torch.Tensor, num_heads:
     raise ValueError("attention: the query and key sequences must not be empty")
   if not 1 <= dk <= MHA_MAX_HEAD_DIM or not 1 <= dv <= MHA_MAX_HEAD_DIM:
     raise ValueError(f"attention: key_dim = {dk} and value_dim = {dv} must be in 1 .. {MHA_MAX_HEAD_DIM}")
-  masks = (_mha_mask(query_mask, (B, T), "query_mask"), _mha_mask(value_mask, (B, S), "value_mask"),
-           _mha_mask(key_mask, (B, S), "key_mask"), _mha_mask(attention_mask, (B, T, S), "attention_mask"))
+  masks = (_mask_arg(query_mask, (B, T), "attention", "query_mask"),
+           _mask_arg(value_mask, (B, S), "attention", "value_mask"),
+           _mask_arg(key_mask, (B, S), "attention", "key_mask"),
+           _mask_arg(attention_mask, (B, T, S), "attention", "attention_mask"))
   Q, K, V = f32c(Q, "query"), f32c(K, "key"), f32c(V, "value")
   if torch.is_grad_enabled() and any(t.requires_grad for t in (Q, K, V)):
-    O, P = _AttentionCore.apply(Q, K, V, H, dk, dv, *masks, bool(causal), bool(return_scores))
+    O, P = _AttentionCore.apply(Q, K, V, H, dk, dv, masks, bool(causal), bool(return_scores))
     return O, (P if return_scores else None)
   O, _, P = _attention_fwd(Q.detach(), K.detach(), V.detach(), H, dk, dv, masks, bool(causal), bool(return_scores),
                            False)
@@ -2473,10 +2492,11 @@ class _DenseAttentionDesc(ctypes.Structure):
 
 
 def _dense_desc(mode, scale, cw, qm, vm, causal, rate, seed, call) -> _DenseAttentionDesc:
+  """qm, vm: the query and value masks as _mask_arg's (mask, kind) pairs."""
   s = _DenseAttentionDesc()
   s.mode, s.scale, s.concat_weight = mode, ptr(scale), ptr(cw)
-  s.query_mask, s.query_mask_kind = ptr(qm), _MASK_KINDS[qm.dtype] if qm is not None else 0
-  s.value_mask, s.value_mask_kind = ptr(vm), _MASK_KINDS[vm.dtype] if vm is not None else 0
+  s.query_mask, s.query_mask_kind = ptr(qm[0]), qm[1]
+  s.value_mask, s.value_mask_kind = ptr(vm[0]), vm[1]
   s.causal, s.rate, s.seed, s.call = int(causal), float(rate), seed, call
   return s
 
@@ -2501,8 +2521,8 @@ class _DenseAttention(torch.autograd.Function):
     args = (mode, scale, cw, qm, vm, causal, rate, seed, call)
     O, stats, P = _dense_attention_fwd(q, k, v, args, want_p, True)
     P = P if want_p else torch.empty((0,), dtype=torch.float32, device=q.device)
-    ctx.save_for_backward(q, k, v, scale, cw, qm, vm, O, stats)
-    ctx.args = (mode, causal, rate, seed, call)
+    ctx.save_for_backward(q, k, v, scale, cw, qm[0], vm[0], O, stats)
+    ctx.args = (mode, qm[1], vm[1], causal, rate, seed, call)
     ctx.mark_non_differentiable(P)
     ctx.set_materialize_grads(False)
     return O, P
@@ -2510,7 +2530,7 @@ class _DenseAttention(torch.autograd.Function):
   @staticmethod
   def backward(ctx, dO, _dP):
     q, k, v, scale, cw, qm, vm, O, stats = ctx.saved_tensors
-    mode, causal, rate, seed, call = ctx.args
+    mode, qk, vk, causal, rate, seed, call = ctx.args
     n = ctx.needs_input_grad
     B, Tq, dim = q.shape
     Tv, dv = v.shape[1], v.shape[2]
@@ -2523,7 +2543,7 @@ class _DenseAttention(torch.autograd.Function):
           t.zero_()
     else:
       dO = f32c(dO, "grad")
-      d = _dense_desc(mode, scale, cw, qm, vm, causal, rate, seed, call)
+      d = _dense_desc(mode, scale, cw, (qm, qk), (vm, vk), causal, rate, seed, call)
       ws = workspace(lib().tfrs_dense_attention_bwd_workspace_bytes(mode, B, Tq, dim), q.device, "dense_attention_bwd")
       check(lib().tfrs_dense_attention_bwd_f32(ptr(q), ptr(k), ptr(v), ctypes.byref(d), ptr(O), ptr(stats), ptr(dO), B,
                                                Tq, Tv, dim, dv, ptr(dq), ptr(dk), ptr(dv_), ptr(dscale), ptr(dcw),
@@ -2575,8 +2595,8 @@ def dense_attention(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
     concat_weight = f32c(concat_weight, "concat_weight")
   else:
     concat_weight = None
-  qm = _mha_mask(query_mask, (B, Tq), "query_mask")
-  vm = _mha_mask(value_mask, (B, Tv), "value_mask")
+  qm = _mask_arg(query_mask, (B, Tq), "dense_attention", "query_mask")
+  vm = _mask_arg(value_mask, (B, Tv), "dense_attention", "value_mask")
   q, k, v = f32c(query, "query"), f32c(key, "key"), f32c(value, "value")
   seed, call = int(seed) & (2**64 - 1), int(call) & (2**64 - 1)
   diff = (q, k, v, scale, concat_weight)
@@ -2789,14 +2809,8 @@ def batch_norm(x: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[to
     require_cuda(p, name)
     if p.dtype != torch.float32 or not p.is_contiguous():
       raise TypeError(f"batch_norm: {name} must be a contiguous float32 tensor (it is updated in place)")
-  m, mk = None, 0
-  if mask is not None:
-    require_cuda(mask, "mask")
-    if mask.dtype not in _MASK_KINDS:
-      raise TypeError(f"batch_norm: the mask must be bool, int32 or int64, got {mask.dtype}")
-    if tuple(mask.shape) != tuple(x.shape[:-1]):
-      raise ValueError(f"batch_norm: the mask has shape {tuple(mask.shape)}, the input {tuple(x.shape)}")
-    m, mk = mask.contiguous().reshape(N), _MASK_KINDS[mask.dtype]
+  m, mk = _mask_arg(mask, x.shape[:-1], "batch_norm")
+  m = None if m is None else m.reshape(N)
   x2 = f32c(x, "inputs").reshape(N, d)
   g = None if gamma is None else f32c(gamma, "gamma")
   b = None if beta is None else f32c(beta, "beta")
