@@ -3,7 +3,8 @@
 //   tfrs_topk_exclude_rerank_f32 : `_exclude` (layers/factorized_top_k.py:83-115) on an over-fetched [Q, kf] list
 //   tfrs_count_above_f32         : #{retrieved scores > positive score}   (metrics/factorized_top_k.py:181-192, in_top_k)
 //   tfrs_topk_hits_accumulate    : the weighted running sums behind FactorizedTopK's Mean metrics, kept on the device
-// One warp per query, no atomics, deterministic.
+// One warp per query, no atomics, deterministic.  An array with no elements may be NULL (torch hands out a NULL
+// data_ptr for empty tensors): exclusions when n_excl == 0, scores when k == 0, every per-query array when Q == 0.
 #include "common.cuh"
 
 namespace tfrs {
@@ -87,7 +88,7 @@ using namespace tfrs;
 extern "C" int tfrs_topk_exclude_rerank_f32(const float* scores, const int64_t* idx, int64_t Q, int k_fetched,
                                             const int64_t* identifiers, const int64_t* exclusions, int n_excl, int k_out,
                                             float* out_scores, int64_t* out_idx, void* stream) {
-  TFRS_CHECK_ARG(scores && idx && exclusions && out_scores && out_idx, "exclude_rerank: NULL pointer");
+  TFRS_CHECK_ARG(scores && idx && (exclusions || n_excl == 0) && out_scores && out_idx, "exclude_rerank: NULL pointer");
   TFRS_CHECK_ARG(Q >= 0 && k_fetched > 0 && k_fetched <= 4096 && n_excl >= 0 && k_out > 0 && k_out <= k_fetched,
                  "exclude_rerank: bad shape (k_fetched=%d k_out=%d)", k_fetched, k_out);
   if (Q == 0) return TFRS_OK;
@@ -103,7 +104,8 @@ extern "C" int tfrs_topk_exclude_rerank_f32(const float* scores, const int64_t* 
 
 extern "C" int tfrs_count_above_f32(const float* scores, int64_t ld, int k, const float* positive_scores, int64_t Q,
                                     int32_t* out_count, void* stream) {
-  TFRS_CHECK_ARG(scores && positive_scores && out_count && ld >= k && k >= 0, "count_above: bad argument");
+  TFRS_CHECK_ARG((Q <= 0 || ((scores || k == 0) && positive_scores && out_count)) && ld >= k && k >= 0,
+                 "count_above: bad argument");
   if (Q <= 0) return TFRS_OK;
   count_above_kernel<<<(unsigned)ceil_div(Q * 32, 256), 256, 0, (cudaStream_t)stream>>>(scores, ld, k, positive_scores, Q, out_count);
   TFRS_LAUNCH_CHECK();
@@ -112,7 +114,8 @@ extern "C" int tfrs_count_above_f32(const float* scores, int64_t ld, int k, cons
 
 extern "C" int tfrs_topk_hits_accumulate(const int32_t* count, const float* positive_scores, const float* sample_weight, int64_t Q,
                                          const int32_t* ks, int n_ks, double* acc, void* stream) {
-  TFRS_CHECK_ARG(count && positive_scores && ks && acc && n_ks > 0 && n_ks <= HA_MAX_KS, "hits_accumulate: bad argument (n_ks <= 16)");
+  TFRS_CHECK_ARG(((count && positive_scores) || Q <= 0) && ks && acc && n_ks > 0 && n_ks <= HA_MAX_KS,
+                 "hits_accumulate: bad argument (n_ks <= 16)");
   if (Q <= 0) return TFRS_OK;
   HitParams hp{};
   hp.n_ks = n_ks;
