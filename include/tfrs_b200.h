@@ -169,6 +169,25 @@ int tfrs_topk_merge_sorted_strided(const float* scores, const int64_t* idx, int6
                                    float* out_scores, int64_t* out_idx, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K26  multi-interest (maxsim) retrieval: a query is H >= 1 vectors q_h and scores candidate c by
+ * m(q, c) = max_h s_h(c), s_h = the canonical fmaf chain of q_h . c (tasks/retrieval.py:172-176).  Heads that tie on the
+ * maximum (+0 and -0 tie) report the lowest head's bits.  Order = (m desc, index asc).
+ *
+ * tfrs_topk_maxsim_merge_f32  scores / idx = [Q, H, w]: per query the H per-head top-w lists, each sorted by (score desc,
+ *                             index asc) with distinct indices -- what the scans emit for the Q*H head rows with k = w.
+ *                             Keeps each candidate's best entry (highest score, then lowest head) and writes the first
+ *                             k_out (1 <= k_out <= w) kept entries in order to out_* [Q, k_out].  With w = min(k, N) the
+ *                             result is the exact maxsim top-min(k, N) (DESIGN.md, K26).  H * w <=
+ *                             TFRS_MAXSIM_MAX_ENTRIES, TFRS_ERR_UNSUPPORTED above.  No workspace; deterministic.
+ * tfrs_rowwise_maxsim_f32     out[r] = max_h dot(q[r, h, :], c[r, :]) for q [rows, H, d], c [rows, d]: FactorizedTopK's
+ *                             positive score for multi-head queries, each head by tfrs_rowwise_dot_f32's chain.
+ * ------------------------------------------------------------------------------------------- */
+#define TFRS_MAXSIM_MAX_ENTRIES 8192
+int tfrs_topk_maxsim_merge_f32(const float* scores, const int64_t* idx, int64_t Q, int H, int w, int k_out,
+                               float* out_scores, int64_t* out_idx, void* stream);
+int tfrs_rowwise_maxsim_f32(const float* q, const float* c, int64_t rows, int H, int d, float* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K14  exact top-K with overridden rows, and its hit count: the device side of examples.movielens.evaluate
  * (examples/movielens.py:71-88, `scores[train_movies] = -1e6; top_movies = argsort(-scores)[:k]`).  Query u lists the
  * rows rows[offsets[u] .. offsets[u+1]) (CSR, int64, sorted and unique per query, in [0, N)); those rows score exactly

@@ -75,6 +75,20 @@ __host__ __device__ __forceinline__ bool better(float sa, long long ia, float sb
   return (sa > sb) || (sa == sb && ia < ib);
 }
 
+// larger float <=> larger unsigned; -0 canonicalised by the caller (+ 0.0f)
+__device__ __forceinline__ unsigned int okey(float f) {
+  unsigned int u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// The canonical fp32 dot of two rows: one sequential fmaf chain over k = 0..d-1 from +0 (tfrs_rowwise_dot_f32,
+// tfrs_rowwise_maxsim_f32; the scans' exact re-scoring computes the same chain).
+__device__ __forceinline__ float dot_chain(const float* __restrict__ a, const float* __restrict__ b, int d) {
+  float acc = 0.f;
+  for (int k = 0; k < d; ++k) acc = fmaf(a[k], b[k], acc);
+  return acc;
+}
+
 // |v| for the rescale statistic max |element|, 0 for Inf and NaN: one non-finite element makes only its own row or column
 // of a split-fp16 product non-finite, instead of leaving the whole operand unscaled.  Every producer of that statistic
 // (tc_split.cuh cx_amax_kernel, the CROSS epilogue's out_amax, cross.cu cross_bwd_elem) uses it, so they agree bit for bit.

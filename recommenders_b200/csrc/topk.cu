@@ -265,10 +265,7 @@ __global__ void __launch_bounds__(256)
 rowwise_dot_kernel(const float* __restrict__ a, const float* __restrict__ b, long long rows, int d, float* __restrict__ out) {
   long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   if (i >= rows) return;
-  const float* pa = a + i * d; const float* pb = b + i * d;
-  float acc = 0.f;
-  for (int k = 0; k < d; ++k) acc = fmaf(pa[k], pb[k], acc);
-  out[i] = acc;
+  out[i] = dot_chain(a + i * d, b + i * d, d);
 }
 }  // namespace tfrs
 

@@ -9,11 +9,6 @@
 
 namespace tfrs {
 
-__device__ __forceinline__ unsigned int okey(float f) {  // larger float <=> larger unsigned; -0 canonicalised by the caller
-  unsigned int u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 constexpr int XR_THREADS = 128;
 
 __global__ void __launch_bounds__(XR_THREADS)

@@ -72,6 +72,16 @@ def _exclude(scores: Tensor, identifiers, exclude, k: int):
   return _take_along_axis(scores, indices), _take_along_axis(identifiers, indices)
 
 
+def _is_multi_head(queries) -> bool:
+  """True for multi-head [Q, H, d] queries (scored by their best head, DESIGN.md K26); ValueError for a tensor of rank
+  other than 1, 2 or 3."""
+  if not isinstance(queries, torch.Tensor):
+    return False
+  if queries.dim() not in (1, 2, 3):
+    raise ValueError(f"Queries must be of rank 1, 2 or 3, got {queries.dim()}.")
+  return queries.dim() == 3
+
+
 def _check_candidates_with_identifiers(element) -> None:
   """factorized_top_k.py:118-137 -- dataset elements are embeddings or (identifiers, embeddings)."""
   if isinstance(element, tuple):
@@ -275,7 +285,8 @@ class Streaming(TopK):
   merged into the carried [Q,k] state -- ties resolve to the lower running index, i.e. state first (:462-463), so the
   result equals BruteForce's.  Batches that live in host memory are staged through pinned double buffers so the copy of
   chunk i+1 overlaps the scan of chunk i (corpora larger than HBM).  Small chunks use the exact CUDA-core scan, which
-  takes the carried state directly."""
+  takes the carried state directly.  Multi-head [Q, H, d] queries carry one state per head row and are merged by their
+  best head once, after the last chunk (DESIGN.md K26)."""
 
   def __init__(self, query_model: Optional[torch.nn.Module] = None, k: int = 10,
                handle_incomplete_batches: bool = True, num_parallel_calls: Optional[int] = None,
@@ -307,10 +318,14 @@ class Streaming(TopK):
       raise ValueError("The `index` method must be called first to create the retrieval index.")
     if self.query_model is not None:
       queries = self.query_model(queries)
+    multi_head = _is_multi_head(queries)
     queries = ops.f32c(queries, "queries")
     Q = queries.shape[0]
-    state = (torch.zeros((Q, 0), dtype=torch.float32, device=queries.device),
-             torch.zeros((Q, 0), dtype=torch.int64, device=queries.device))
+    if multi_head:   # every head row carries its own state; K26 merges the heads once, after the last chunk
+      H, qd = int(queries.shape[1]), int(queries.shape[2])
+      queries = ops.maxsim_queries(queries, qd).reshape(Q * H, qd)
+    state = (torch.zeros((queries.shape[0], 0), dtype=torch.float32, device=queries.device),
+             torch.zeros((queries.shape[0], 0), dtype=torch.int64, device=queries.device))
     counter = 0
     id_chunks = []
     pending, pending_rows = [], 0
@@ -328,6 +343,8 @@ class Streaming(TopK):
         emb = st.stage([p if p.is_cuda else p.to(torch.float32) for p in pending])
       else:
         emb = pending[0] if len(pending) == 1 else torch.cat(pending, 0)
+      if multi_head and emb.shape[1] != qd:
+        raise ValueError(f"The queries have d={qd} but the candidates have d={emb.shape[1]}.")
       # state + top-k of the chunk, its rows numbered with the running counter (enumerate_rows, :474-485); the chunk's
       # tensor-core image is built in a per-stream scratch slot
       state = ops.topk(queries, ops.f32c(emb, "candidates"), k, image="stream_index" if self.use_tensor_cores else None,
@@ -353,6 +370,12 @@ class Streaming(TopK):
         flush()
     flush()
     self._counter.fill_(counter)
+    if multi_head:
+      w = state[0].shape[1]
+      if w:
+        state = ops.maxsim_merge(state[0].reshape(Q, H, w), state[1].reshape(Q, H, w), w)
+      else:
+        state = (state[0].reshape(Q, 0), state[1].reshape(Q, 0))
     return state[0], state[1], (id_chunks if id_chunks else None)
 
   def call(self, queries, k: Optional[int] = None):
@@ -385,7 +408,9 @@ class BruteForce(TopK):
   `index` keeps the fp32 corpus and, for large corpora, builds the fp16 tensor-core screening image;
   `call` returns exactly the top-k of the fp32 scores either way.  `index_shard` adds the row-sharded
   multi-GPU mode: every rank scans its contiguous shard, ONE all-gather of the per-shard (score, index)
-  lists (issued by libtfrs_b200.so through its own NCCL communicator) is merged on every rank."""
+  lists (issued by libtfrs_b200.so through its own NCCL communicator) is merged on every rank.  Multi-head [Q, H, d]
+  queries score a candidate by their best head (`ops.topk_maxsim`, DESIGN.md K26); the sharded mode takes 2-D queries
+  only."""
 
   def __init__(self, query_model: Optional[torch.nn.Module] = None, k: int = 10, name: Optional[Text] = None):
     super().__init__(k=k, name=name)
@@ -456,8 +481,10 @@ class BruteForce(TopK):
 
   def in_top_k_count(self, queries: Tensor, positive_scores: Tensor, k: int) -> Optional[Tensor]:
     """Counted inside the tensor-core scan (`tfrs_topk_tc_count_f32`) when the index is unsharded and has no query
-    model, so `queries` are already the embeddings the corpus is scored against."""
-    if self._candidates is None or self._shard is not None or self.query_model is not None:
+    model, so `queries` are already the embeddings the corpus is scored against.  Multi-head [Q, H, d] queries are
+    counted on their retrieved list instead."""
+    if (self._candidates is None or self._shard is not None or self.query_model is not None or
+        _is_multi_head(queries)):
       return None
     k = min(k, self._candidates.shape[0])
     if not self._tc_ok(queries.shape[0], k):
@@ -470,11 +497,18 @@ class BruteForce(TopK):
       raise ValueError("The `index` method must be called first to create the retrieval index.")
     if self.query_model is not None:
       queries = self.query_model(queries)
+    multi_head = _is_multi_head(queries)
+    if multi_head and self._shard is not None:
+      raise NotImplementedError("BruteForce.index_shard does not take multi-head [Q, H, d] queries; index the whole "
+                                "corpus with `index` instead.")
     if self._shard is None:
       n_total = self._candidates.shape[0]
       if k > n_total:
         raise ValueError(f"input must have at least k columns. Had {n_total}, needed {k}")
-      values, indices = self._local_topk(queries, k, 0)
+      if multi_head:   # maxsim over the heads (DESIGN.md, K26)
+        values, indices = ops.topk_maxsim(queries, self._candidates, k, image=self._tc_index)
+      else:
+        values, indices = self._local_topk(queries, k, 0)
     else:
       values, indices = self._sharded_topk(queries, k)
     if self._identifiers is None:
@@ -491,7 +525,7 @@ class BruteForce(TopK):
     if (self._candidates is not None and self._shard is None and int_ids and E > 0 and
         k + E <= self._candidates.shape[0]):
       q = self.query_model(queries) if self.query_model is not None else queries
-      if self._tc_ok(q.shape[0], k + E):
+      if not _is_multi_head(q) and self._tc_ok(q.shape[0], k + E):
         s, i = ops.topk_tc_exclude(q, self._candidates, self._tc_index, k, exclusions, identifiers=ids)
         if ids is None:
           return s, i.to(torch.int32)

@@ -117,7 +117,8 @@ class FactorizedTopK(Factorized):
   strictly above the positive}, clipped at max(ks).  When the layer can count inside its scan (`TopK.in_top_k_count`,
   e.g. a tensor-core `BruteForce` index: no top-K list, no sort) it does; otherwise it is counted on the retrieved list.
   Either way ONE kernel folds  w_q * [c_q < k]  for every k into a device accumulator -- update_state never
-  synchronises with the host."""
+  synchronises with the host.  Multi-head [Q, H, d] query embeddings are scored by their best head (positive and
+  candidates alike) and counted on the retrieved list."""
 
   def __init__(self, candidates: Union[ftk.TopK, Dataset, list], ks: Sequence[int] = (1, 5, 10, 50, 100),
                name: str = "factorized_top_k") -> None:
@@ -170,8 +171,12 @@ class FactorizedTopK(Factorized):
     w = None if sample_weight is None else _flat_device(sample_weight, query_embeddings.device)
 
     if true_candidate_ids is None:
-      # positive score with the same canonical chain as the retrieved scores (:133-134)
-      positive_scores = ops.rowwise_dot(query_embeddings, true_candidate_embeddings)
+      # positive score with the same canonical chain as the retrieved scores (:133-134); multi-head [Q, H, d] queries
+      # score it by their best head, as the layer scores the candidates
+      if query_embeddings.dim() == 3:
+        positive_scores = ops.rowwise_maxsim(query_embeddings, true_candidate_embeddings)
+      else:
+        positive_scores = ops.rowwise_dot(query_embeddings, true_candidate_embeddings)
       layer = self._candidates
       count = layer.in_top_k_count(query_embeddings, positive_scores, kmax)
       if count is None:

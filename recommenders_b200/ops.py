@@ -650,6 +650,96 @@ def topk_merge(scores: torch.Tensor, idx: torch.Tensor, k: int, sorted_lists: bo
 
 
 # ------------------------------------------------------------------------------------------------
+# K26 multi-interest (maxsim) top-k: a [Q, H, d] query scores a candidate by its best head (DESIGN.md, K26)
+# ------------------------------------------------------------------------------------------------
+MAXSIM_MAX_ENTRIES = 8192   # TFRS_MAXSIM_MAX_ENTRIES of include/tfrs_b200.h: H * min(k, N) per query
+
+
+def _maxsim_limit(H: int, w: int) -> None:
+  if H * w > MAXSIM_MAX_ENTRIES:
+    raise NotImplementedError(f"maxsim top-k: H={H} heads of {w} entries each is {H * w} entries per query, above "
+                              f"{MAXSIM_MAX_ENTRIES}; use fewer heads or a smaller k")
+
+
+def _maxsim_merge(scores: torch.Tensor, idx: torch.Tensor, k_out: int, out_s: torch.Tensor, out_i: torch.Tensor) -> None:
+  Q, H, w = scores.shape
+  if Q:
+    check(lib().tfrs_topk_maxsim_merge_f32(ptr(scores), ptr(idx), Q, H, w, k_out, ptr(out_s), ptr(out_i), stream()),
+          "maxsim_merge")
+
+
+def maxsim_merge(scores: torch.Tensor, idx: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+  """[Q, H, w] per-head lists, each sorted by (score desc, index asc) with distinct indices (what the scans emit for the
+  head rows) -> the first min(k, w) entries per query after keeping each candidate's best entry (highest score, then
+  lowest head): ([Q, k_out] f32, [Q, k_out] i64)."""
+  scores = f32c(scores, "scores"); idx = _i64(require_cuda(idx, "idx"), "idx", scores.device)
+  if scores.dim() != 3 or tuple(idx.shape) != tuple(scores.shape):
+    raise ValueError(f"maxsim_merge: scores and idx must both be [Q, H, w], got {tuple(scores.shape)} and {tuple(idx.shape)}")
+  if k < 1:
+    raise ValueError(f"maxsim_merge: k must be positive, got {k}")
+  Q, H, w = scores.shape
+  k_out = min(k, w)
+  out_s = torch.empty((Q, k_out), dtype=torch.float32, device=scores.device)
+  out_i = torch.empty((Q, k_out), dtype=torch.int64, device=scores.device)
+  if k_out == 0:
+    return out_s, out_i
+  _maxsim_limit(H, w)
+  _maxsim_merge(scores, idx, k_out, out_s, out_i)
+  return out_s, out_i
+
+
+def maxsim_queries(q3: torch.Tensor, d: int) -> torch.Tensor:
+  """[Q, H, d] float32 contiguous queries with H >= 1 and the corpus's d, else ValueError."""
+  q3 = f32c(q3, "queries")
+  if q3.dim() != 3 or q3.shape[1] < 1 or q3.shape[2] != d:
+    raise ValueError(f"maxsim queries must be [Q, H >= 1, {d}], got {tuple(q3.shape)}")
+  return q3
+
+
+def topk_maxsim(q3: torch.Tensor, corpus: torch.Tensor, k: int, image=None) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Exact maxsim top-min(k, N) of [Q, H, d] queries: (m desc, index asc), m = max over heads of the canonical dot.  Each
+  head row gets its own top-w (w = min(k, N)) from `topk` (tensor-core scan with `image` when it applies, exact scan
+  otherwise), then K26 merges the H lists of every query.  At most max(1, TC_MAX_Q_PER_CALL // H) queries go into one
+  scan call, so the per-head lists stay ~25 MB whatever Q is.  `image` is the corpus's index_build image, the name of a
+  scratch slot to build it in, or None."""
+  corpus = f32c(corpus, "candidates")
+  if corpus.dim() != 2:
+    raise ValueError(f"topk_maxsim: the corpus must be [N, d], got {tuple(corpus.shape)}")
+  N, d = corpus.shape
+  q3 = maxsim_queries(q3, d)
+  Q, H, _ = q3.shape
+  w = min(k, N)
+  out_s = torch.empty((Q, max(w, 0)), dtype=torch.float32, device=q3.device)
+  out_i = torch.empty((Q, max(w, 0)), dtype=torch.int64, device=q3.device)
+  if Q == 0 or w <= 0:
+    return out_s, out_i
+  _maxsim_limit(H, w)
+  step = max(1, TC_MAX_Q_PER_CALL // H)
+  if isinstance(image, str):   # one image for every chunk
+    corpus = tc_corpus(corpus)
+    image = index_build(corpus, reuse_slot=image) if uses_tc_scan(min(Q, step) * H, N, d, w) else None
+  for lo in range(0, Q, step):
+    hi = min(Q, lo + step)
+    s, i = topk(q3[lo:hi].reshape((hi - lo) * H, d), corpus, w, image=image)
+    _maxsim_merge(s.reshape(hi - lo, H, w), i.reshape(hi - lo, H, w), w, out_s[lo:hi], out_i[lo:hi])
+  return out_s, out_i
+
+
+def rowwise_maxsim(q3: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+  """out[r] = max_h dot(q3[r, h], c[r]) with rowwise_dot's chain per head; ties keep the lowest head's bits."""
+  c = f32c(c, "c")
+  if c.dim() != 2:
+    raise ValueError(f"rowwise_maxsim: c must be [R, d], got {tuple(c.shape)}")
+  q3 = maxsim_queries(q3, c.shape[1])
+  if q3.shape[0] != c.shape[0]:
+    raise ValueError(f"rowwise_maxsim: {q3.shape[0]} query rows but {c.shape[0]} candidate rows")
+  R, H, d = q3.shape
+  out = torch.empty((R,), dtype=torch.float32, device=q3.device)
+  check(lib().tfrs_rowwise_maxsim_f32(ptr(q3), ptr(c), R, H, d, ptr(out), stream()), "rowwise_maxsim")
+  return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K14 top-k with overridden rows (examples.movielens.evaluate; DESIGN.md §2 pins the rules)
 # ------------------------------------------------------------------------------------------------
 OVERRIDE_SCORE = np.float32(-1e6)
