@@ -8,6 +8,7 @@ treats the mask adder as an addition (derivative 1), as autograd does."""
 import numpy as np
 
 MASK_ADDER = -1e9
+TINY = 2.0 ** -125          # one float32 denormal step, 2^-149, in units of u = 2^-24
 
 
 def _f64(a):
@@ -59,6 +60,41 @@ def core_backward(Q, K, V, P, Qs, dO):
   dQ = np.einsum("bhts,bshd->bthd", dS, K) * scale_of(Q.shape[-1])
   dK = np.einsum("bhts,bthd->bshd", dS, Qs)
   return dQ, dK, dV
+
+
+def core_error_bounds(Q, K, V, P, Qs, dO):
+  """First-order bounds on the float32 kernels' absolute error, per element and in units of u = 2^-24, for O, P, dQ,
+  dK and dV of the core (shapes as core_forward / core_backward return them).  They count the roundings of the
+  kernels' operation order (csrc/attention.cuh):
+    score   the team's fmaf chain of ceil(dk / 8) terms per lane, 3 butterfly adds and the fp32 q * 1/sqrt(dk): n_k
+            roundings of magnitude A = sum_d |qs_d k_d|;
+    P       e^{s - m} / l moves by the score's error, by l's (a sum of S terms, at most the largest score error plus S
+            roundings), and by expf and __fdividef (2 ulp each);
+    O       S fmafs into o, S rescales by e^{m_old - m}, the division by l;
+    dV      T fmafs of p dO;  dP = dO . v and delta = dO . O are chains of n_v roundings;
+    dK, dQ  T (S) fmafs of ds q (ds k) over the staged q * 1/sqrt(dk) (k), ds = p (dP - delta) with both errors;
+    and every operation whose result falls below 2^-126 (a p of e^-100, its products) errs by up to one denormal
+    step, 2^-149 absolute: TINY in units of u, once per operation of the chain."""
+  dk, dv = Q.shape[-1], V.shape[-1]
+  S, T = K.shape[1], Q.shape[1]
+  n_k, n_v = -(-dk // 8) + 4, -(-dv // 8) + 3
+  aQs, aK, aV, adO = np.abs(Qs), np.abs(K), np.abs(V), np.abs(dO)
+  eS = n_k * np.einsum("bthd,bshd->bhts", aQs, aK)
+  eP = P * (eS + eS.max(-1, keepdims=True) + S + 6) + 4 * TINY
+  PaV = np.einsum("bhts,bshd->bthd", P, aV)
+  eO = np.einsum("bhts,bshd->bthd", eP, aV) + (2 * S + 2) * PaV + (2 * S + 2) * TINY
+  eV = np.einsum("bhts,bthd->bshd", eP, adO) + (T + 1) * np.einsum("bhts,bthd->bshd", P, adO) + (T + 1) * TINY
+  O = np.einsum("bhts,bshd->bthd", P, V)
+  dP = np.einsum("bthd,bshd->bhts", dO, V)
+  delta = np.einsum("bthd,bthd->bht", dO, O)[..., None]
+  e_delta = (n_v * np.einsum("bthd,bthd->bht", adO, np.abs(O)) + np.einsum("bthd,bthd->bht", adO, eO))[..., None]
+  e_dP = n_v * np.einsum("bthd,bshd->bhts", adO, aV)
+  dS = P * (dP - delta)
+  eDS = eP * np.abs(dP - delta) + P * (e_dP + e_delta) + 2 * np.abs(dS) + 2 * TINY
+  aDS = np.abs(dS)
+  eK = np.einsum("bhts,bthd->bshd", eDS, aQs) + (T + 2) * (np.einsum("bhts,bthd->bshd", aDS, aQs) + TINY)
+  eQ = scale_of(dk) * (np.einsum("bhts,bshd->bthd", eDS, aK) + (S + 2) * (np.einsum("bhts,bshd->bthd", aDS, aK) + TINY))
+  return dict(O=eO, P=eP, dQ=eQ, dK=eK, dV=eV)
 
 
 def _proj(x, W, b):

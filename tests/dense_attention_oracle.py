@@ -14,6 +14,7 @@ from __future__ import annotations
 import numpy as np
 
 MODES = ("dot", "concat", "additive")
+TINY = 2.0 ** -125          # one float32 denormal step, 2^-149, in units of u = 2^-24
 
 
 def _f64(a):
@@ -95,6 +96,87 @@ def backward(cache, dout):
     if scale is not None:
       dscale = (ds[..., None] * t).sum((0, 1, 2))
   return G.sum(2), G.sum(1), dv, dscale, dwc
+
+
+def _ds(cache, dout):
+  g = _f64(dout) * cache["qm"][..., None]
+  dw = (g @ cache["v"].transpose(0, 2, 1)) * cache["z"]
+  w = cache["w"]
+  return g, dw, w * (dw - (w * dw).sum(-1, keepdims=True))
+
+
+def error_bounds(cache, dout):
+  """First-order bounds on the float32 kernels' absolute error, per element and in units of u = 2^-24, for out, the
+  returned weights, dq, dk and dv (shapes as forward / backward return them).  They count the roundings of the kernels'
+  operation order (csrc/attention.cuh, the dense modes):
+    score   dot: the team's fmaf chain (ceil(dim / 8) per lane, 3 butterfly adds) times the fp32 scale; concat /
+            additive: the tanh argument (two roundings: q + k, times c), tanhf (2 ulp), the chain of w_d t_d, times wc;
+    weights e^{s - m} / l moves by the score's error and by l's (a sum of Tv terms), expf and __fdividef (2 ulp each),
+            and the fp32 dropout factor;
+    out     Tv fmafs, Tv rescales and the division by l;
+    dv      Tq fmafs of w' dO;  dO . (z v - O) and its delta a chain of ceil(dv / 8) + 3 roundings with O's error;
+    dq, dk  Tv (Tq) fmafs of ds times k / q (dot), or of ds wc c w_d (1 - t_d^2) with 1 - t^2 one fmaf on a t carrying
+            its own error (concat / additive);
+    and every operation whose result falls below 2^-126 errs by up to one denormal step: TINY per operation."""
+  q, k, v, w, z, wd, t = (cache[n] for n in ("q", "k", "v", "w", "z", "wd", "t"))
+  mode, scale, wc = cache["mode"], cache["scale"], cache["wc"]
+  D, dv = q.shape[-1], v.shape[-1]
+  Tq, Tv = q.shape[1], k.shape[1]
+  n_k, n_v = -(-D // 8) + 3, -(-dv // 8) + 3
+  aq, ak, av = np.abs(q), np.abs(k), np.abs(v)
+  if mode == "dot":
+    c = 1.0 if scale is None else float(scale)
+    eS = (n_k + 1) * abs(c) * (aq @ ak.transpose(0, 2, 1))
+  else:
+    c = 1.0 if scale is None or mode == "additive" else float(scale)
+    a = np.ones(D) if mode == "concat" or scale is None else np.abs(scale)
+    cw = 1.0 if wc is None else abs(wc)
+    arg = np.abs(c * (q[:, :, None, :] + k[:, None, :, :]))
+    dt = 1.0 - t * t
+    e_t = 2 * dt * arg + 2 * np.abs(t)                       # the argument's two roundings, tanhf's 2 ulp
+    eS = cw * (a * (e_t + n_k * np.abs(t))).sum(-1) + cw * np.abs((a * t).sum(-1))
+  eW = w * (eS + eS.max(-1, keepdims=True) + Tv + 6) + 4 * TINY
+  eWd = z * (eW + w)
+  g = _f64(dout) * cache["qm"][..., None]
+  ag = np.abs(g)
+  O = wd @ v
+  eO = eWd @ av + (2 * Tv + 2) * (wd @ av + TINY)
+  edv = eWd.transpose(0, 2, 1) @ ag + (Tq + 1) * (wd.transpose(0, 2, 1) @ ag + TINY)
+  _, dw, ds = _ds(cache, dout)
+  delta = (g * O).sum(-1, keepdims=True)
+  e_dmd = ((n_v + 2) * ((ag @ av.transpose(0, 2, 1)) * z + (ag * np.abs(O)).sum(-1, keepdims=True))
+           + (ag * eO).sum(-1, keepdims=True))
+  eDS = eW * np.abs(dw - delta) + w * e_dmd + 2 * np.abs(ds) + 2 * TINY
+  ads = np.abs(ds)
+  if mode == "dot":
+    edq = abs(c) * (eDS @ ak + (Tv + 2) * (ads @ ak + TINY))
+    edk = abs(c) * (eDS.transpose(0, 2, 1) @ aq + (Tq + 2) * (ads.transpose(0, 2, 1) @ aq + TINY))
+  else:
+    f = cw * abs(c) * a
+    e_dt = 2 * np.abs(t) * e_t + dt
+    eG = f * (eDS[..., None] * dt + ads[..., None] * (e_dt + 4 * dt))
+    aG = f * ads[..., None] * dt
+    edq = eG.sum(2) + (Tv + 1) * (aG.sum(2) + TINY)
+    edk = eG.sum(1) + (Tq + 1) * (aG.sum(1) + TINY)
+  qm = cache["qm"][..., None]
+  return dict(out=eO * qm, weights=eWd, dq=edq, dk=edk, dv=edv)
+
+
+def weight_grad_magnitudes(cache, dout):
+  """The weight gradients with ds_j = w_j (dw_j - delta) replaced by w_j (|dw_j| + |delta|) and every other factor by
+  its magnitude: (dscale, dconcat_weight), dscale scalar or [dim] as backward returns it, None where backward's is.  A
+  float32 ds errs relative to |dw_j| + |delta|, not to the difference, which cancels to exactly 0 at Tv = 1."""
+  q, k, t, w = (cache[n] for n in ("q", "k", "t", "w"))
+  mode, scale, wc = cache["mode"], cache["scale"], cache["wc"]
+  _, dw, _ = _ds(cache, dout)
+  m = w * (np.abs(dw) + np.abs((w * dw).sum(-1, keepdims=True)))
+  if mode == "dot":
+    return (None if scale is None else float((m * np.abs(q @ k.transpose(0, 2, 1))).sum())), None
+  if mode == "additive":
+    return (None if scale is None else (m[..., None] * np.abs(t)).sum((0, 1, 2))), None
+  u = np.abs(q[:, :, None, :] + k[:, None, :, :])
+  dsc = None if scale is None else float((m * abs(wc) * (u * (1.0 - t * t)).sum(-1)).sum())
+  return dsc, float((m * np.abs(t).sum(-1)).sum())
 
 
 def weight_grad_rows(cache, dout):
