@@ -94,7 +94,9 @@ class Retrieval(torch.nn.Module, Task):
                   (self._temperature is None or self._temperature > 0) and
                   ops.inbatch_softmax_bias_supported(B_, C_, d_))
     plain = not three_d and self._loss is None and self._num_hard_negatives is None and not options
-    # multi-head queries (maxsim, :172-176) with the default loss: the head maximum is folded inside the blocked loss kernels
+    # multi-head queries (maxsim, :172-176) with the default loss: the head maximum is folded inside the blocked loss kernels.
+    # Every other 3-D case takes the maximum over the head rows of the score matrix with `amax`, whose gradient -- like
+    # tf.reduce_max's and the kernels' -- is split evenly among the heads that tie for the maximum.
     fused_maxsim = (three_d and self._loss is None and self._num_hard_negatives is None and not options and
                     (self._temperature is None or self._temperature > 0))
     need_scores = wants_batch_scores or not (fused_hard or fused_opts or plain or fused_maxsim)
@@ -104,7 +106,7 @@ class Retrieval(torch.nn.Module, Task):
       if three_d:  # maxsim over query heads, :172-176
         nq, nh, e = query_embeddings.shape
         s = ops.scores(query_embeddings.reshape(nq * nh, e), candidate_embeddings)
-        scores = s.reshape(nq, nh, -1).max(dim=1).values
+        scores = s.reshape(nq, nh, -1).amax(dim=1)   # a tie splits the gradient evenly among the heads
       else:
         scores = ops.scores(query_embeddings, candidate_embeddings)  # :178-180
       num_queries, num_candidates = scores.shape

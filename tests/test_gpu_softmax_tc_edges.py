@@ -740,29 +740,46 @@ def test_exact_forward_and_backward_multi_block(ops, monkeypatch):
   check_all(r, "exact multi-block", loss, lse, dq, dc)
 
 
-def _maxsim_reference(q3, c, inv_t, w, chain, rel):
-  """float64 maxsim loss: s_ij = max_h q_ih . c_j; the gradient goes to the maximising head(s), split evenly among ties."""
+def _maxsim_reference(q3, c, inv_t, w, chain, rel, g=1.0, bias=None, ids=None, mask=None, hard=None, keep_g=False):
+  """float64 maxsim loss: s_ij = max_h q_ih . c_j; the gradient goes to the maximising head(s), split evenly among ties.
+  The options of tasks.Retrieval in the reference's order (retrieval.py:187-208): l = s / T + b (b the sampling
+  correction); accidental hits (equal candidate ids off the diagonal) and entries the mask drops are left out of the sum
+  (a masked positive has l_ii = MIN_FLOAT); `hard` keeps each row's positive and its `hard` largest other logits.
+  w = None is unit weights, g the incoming gradient of the loss; keep_g also returns the head gradients [B, H, C]."""
   q64, c64 = q3.double(), c.double()
   B, H, d = q64.shape
   C = c64.shape[0]
+  dev = q3.device
   sh = torch.einsum("bhd,cd->bhc", q64, c64)
   s = sh.max(1).values
   at = (sh == s[:, None, :]).double()
   at = at / at.sum(1, keepdim=True)
-  l = s * inv_t
-  lse = torch.logsumexp(l, 1)
+  b64 = torch.zeros(C, dtype=F64, device=dev) if bias is None else bias.detach().to(device=dev, dtype=F64).reshape(-1)
+  l = s * inv_t + b64[None, :]
+  diag = torch.eye(B, C, dtype=torch.bool, device=dev)
+  keep = torch.ones_like(diag) if mask is None else mask.to(dev).bool()
+  if ids is not None:
+    idv = ids.to(dev)
+    keep = keep & ~((idv[None, :] == idv[:B, None]) & ~diag)
+  if hard is not None:
+    top = torch.where(keep, l, torch.full_like(l, MIN_FLOAT)).masked_fill(diag, math.inf).topk(min(hard + 1, C), 1).indices
+    keep = keep & torch.zeros_like(keep).scatter_(1, top, True)
+  lse = torch.logsumexp(torch.where(keep, l, torch.full_like(l, -math.inf)), 1)
   # every head's bar (E) is below 1e-5 (max_h |q_ih|) . |c_j|; the scores themselves are exact here
-  E = 1e-5 * abs(inv_t) * (q64.abs().amax(1) @ c64.abs().T) + 2.0 ** -22 * l.abs()
+  E = 1e-5 * abs(inv_t) * (q64.abs().amax(1) @ c64.abs().T) + 2.0 ** -22 * (l.abs() + b64.abs()[None, :])
   eps = 2.0 ** -21 * chain + 2.0 ** -19 + 2.0 ** -22 * (lse.abs() + 1) + C * 2.0 ** -126
-  barL = E.max(1).values + eps
-  eye = torch.eye(B, C, dtype=F64, device=q3.device)
-  w64 = w.double()
-  loss = float((w64 * (lse - l.diagonal())).sum())
-  bar_loss = float((w64.abs() * (barL + E.diagonal()) + 2.0 ** -21 * (w64 * (lse - l.diagonal())).abs()).sum())
-  p = torch.exp(l - lse[:, None])
-  fac = w64 * inv_t
-  G = (p - eye) * fac[:, None]
-  dP = p * (torch.expm1(E + 2.0 ** -22 * (lse.abs()[:, None] + 10) + barL[:, None]) + 2.0 ** -21)
+  barL = torch.where(keep, E, torch.zeros_like(E)).max(1).values + eps
+  kii = keep.diagonal()
+  pos = torch.where(kii, l.diagonal(), torch.full_like(lse, MIN_FLOAT))
+  E_pos = torch.where(kii, E.diagonal(), torch.full_like(lse, 2.0 ** -22 * abs(MIN_FLOAT)))
+  w64 = torch.ones(B, dtype=F64, device=dev) if w is None else w.detach().double().reshape(-1)
+  loss = float((w64 * (lse - pos)).sum())
+  bar_loss = float((w64.abs() * (barL + E_pos) + 2.0 ** -21 * (w64 * (lse - pos)).abs()).sum())
+  p = torch.where(keep, torch.exp(l - lse[:, None]), torch.zeros_like(l))
+  fac = w64 * (float(g) * inv_t)
+  G = (p - (diag & keep).double()) * fac[:, None]
+  dP = torch.where(keep, p * (torch.expm1(E + 2.0 ** -22 * (lse.abs()[:, None] + 10) + barL[:, None]) + 2.0 ** -21),
+                   torch.zeros_like(p))
   Gh = G[:, None, :] * at                                  # [B, H, C]
   dPh = dP[:, None, :] * at * fac.abs()[:, None, None]
   dq = torch.einsum("bhc,cd->bhd", Gh, c64)
@@ -770,7 +787,8 @@ def _maxsim_reference(q3, c, inv_t, w, chain, rel):
   dc = torch.einsum("bhc,bhd->cd", Gh, q64)
   bar_dc = torch.einsum("bhc,bhd->cd", dPh + rel[1] * Gh.abs(), q64.abs())
   floor = 2.0 ** -36 * (float(Gh.abs().max()) * c64.abs().sum() + float(c64.abs().max()) * Gh.abs().sum())
-  return loss, bar_loss, lse, barL, dq, bar_dq + floor, dc, bar_dc + floor
+  out = (loss, bar_loss, lse, barL, dq, bar_dq + floor, dc, bar_dc + floor)
+  return out + (Gh,) if keep_g else out
 
 
 @gpu
