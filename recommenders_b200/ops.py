@@ -2236,6 +2236,47 @@ def layer_mask(x: torch.Tensor, mask=None) -> Optional[torch.Tensor]:
 
 
 # ------------------------------------------------------------------------------------------------
+# K19 / K20 recurrences: what ops.gru and ops.lstm share
+# ------------------------------------------------------------------------------------------------
+def _recurrence_shapes(name: str, x, kernel, recurrent_kernel, gates: int, max_units: int):
+  """The checks of x [B, T, D], recurrent_kernel [u, gates * u] and kernel [D, gates * u]; returns (B, T, D, u)."""
+  require_cuda(x, "inputs")
+  if x.dim() != 3:
+    raise ValueError(f"{name}: inputs must be [batch, timesteps, features], got shape {tuple(x.shape)}")
+  B, T, D = x.shape
+  if T == 0:
+    raise ValueError(f"{name}: the inputs have no time steps (T = 0)")
+  require_cuda(recurrent_kernel, "recurrent_kernel")
+  u = recurrent_kernel.shape[0] if recurrent_kernel.dim() == 2 else 0
+  if recurrent_kernel.dim() != 2 or recurrent_kernel.shape[1] != gates * u or u == 0:
+    raise ValueError(f"{name}: recurrent_kernel must be [units, {gates} * units], got {tuple(recurrent_kernel.shape)}")
+  if u > max_units:
+    raise ValueError(f"{name}: units = {u} is above the kernel's ceiling of {max_units}")
+  if tuple(kernel.shape) != (D, gates * u):
+    raise ValueError(f"{name}: kernel must be [{D}, {gates * u}], got {tuple(kernel.shape)}")
+  return B, T, D, u
+
+
+def _recurrence(name: str, recurrence, fwd, x, kernel, b_i, recurrent_kernel, operands, mask, return_sequences: bool):
+  """The mask, the K6 projection gx = x.W + b_i and the T steps: through the autograd Function `recurrence` when
+  anything needs a gradient, else one `fwd` launch that saves nothing.  `operands` are the cell's inputs after U (each
+  None or float32 contiguous).  Returns (output, *final states)."""
+  B, T, D = x.shape
+  if mask is not None and return_sequences:
+    raise NotImplementedError(f"{name}: a mask together with return_sequences=True is not supported")
+  m, mk = _mask_arg(mask, (B, T), name)
+  gx = dense(x.reshape(B * T, D), kernel, b_i).reshape(B, T, recurrent_kernel.shape[1])
+  U = f32c(recurrent_kernel, "recurrent_kernel")
+  operands = [f32c(t, what) if t is not None else None for t, what in operands]
+  rs = bool(return_sequences)
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, *operands)):
+    out = recurrence.apply(gx, U, *operands, m, mk, rs)
+    return out if rs else (out[0], *out)
+  seq, finals, _ = fwd(gx.detach(), U.detach(), *(None if t is None else t.detach() for t in operands), m, mk, rs, False)
+  return (seq if rs else finals[0], *finals)
+
+
+# ------------------------------------------------------------------------------------------------
 # K19 GRU recurrence: layers.GRU (reset_after=True); the input projection runs on K6
 # ------------------------------------------------------------------------------------------------
 GRU_MAX_UNITS = 2048   # TFRS_GRU_MAX_UNITS of include/tfrs_b200.h
@@ -2250,20 +2291,20 @@ def _gru_fwd(gx, U, b_r, h0, m, mk, return_sequences: bool, save: bool):
   gates, h_prev = (new(B, T, 4 * u), new(B, T, u)) if save else (None, None)
   check(lib().tfrs_gru_fwd_f32(ptr(gx), ptr(U), ptr(b_r), ptr(h0), ptr(m), mk, B, T, u, ptr(seq), ptr(h_last), ptr(gates),
                                ptr(h_prev), stream()), "gru_fwd")
-  return seq, h_last, gates, h_prev
+  return seq, (h_last,), (gates, h_prev)
 
 
 class _GRURecurrence(torch.autograd.Function):
-  """(out_seq, h_T) with return_sequences, else h_T alone, from gx = x.W + b_i [B, T, 3u]; differentiable in gx, U, b_r
+  """(out_seq, h_T) with return_sequences, else (h_T,), from gx = x.W + b_i [B, T, 3u]; differentiable in gx, U, b_r
   and h0."""
 
   @staticmethod
   def forward(ctx, gx, U, b_r, h0, m, mk, return_sequences):
-    seq, h_last, gates, h_prev = _gru_fwd(gx, U, b_r, h0, m, mk, return_sequences, True)
+    seq, finals, (gates, h_prev) = _gru_fwd(gx, U, b_r, h0, m, mk, return_sequences, True)
     ctx.save_for_backward(U, gates, h_prev, m)
     ctx.mk, ctx.return_sequences = mk, return_sequences
     ctx.set_materialize_grads(False)
-    return (seq, h_last) if return_sequences else h_last
+    return (seq, *finals) if return_sequences else finals
 
   @staticmethod
   def backward(ctx, *grads):
@@ -2298,37 +2339,14 @@ def gru(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, b
   (nonzero = kept): a masked step carries h unchanged.  gx = x.W + b_i is one K6 Dense call (ops.dense), the T steps are
   one K19 launch; the backward is K19's reverse launch plus K6's backward for the projection and for dU, db_r.
   Differentiable in x, all three weights and initial_state."""
-  require_cuda(x, "inputs")
-  if x.dim() != 3:
-    raise ValueError(f"gru: inputs must be [batch, timesteps, features], got shape {tuple(x.shape)}")
-  B, T, D = x.shape
-  if T == 0:
-    raise ValueError("gru: the inputs have no time steps (T = 0)")
-  require_cuda(recurrent_kernel, "recurrent_kernel")
-  u = recurrent_kernel.shape[0] if recurrent_kernel.dim() == 2 else 0
-  if recurrent_kernel.dim() != 2 or recurrent_kernel.shape[1] != 3 * u or u == 0:
-    raise ValueError(f"gru: recurrent_kernel must be [units, 3 * units], got {tuple(recurrent_kernel.shape)}")
-  if u > GRU_MAX_UNITS:
-    raise ValueError(f"gru: units = {u} is above the kernel's ceiling of {GRU_MAX_UNITS}")
-  if tuple(kernel.shape) != (D, 3 * u):
-    raise ValueError(f"gru: kernel must be [{D}, {3 * u}], got {tuple(kernel.shape)}")
+  B, T, D, u = _recurrence_shapes("gru", x, kernel, recurrent_kernel, 3, GRU_MAX_UNITS)
   if bias is not None and tuple(bias.shape) != (2, 3 * u):
     raise ValueError(f"gru: bias must be [2, {3 * u}] (reset_after=True), got {tuple(bias.shape)}")
   if initial_state is not None and tuple(initial_state.shape) != (B, u):
     raise ValueError(f"gru: initial_state must be [{B}, {u}], got {tuple(initial_state.shape)}")
-  if mask is not None and return_sequences:
-    raise NotImplementedError("gru: a mask together with return_sequences=True is not supported")
-  m, mk = _mask_arg(mask, (B, T), "gru")
-  gx = dense(x.reshape(B * T, D), kernel, None if bias is None else bias[0]).reshape(B, T, 3 * u)
-  U = f32c(recurrent_kernel, "recurrent_kernel")
-  b_r = None if bias is None else f32c(bias[1], "bias")
-  h0 = None if initial_state is None else f32c(initial_state, "initial_state")
-  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, b_r, h0)):
-    out = _GRURecurrence.apply(gx, U, b_r, h0, m, mk, bool(return_sequences))
-    return out if return_sequences else (out, out)
-  seq, h_last, _, _ = _gru_fwd(gx.detach(), U.detach(), None if b_r is None else b_r.detach(),
-                               None if h0 is None else h0.detach(), m, mk, bool(return_sequences), False)
-  return (seq if return_sequences else h_last), h_last
+  return _recurrence("gru", _GRURecurrence, _gru_fwd, x, kernel, None if bias is None else bias[0], recurrent_kernel,
+                     [(None if bias is None else bias[1], "bias"), (initial_state, "initial_state")], mask,
+                     return_sequences)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -2346,7 +2364,7 @@ def _lstm_fwd(gx, U, h0, c0, m, mk, return_sequences: bool, save: bool):
   gates, c_seq, h_prev = (new(B, T, 4 * u), new(B, T, u), new(B, T, u)) if save else (None, None, None)
   check(lib().tfrs_lstm_fwd_f32(ptr(gx), ptr(U), ptr(h0), ptr(c0), ptr(m), mk, B, T, u, ptr(seq), ptr(h_last),
                                 ptr(c_last), ptr(gates), ptr(c_seq), ptr(h_prev), stream()), "lstm_fwd")
-  return seq, h_last, c_last, gates, c_seq, h_prev
+  return seq, (h_last, c_last), (gates, c_seq, h_prev)
 
 
 class _LSTMRecurrence(torch.autograd.Function):
@@ -2355,11 +2373,11 @@ class _LSTMRecurrence(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, gx, U, h0, c0, m, mk, return_sequences):
-    seq, h_last, c_last, gates, c_seq, h_prev = _lstm_fwd(gx, U, h0, c0, m, mk, return_sequences, True)
+    seq, finals, (gates, c_seq, h_prev) = _lstm_fwd(gx, U, h0, c0, m, mk, return_sequences, True)
     ctx.save_for_backward(U, gates, c_seq, h_prev, c0, m)
     ctx.mk, ctx.return_sequences = mk, return_sequences
     ctx.set_materialize_grads(False)
-    return (seq, h_last, c_last) if return_sequences else (h_last, c_last)
+    return (seq, *finals) if return_sequences else finals
 
   @staticmethod
   def backward(ctx, *grads):
@@ -2394,20 +2412,7 @@ def lstm(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, 
   (nonzero = kept): a masked step carries h and c unchanged.  gx = x.W + b is one K6 Dense call (ops.dense), the T steps
   are one K20 launch; the backward is K20's reverse launch plus K6's backward for the projection and for dU.
   Differentiable in x, all three weights and both initial states."""
-  require_cuda(x, "inputs")
-  if x.dim() != 3:
-    raise ValueError(f"lstm: inputs must be [batch, timesteps, features], got shape {tuple(x.shape)}")
-  B, T, D = x.shape
-  if T == 0:
-    raise ValueError("lstm: the inputs have no time steps (T = 0)")
-  require_cuda(recurrent_kernel, "recurrent_kernel")
-  u = recurrent_kernel.shape[0] if recurrent_kernel.dim() == 2 else 0
-  if recurrent_kernel.dim() != 2 or recurrent_kernel.shape[1] != 4 * u or u == 0:
-    raise ValueError(f"lstm: recurrent_kernel must be [units, 4 * units], got {tuple(recurrent_kernel.shape)}")
-  if u > LSTM_MAX_UNITS:
-    raise ValueError(f"lstm: units = {u} is above the kernel's ceiling of {LSTM_MAX_UNITS}")
-  if tuple(kernel.shape) != (D, 4 * u):
-    raise ValueError(f"lstm: kernel must be [{D}, {4 * u}], got {tuple(kernel.shape)}")
+  B, T, D, u = _recurrence_shapes("lstm", x, kernel, recurrent_kernel, 4, LSTM_MAX_UNITS)
   if bias is not None and tuple(bias.shape) != (4 * u,):
     raise ValueError(f"lstm: bias must be [{4 * u}], got {tuple(bias.shape)}")
   h0 = c0 = None
@@ -2417,18 +2422,9 @@ def lstm(x: torch.Tensor, kernel: torch.Tensor, recurrent_kernel: torch.Tensor, 
     for name, s in zip(("h_0", "c_0"), initial_state):
       if tuple(s.shape) != (B, u):
         raise ValueError(f"lstm: initial_state {name} must be [{B}, {u}], got {tuple(s.shape)}")
-    h0, c0 = (f32c(s, "initial_state") for s in initial_state)
-  if mask is not None and return_sequences:
-    raise NotImplementedError("lstm: a mask together with return_sequences=True is not supported")
-  m, mk = _mask_arg(mask, (B, T), "lstm")
-  gx = dense(x.reshape(B * T, D), kernel, bias).reshape(B, T, 4 * u)
-  U = f32c(recurrent_kernel, "recurrent_kernel")
-  if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (gx, U, h0, c0)):
-    out = _LSTMRecurrence.apply(gx, U, h0, c0, m, mk, bool(return_sequences))
-    return out if return_sequences else (out[0], out[0], out[1])
-  seq, h_last, c_last, _, _, _ = _lstm_fwd(gx.detach(), U.detach(), None if h0 is None else h0.detach(),
-                                           None if c0 is None else c0.detach(), m, mk, bool(return_sequences), False)
-  return (seq if return_sequences else h_last), h_last, c_last
+    h0, c0 = (f32c(s, "initial_state") for s in initial_state)   # checked before the mask and the projection
+  return _recurrence("lstm", _LSTMRecurrence, _lstm_fwd, x, kernel, bias, recurrent_kernel,
+                     [(h0, "initial_state"), (c0, "initial_state")], mask, return_sequences)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -15,11 +15,11 @@ from recommenders_b200.layers.embedding import Embedding
 
 pytestmark = pytest.mark.gpu
 
-UNITS = [1, 2, 31, 32, 33, 64, 65, 127, 128, 129, 257, 512, 513, 600, 768, 769, 1024, 1025, ops.GRU_MAX_UNITS]
+SMEM_MAX = 227 * 1024
 
 
 def _row_tile(u):
-  """The batch rows of one CTA for u units (csrc/gru.cu gru_tile)."""
+  """The batch rows of one CTA for u units (csrc/rnn.cuh rnn_tile)."""
   jt = 32
   while jt < u and jt < 256:
     jt *= 2
@@ -27,6 +27,18 @@ def _row_tile(u):
   while uj * jt < u:
     uj *= 2
   return (256 // jt) * (8 // uj)
+
+
+def _resident_edges(smem_bytes):
+  """Every u after which the whole U (or U^T) stops or starts fitting in shared memory next to the step buffers
+  (csrc/rnn.cuh rnn_smem); not monotonic in u, since the row tile halves as u passes a power of two."""
+  return [u for u in range(1, ops.GRU_MAX_UNITS) if (smem_bytes(u) <= SMEM_MAX) != (smem_bytes(u + 1) <= SMEM_MAX)]
+
+
+FWD_EDGES = _resident_edges(lambda u: 4 * (2 * _row_tile(u) * u + u * 3 * u))              # h buffers + U
+BWD_EDGES = _resident_edges(lambda u: 4 * (2 * _row_tile(u) * 3 * u + 3 * u * (u + 1)))     # dgr buffers + U^T
+UNITS = sorted({1, 2, 31, 32, 33, 64, 65, 127, 128, 129, 257, 512, 513, 600, 768, 769, 1024, 1025, ops.GRU_MAX_UNITS}
+               | {e + d for e in FWD_EDGES + BWD_EDGES for d in (-1, 0, 1)})
 
 
 def _cu(a, grad=False):
@@ -91,6 +103,12 @@ def _run_case(B, T, D, u, bias=True, h0=True, mask=None, seq=None, seed=0, mask_
     _check("dbias", bt.grad, g["dbias"])
   if h0:
     _check("dh0", ht.grad, g["dh0"])
+
+
+def test_the_resident_boundaries_are_where_the_plan_says():
+  # U resident to u = 136; U^T resident to u = 123 and at u = 129, 130, where the row tile halves (DESIGN.md K19)
+  assert FWD_EDGES == [136] and BWD_EDGES == [123, 128, 130]
+  assert {122, 124, 127, 131, 135, 137} <= set(UNITS)
 
 
 @pytest.mark.parametrize("u", UNITS)

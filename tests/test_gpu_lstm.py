@@ -13,55 +13,14 @@ import recommenders_b200 as tfrs
 from recommenders_b200 import ops
 from recommenders_b200.data import Dataset
 from recommenders_b200.layers.embedding import Embedding
-from test_gpu_gru import _SequentialModel, _histories
+from test_gpu_gru import _SequentialModel, _check, _cu, _histories, _mask, _resident_edges, _row_tile
 
 pytestmark = pytest.mark.gpu
 
-SMEM_MAX = 227 * 1024
-
-
-def _row_tile(u):
-  """The batch rows of one CTA for u units (csrc/rnn.cuh rnn_tile)."""
-  jt = 32
-  while jt < u and jt < 256:
-    jt *= 2
-  uj = 1
-  while uj * jt < u:
-    uj *= 2
-  return (256 // jt) * (8 // uj)
-
-
-def _last_resident(smem_bytes):
-  """The largest u whose whole U (or U^T) fits in shared memory next to the step buffers (csrc/rnn.cuh rnn_smem)."""
-  u = 1
-  while smem_bytes(u + 1) <= SMEM_MAX:
-    u += 1
-  return u
-
-
-FWD_RESIDENT = _last_resident(lambda u: 4 * (2 * _row_tile(u) * u + u * 4 * u))              # h buffers + U
-BWD_RESIDENT = _last_resident(lambda u: 4 * (2 * _row_tile(u) * 4 * u + 4 * u * (u + 1)))     # dz buffers + U^T
-UNITS = sorted({1, 2, 31, 32, 33, 64, 65, 127, 128, 129, 257, ops.LSTM_MAX_UNITS,
+(FWD_RESIDENT,) = _resident_edges(lambda u: 4 * (2 * _row_tile(u) * u + u * 4 * u))              # h buffers + U
+(BWD_RESIDENT,) = _resident_edges(lambda u: 4 * (2 * _row_tile(u) * 4 * u + 4 * u * (u + 1)))     # dz buffers + U^T
+UNITS = sorted({1, 2, 31, 32, 33, 64, 65, 127, 128, 129, 257, 512, 513, 600, 768, 769, 1024, 1025, ops.LSTM_MAX_UNITS,
                 FWD_RESIDENT - 1, FWD_RESIDENT, FWD_RESIDENT + 1, BWD_RESIDENT - 1, BWD_RESIDENT, BWD_RESIDENT + 1})
-
-
-def _cu(a, grad=False):
-  return None if a is None else torch.from_numpy(np.ascontiguousarray(a)).cuda().requires_grad_(grad)
-
-
-def _mask(kind, B, T, rng):
-  if kind is None:
-    return None
-  if kind == "random":
-    m = rng.rand(B, T) < 0.6
-  elif kind == "leading":          # left padding: the first steps of each row are masked
-    m = np.arange(T)[None] >= rng.randint(0, T + 1, size=(B, 1))
-  elif kind == "trailing":         # right padding
-    m = np.arange(T)[None] < rng.randint(0, T + 1, size=(B, 1))
-  else:                            # "all": some rows entirely masked, the others random
-    m = rng.rand(B, T) < 0.5
-    m[::3] = False
-  return m
 
 
 def _inputs(B, T, D, u, bias, state, seed):
@@ -73,14 +32,6 @@ def _inputs(B, T, D, u, bias, state, seed):
   h = rng.uniform(-1, 1, size=(B, u)).astype(np.float32) if state else None
   c = rng.uniform(-2, 2, size=(B, u)).astype(np.float32) if state else None
   return rng, x, W, U, b, h, c
-
-
-def _check(name, got, exp):
-  got = got.detach().double().cpu().numpy() if isinstance(got, torch.Tensor) else got
-  scale = np.abs(exp).max() if exp.size else 0.0
-  err = np.abs(got - exp).max() if exp.size else 0.0
-  assert got.shape == exp.shape, (name, got.shape, exp.shape)
-  assert err <= 1e-5 * scale, f"{name}: max |error| {err:.3g} > 1e-5 * max |value| {scale:.3g}"
 
 
 def _run_case(B, T, D, u, bias=True, state=True, mask=None, seq=None, seed=0, mask_dtype=torch.bool, c_grad=True):
