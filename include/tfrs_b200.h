@@ -512,6 +512,30 @@ int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y, const flo
                        int N, int activation, float* dx, float* dW, float* dbias, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K27  1-D convolution (tf.keras.layers.Conv1D, channels_last, groups = 1):  x [B, T, C], W [k, C, F] (Keras layout),
+ * bias [F] nullable, stride s, dilation d, left pad p >= 0, T_out output steps, act = TFRS_ACT_*:
+ *   y [B, T_out, F]:  y[b, t, n] = act(bias[n] + sum_j sum_c x[b, t s + j d - p, c] W[j, c, n]),  x outside [0, T) reads 0.
+ * The caller maps Keras's padding to (p, T_out): "valid" p = 0, T_out = floor((T - d (k - 1) - 1) / s) + 1; "same"
+ * T_out = ceil(T / s), p = floor(max((T_out - 1) s + d (k - 1) + 1 - T, 0) / 2); "causal" T_out = ceil(T / s),
+ * p = d (k - 1).  Windows may read past either end of the sequence (the right pad is implied).
+ * This is the Dense layer (K6) on the im2col matrix col [B T_out, k C] with W viewed as [k C, F], on K6's route rule
+ * (tfrs_dense_uses_tc(B T_out, k C, F)).  Tensor cores: K6's split-fp16 GEMM and bias + activation epilogue, the A image
+ * gathered from x window by window (col is never formed; its power-of-two rescale is taken from max |x| over all of x).
+ * Otherwise col is gathered into the workspace and K6's exact CUDA-core kernels run on it.
+ * Backward from the saved OUTPUT y, as K6:  dz = dy * act'(y);  dbias = colsum(dz);  dW [k, C, F] = col^T . dz (the
+ * reduction over B T_out chunked by 1024 and summed in fixed order);  dx = col2im(dz . W^T): dx[b, t, c] is the sum over j
+ * ascending of the terms whose window reads (b, t, c).  dx / dW / dbias are nullable.  Deterministic, no float atomics.
+ * ws: tfrs_conv1d_fwd_workspace_bytes / tfrs_conv1d_bwd_workspace_bytes, 16-byte aligned.  B = 0 is a no-op forward.
+ * ------------------------------------------------------------------------------------------- */
+size_t tfrs_conv1d_fwd_workspace_bytes(int64_t B, int T_out, int C, int k, int F);
+int tfrs_conv1d_fwd_f32(const float* x, const float* W, const float* bias, int64_t B, int T, int C, int k, int F, int stride,
+                        int dilation, int pad, int T_out, int activation, float* y, void* ws, size_t ws_bytes, void* stream);
+size_t tfrs_conv1d_bwd_workspace_bytes(int64_t B, int T_out, int C, int k, int F);
+int tfrs_conv1d_bwd_f32(const float* x, const float* W, const float* y, const float* dy, int64_t B, int T, int C, int k, int F,
+                        int stride, int dilation, int pad, int T_out, int activation, float* dx, float* dW, float* dbias, void* ws,
+                        size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Ranking loss + metrics (tasks/ranking.py:26-119 with the tf.keras losses / metrics the tutorials pass).
  * One pass over the B predictions computes the per-example loss, the reduced loss (fixed-order reduction to a device
  * scalar) and, in the same launch, the batch statistics of the ranking metrics:

@@ -117,7 +117,12 @@ _SIGNATURES = {
     "tfrs_dense_fwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_i, c_p, c_p, c_p, c_sz, c_p]),
     "tfrs_dense_bwd_workspace_bytes": (c_sz, [c_l, c_i, c_i]),
     "tfrs_dense_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_p, c_l, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz, c_p]),
-    "tfrs_ranking_workspace_bytes": (c_sz, [c_l, c_i]),
+    "tfrs_conv1d_fwd_workspace_bytes": (c_sz, [c_l, c_i, c_i, c_i, c_i]),
+    "tfrs_conv1d_fwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
+    "tfrs_conv1d_bwd_workspace_bytes": (c_sz, [c_l, c_i, c_i, c_i, c_i]),
+    "tfrs_conv1d_bwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz,
+                                  c_p]),
+    "tfrs_ranking_workspace_bytes":(c_sz, [c_l, c_i]),
     "tfrs_ranking_loss_fwd_f32": (c_i, [c_p, c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p, c_f, c_i, c_p, c_sz, c_p]),
     "tfrs_ranking_loss_bwd_f32": (c_i, [c_p, c_p, c_p, c_l, c_i, c_i, c_p, c_p, c_p]),
     "tfrs_ranking_metrics_f32": (c_i, [c_p, c_p, c_p, c_l, c_p, c_f, c_i, c_p, c_sz, c_p]),

@@ -14,7 +14,7 @@ namespace tfrs {
 constexpr int DENSE_NARROW_N = 16;     // widest layer that runs the warp-per-row kernel
 constexpr int DENSE_COL_SPLITS = 64;   // row splits of the bias-gradient column sum
 
-static bool dense_tc(long long B, int K, int N) { return B >= 1024 && K >= 64 && N >= 64 && B < (1ll << 31); }
+bool dense_tc(long long B, int K, int N) { return B >= 1024 && K >= 64 && N >= 64 && B < (1ll << 31); }
 
 struct EpiDense {
   const float* bias; int act; long long ld; float* y; float* logits;
@@ -84,6 +84,24 @@ dense_colsum_reduce(const double* __restrict__ partial, int N, int splits, float
   out[n] = (float)a;
 }
 
+int dense_dz(const float* y, const float* dy, const float* dl, long long total, int act, float* dz, cudaStream_t st) {
+  dense_dz_kernel<<<elementwise_grid(total), 256, 0, st>>>(y, dy, dl, total, act, dz);
+  TFRS_LAUNCH_CHECK();
+  return TFRS_OK;
+}
+
+size_t dense_colsum_bytes(int N) { return (size_t)DENSE_COL_SPLITS * N * 8; }
+
+int dense_colsum(const float* dz, long long B, int N, double* colpart, float* out, cudaStream_t st) {
+  const long long rps = ceil_div(B, DENSE_COL_SPLITS);
+  const int used = (int)ceil_div(B, rps);
+  dense_colsum_partial<<<dim3((unsigned)ceil_div(N, 256), (unsigned)used), 256, 0, st>>>(dz, B, N, rps, colpart);
+  TFRS_LAUNCH_CHECK();
+  dense_colsum_reduce<<<(unsigned)ceil_div(N, 256), 256, 0, st>>>(colpart, N, used, out);
+  TFRS_LAUNCH_CHECK();
+  return TFRS_OK;
+}
+
 static size_t dense_bwd_gemm_ws(long long B, int K, int N) {
   if (dense_tc(B, K, N)) {
     const size_t a = tc::gemm_tc_workspace(B, K, N), b = tc::gemm_tc_workspace(K, N, B);
@@ -140,9 +158,8 @@ extern "C" int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y
   double* colpart = (double*)w; w += align_up((size_t)DENSE_COL_SPLITS * N * 8, 1024);
   const size_t gws = ws_bytes - (size_t)(w - (unsigned char*)ws);
   const long long total = (long long)B * N;
-  dense_dz_kernel<<<elementwise_grid(total), 256, 0, st>>>(y, dy, dlogits, total, activation, dz);
-  TFRS_LAUNCH_CHECK();
-  int rc;
+  int rc = dense_dz(y, dy, dlogits, total, activation, dz, st);
+  if (rc) return rc;
   if (dense_tc(B, K, N)) {
     const tc::GemmEpilogue plain{tc::GEMM_EPI_PLAIN, nullptr, 0, nullptr, 0, nullptr, 0.f, nullptr, 0};
     if (dx) {   // dx[b, i] = sum_o dz[b, o] W[i, o]
@@ -163,13 +180,6 @@ extern "C" int tfrs_dense_bwd_f32(const float* x, const float* W, const float* y
       if (rc) return rc;
     }
   }
-  if (dbias) {
-    const long long rps = ceil_div(B, DENSE_COL_SPLITS);
-    const int used = (int)ceil_div(B, rps);
-    dense_colsum_partial<<<dim3((unsigned)ceil_div(N, 256), (unsigned)used), 256, 0, st>>>(dz, B, N, rps, colpart);
-    TFRS_LAUNCH_CHECK();
-    dense_colsum_reduce<<<(unsigned)ceil_div(N, 256), 256, 0, st>>>(colpart, N, used, dbias);
-    TFRS_LAUNCH_CHECK();
-  }
+  if (dbias) return dense_colsum(dz, B, N, colpart, dbias, st);
   return TFRS_OK;
 }

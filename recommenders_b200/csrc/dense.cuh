@@ -1,5 +1,5 @@
 // dense.cuh -- activations of the Dense layer (K6), shared by the exact kernels (dense.cu) and the DENSE epilogues of the
-// split-fp16 tensor-core GEMM (split_gemm.cu).
+// split-fp16 tensor-core GEMM (split_gemm.cu); and the steps of K6's backward that the 1-D convolution (K27) shares.
 #pragma once
 #include "common.cuh"
 
@@ -19,5 +19,14 @@ __device__ __forceinline__ float dense_act_grad(int act, float y, float g) {
   if (act == TFRS_ACT_SIGMOID) return g * y * (1.f - y);
   return g;
 }
+
+// K6's route rule: the split-fp16 tensor-core GEMM for a [B, K] . [K, N] product when true, the exact CUDA-core kernels else
+bool dense_tc(long long B, int K, int N);
+// dz = dy * act'(y) + dl over `total` elements (dy or dl nullable), one launch
+int dense_dz(const float* y, const float* dy, const float* dl, long long total, int act, float* dz, cudaStream_t st);
+// out[n] = sum over the B rows of dz [B, N], in float64 and a fixed order: row splits summed into colpart
+// (dense_colsum_bytes(N) bytes), then folded in split order; two launches
+size_t dense_colsum_bytes(int N);
+int dense_colsum(const float* dz, long long B, int N, double* colpart, float* out, cudaStream_t st);
 
 }  // namespace tfrs

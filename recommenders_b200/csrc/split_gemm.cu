@@ -1,5 +1,6 @@
 // split_gemm.cu -- the split-fp16 tensor-core GEMM:  C[M,N] = A'[M,K] . B'[N,K]^T  with a fused epilogue.  It runs the
-// full-rank and low-rank Cross layers (K5, forward and backward), the Dense layer (K6) and tfrs_gemm_tc_f32.
+// full-rank and low-rank Cross layers (K5, forward and backward), the Dense layer (K6), the 1-D convolution (K27, whose A
+// operand is gathered from the input's time windows) and tfrs_gemm_tc_f32.
 //
 // fp32 parity on fp16 tensor cores: each operand is rescaled by an exact power of two and split into
 //   v = hi + lo,  hi = fp16(v), lo = fp16(v - hi)            (|v - hi - lo| <= 2^-22 |v|)
@@ -193,6 +194,42 @@ static int sg_launch(int mode, const SgParams& p, cudaStream_t st) {
   return TFRS_OK;
 }
 
+// ---- K27: the im2col operand of a 1-D convolution, gathered from x while its image is written ------------------------------
+// K27's A operand: the im2col rows of x gathered straight into the image
+static __global__ void __launch_bounds__(256)
+cx_window_image_kernel(const WindowSrc src, long long rows, int K, int kb, long long n_tiles, const CxStats* __restrict__ st,
+                       unsigned char* __restrict__ img) {
+  split_image_rows(src, rows, K, kb, n_tiles, st, img);
+}
+
+// K27's colT operand (the weight gradient's A): image row = im2col column kk, reduction index = im2col row r
+static __global__ void __launch_bounds__(256)
+cx_window_image_t_kernel(const WindowSrc src, long long K, int M, int kb_total, const CxStats* __restrict__ st,
+                         unsigned char* __restrict__ img) {
+  split_image_cols(src, K, M, kb_total, st, img);
+}
+
+// The split image of the im2col matrix `win` describes ([B * T_out, k * C]), or of its transpose, as split_image does for a
+// stored matrix.  The exponent is taken from max |x| over all of x: every image element is an element of x or 0, so that
+// max bounds the image's (no fp16 overflow), and equals it whenever the windows cover every position of x (stride 1).
+static inline int split_image_windows(const WindowSrc& win, bool transposed, long long rows, long long K, int kb,
+                                      long long n_tiles, CxStats* st, unsigned char* img, cudaStream_t s) {
+  const long long bt = (transposed ? K : rows) / win.T_out * (long long)win.T;   // the B * T rows of x
+  cx_amax_kernel<<<cx_amax_grid(bt), 256, 0, s>>>(win.x, bt, win.C, win.C, st);
+  TFRS_LAUNCH_CHECK();
+  cx_exp_kernel<<<1, 1, 0, s>>>(st);
+  TFRS_LAUNCH_CHECK();
+  if (transposed) {
+    cx_window_image_t_kernel<<<dim3((unsigned)kb, (unsigned)n_tiles), 256, 0, s>>>(win, K, (int)rows, kb, st, img);
+  } else {
+    const long long chunks = n_tiles * 128 * (long long)kb * 8;
+    const unsigned g = (unsigned)(ceil_div(chunks, 256) < (1 << 20) ? ceil_div(chunks, 256) : (1 << 20));
+    cx_window_image_kernel<<<g, 256, 0, s>>>(win, rows, (int)K, kb, n_tiles, st, img);
+  }
+  TFRS_LAUNCH_CHECK();
+  return TFRS_OK;
+}
+
 // ---- the driver: operand images, then one launch (plus the partials' reduction when chunked) ------------------------------
 struct GtPlan { int n_mb, n_nt, kb, n_kc; size_t o_st, o_aimg, o_bimg, o_partial, total; };
 static void gt_plan(long long M, long long N, long long K, GtPlan& pl) {
@@ -272,7 +309,8 @@ int gemm_tc(const GemmOperand& A, const GemmOperand& Bop, long long M, long long
   unsigned char* w8 = (unsigned char*)ws;
   CxStats* ast = (CxStats*)(w8 + pl.o_st); CxStats* bst = (CxStats*)(w8 + pl.o_st + 1024);
   TFRS_CUDA(cudaMemsetAsync(w8 + pl.o_st, 0, 2048, st));
-  int rc = split_image(A.ptr, A.ld, A.transposed, A.amax_bits, M, K, pl.kb, (long long)pl.n_mb * 2, ast, w8 + pl.o_aimg, st);
+  int rc = A.win ? split_image_windows(*A.win, A.transposed, M, K, pl.kb, (long long)pl.n_mb * 2, ast, w8 + pl.o_aimg, st)
+                 : split_image(A.ptr, A.ld, A.transposed, A.amax_bits, M, K, pl.kb, (long long)pl.n_mb * 2, ast, w8 + pl.o_aimg, st);
   if (rc) return rc;
   rc = split_image(Bop.ptr, Bop.ld, Bop.transposed, Bop.amax_bits, N, K, pl.kb, pl.n_nt, bst, w8 + pl.o_bimg, st);
   if (rc) return rc;

@@ -51,11 +51,20 @@ static __global__ void cx_exp_kernel(CxStats* st) {
   st->exp = ok ? (CX_TARGET_EXP - x) : 0;
 }
 
-// fp32 [rows, K] (row stride ld) -> hi/lo fp16 tile image:
+// Where an image's elements come from: element (i, j) of an fp32 matrix, at(i, j) as a plain load and at_ldg(i, j) through
+// the read-only path.  MatrixSrc is a stored row-major matrix with row stride ld; split_gemm.cuh's WindowSrc is the im2col
+// matrix of a 1-D convolution, gathered from its input.
+struct MatrixSrc {
+  const float* p; long long ld;
+  __device__ __forceinline__ float at(long long i, long long j) const { return p[i * ld + j]; }
+  __device__ __forceinline__ float at_ldg(long long i, long long j) const { return __ldg(p + i * ld + j); }
+};
+
+// fp32 [rows, K] -> hi/lo fp16 tile image:
 //   tile t (128 rows) : slab s (64 K) : {hi, lo} : 128 rows x 128 B, 16-byte chunk j of row r at chunk j ^ (r & 7)
-static __global__ void __launch_bounds__(256)
-cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long long ld, int kb, long long n_tiles,
-                      const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
+template <class Src>
+__device__ __forceinline__ void split_image_rows(const Src& src, long long rows, int K, int kb, long long n_tiles,
+                                                 const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
   const int sexp = st->exp;
   const long long total = n_tiles * 128 * (long long)kb * 8;
   const unsigned int cpr = (unsigned int)(kb * 8);  // 16-byte chunks per row
@@ -72,7 +81,7 @@ cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       float f = 0.f;
-      if (row < rows && k0 + j < K) f = src[row * ld + k0 + j];
+      if (row < rows && k0 + j < K) f = src.at(row, k0 + j);
       const float v = ldexpf(f, sexp);
       const __half h = __float2half_rn(v);
       hi[j] = h;
@@ -83,13 +92,17 @@ cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long
     *reinterpret_cast<uint4*>(dst + 16384) = *reinterpret_cast<const uint4*>(lo);
   }
 }
-
-// fp32 src [K, M] (row stride ld)  ->  hi/lo fp16 image of src^T: image rows = columns m of src, reduction index = rows
-// k of src.  One CTA per (64-row K slab, 128-column tile): coalesced 512-byte row reads, transpose through shared
-// memory, 128-byte swizzled row writes.
 static __global__ void __launch_bounds__(256)
-cx_split_image_t_kernel(const float* __restrict__ src, long long K, int M, long long ld, int kb_total,
-                        const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
+cx_split_image_kernel(const float* __restrict__ src, long long rows, int K, long long ld, int kb, long long n_tiles,
+                      const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
+  split_image_rows(MatrixSrc{src, ld}, rows, K, kb, n_tiles, st, img);
+}
+// fp32 src [K, M]  ->  hi/lo fp16 image of src^T: image rows = columns m of src, reduction index = rows k of src.  One
+// CTA per (64-row K slab, 128-column tile): coalesced 512-byte row reads, transpose through shared memory, 128-byte
+// swizzled row writes.
+template <class Src>
+__device__ __forceinline__ void split_image_cols(const Src& src, long long K, int M, int kb_total, const CxStats* __restrict__ st,
+                                                 unsigned char* __restrict__ img) {
   __shared__ float tile[64][129];
   const int ks = blockIdx.x, mt = blockIdx.y;
   // v * 2^exp as two exact power-of-two factors: 2^exp alone overflows when exp > 127 (max |element| < 2^-113), and exp >= -114
@@ -100,7 +113,7 @@ cx_split_image_t_kernel(const float* __restrict__ src, long long K, int M, long 
   for (int e = threadIdx.x; e < 64 * 128; e += 256) {
     const int kk = e >> 7, mm = e & 127;
     const long long k = (long long)ks * 64 + kk; const int m = mt * 128 + mm;
-    const float f = (k < K && m < M) ? __ldg(src + k * ld + m) : 0.f;
+    const float f = (k < K && m < M) ? src.at_ldg(k, m) : 0.f;
     tile[kk][mm] = f * sc1 * sc2;
   }
   __syncthreads();
@@ -122,7 +135,11 @@ cx_split_image_t_kernel(const float* __restrict__ src, long long K, int M, long 
     *reinterpret_cast<uint4*>(dst + 16384) = *reinterpret_cast<const uint4*>(lo);
   }
 }
-
+static __global__ void __launch_bounds__(256)
+cx_split_image_t_kernel(const float* __restrict__ src, long long K, int M, long long ld, int kb_total,
+                        const CxStats* __restrict__ st, unsigned char* __restrict__ img) {
+  split_image_cols(MatrixSrc{src, ld}, K, M, kb_total, st, img);
+}
 // The split image of one operand, three launches: max |element| into st (a pass over the operand, or a copy of the caller's
 // amax_bits when it already knows it), the exponent, then the hi/lo image of n_tiles 128-row tiles x kb K slabs.
 // Element (image row r, reduction index k) = transposed ? src[k * ld + r] : src[r * ld + k], for r < rows and k < K; the

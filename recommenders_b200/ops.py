@@ -1749,6 +1749,110 @@ def attached_logits(pred: torch.Tensor) -> Optional[torch.Tensor]:
 
 
 # ------------------------------------------------------------------------------------------------
+# K27 1-D convolution (layers.Conv1D): K6 on the im2col windows of x
+# ------------------------------------------------------------------------------------------------
+CONV1D_PADDINGS = ("valid", "same", "causal")
+
+
+def conv1d_geometry(T: int, k: int, strides: int = 1, padding: str = "valid", dilation_rate: int = 1, name: str = "conv1d",
+                    input_shape=None):
+  """(T_out, left pad) of tf-keras's Conv1D over T steps: "valid" reads no padding, T_out = floor((T - d (k - 1) - 1) / s) +
+  1, and raises ValueError when T < d (k - 1) + 1; "same" has T_out = ceil(T / s) and the total pad max((T_out - 1) s +
+  d (k - 1) + 1 - T, 0), of which the left gets half rounded down (TF's rule); "causal" pads d (k - 1) on the left only,
+  T_out = ceil(T / s)."""
+  if padding not in CONV1D_PADDINGS:
+    raise ValueError(f"{name}: padding must be one of {CONV1D_PADDINGS}, got {padding!r}")
+  span = dilation_rate * (k - 1) + 1
+  if padding == "valid":
+    if T < span:
+      shape = tuple(input_shape) if input_shape is not None else ("batch", T, "channels")
+      raise ValueError(f"One of the dimensions in the output is <= 0 due to downsampling in {name}. Consider increasing the "
+                       f"input size. Received input shape {shape} which would produce output shape with a zero or negative "
+                       f"value in a dimension.")
+    return (T - span) // strides + 1, 0
+  T_out = -(-T // strides)
+  if padding == "same":
+    return T_out, max((T_out - 1) * strides + span - T, 0) // 2
+  return T_out, span - 1
+
+
+def _conv1d_fwd(x, W, b, geo, act):
+  B, T, C = x.shape
+  k, _, F = W.shape
+  s, d, p, T_out = geo
+  y = torch.empty((B, T_out, F), dtype=torch.float32, device=x.device)
+  if B:
+    ws = workspace(max(lib().tfrs_conv1d_fwd_workspace_bytes(B, T_out, C, k, F), 256), x.device, "conv1d")
+    check(lib().tfrs_conv1d_fwd_f32(ptr(x), ptr(W), ptr(b), B, T, C, k, F, s, d, p, T_out, act, ptr(y), ptr(ws), ws.numel(),
+                                    stream()), "conv1d_fwd")
+  return y
+
+
+class _Conv1D(torch.autograd.Function):
+  """act(conv1d(x, W) + bias) with x [B, T, C], W [k, C, F]; the backward works from the saved OUTPUT y, as K6's."""
+
+  @staticmethod
+  def forward(ctx, x, W, bias, act, geo):
+    y = _conv1d_fwd(x, W, bias, geo, act)
+    ctx.save_for_backward(x, W, y)
+    ctx.act, ctx.geo, ctx.has_bias = act, geo, bias is not None
+    return y
+
+  @staticmethod
+  def backward(ctx, gy):
+    x, W, y = ctx.saved_tensors
+    B, T, C = x.shape
+    k, _, F = W.shape
+    s, d, p, T_out = ctx.geo
+    n0, n1, n2 = ctx.needs_input_grad[:3]
+    dx = torch.empty_like(x) if n0 else None
+    dW = torch.empty_like(W) if n1 else None
+    db = torch.empty((F,), dtype=torch.float32, device=x.device) if (n2 and ctx.has_bias) else None
+    if B == 0:
+      for t in (dx, dW, db):
+        if t is not None:
+          t.zero_()
+      return dx, dW, db, None, None
+    gy = f32c(gy, "grad")
+    ws = workspace(lib().tfrs_conv1d_bwd_workspace_bytes(B, T_out, C, k, F), x.device, "conv1d_bwd")
+    check(lib().tfrs_conv1d_bwd_f32(ptr(x), ptr(W), ptr(y), ptr(gy), B, T, C, k, F, s, d, p, T_out, ctx.act, ptr(dx), ptr(dW),
+                                    ptr(db), ptr(ws), ws.numel(), stream()), "conv1d_bwd")
+    return dx, dW, db, None, None
+
+
+def conv1d_uses_tc(B: int, T_out: int, C: int, k: int, filters: int) -> bool:
+  """Whether a 1-D convolution runs on tensor cores: K6's rule on the im2col GEMM (B T_out, k C, filters)."""
+  return dense_uses_tc(B * T_out, k * C, filters)
+
+
+def conv1d(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor] = None, strides: int = 1, padding: str = "valid",
+           dilation_rate: int = 1, activation: Optional[str] = None) -> torch.Tensor:
+  """tf.keras.layers.Conv1D's arithmetic: x [B, T, C] float32 (CUDA), kernel W [k, C, filters], bias [filters] ->
+  act(bias[n] + sum_j sum_c x[b, t s + j d - p, c] W[j, c, n]) of shape [B, T_out, filters], positions outside [0, T)
+  reading 0; (T_out, p) from `padding` as `conv1d_geometry` says.  activation None / "linear" / "relu" / "sigmoid" run
+  fused.  One K27 call each way (include/tfrs_b200.h), differentiable in x, W and bias."""
+  if activation not in DENSE_ACTIVATIONS:
+    raise ValueError(f"conv1d: activation {activation!r} is not fused (use None and apply it afterwards)")
+  x = f32c(x, "inputs"); W = f32c(W, "kernel")
+  b = None if bias is None else f32c(bias, "bias")
+  if x.dim() != 3:
+    raise ValueError(f"conv1d: inputs must be [batch, steps, channels], got shape {tuple(x.shape)}")
+  B, T, C = x.shape
+  if W.dim() != 3 or W.shape[1] != C or W.shape[0] == 0 or W.shape[2] == 0:
+    raise ValueError(f"conv1d: kernel must be [kernel_size, {C}, filters], got {tuple(W.shape)}")
+  k, _, F = W.shape
+  if b is not None and b.numel() != F:
+    raise ValueError(f"conv1d: bias must have {F} entries, got {b.numel()}")
+  for arg, v in (("strides", strides), ("dilation_rate", dilation_rate)):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v <= 0:
+      raise ValueError(f"conv1d: {arg} must be a positive integer, got {v!r}")
+  if T == 0 or C == 0:
+    raise ValueError(f"conv1d: the inputs have no time steps or channels, shape {tuple(x.shape)}")
+  T_out, p = conv1d_geometry(T, k, int(strides), padding, int(dilation_rate), input_shape=tuple(x.shape))
+  return _Conv1D.apply(x, W, b, DENSE_ACTIVATIONS[activation], (int(strides), int(dilation_rate), p, T_out))
+
+
+# ------------------------------------------------------------------------------------------------
 # ranking loss + metrics
 # ------------------------------------------------------------------------------------------------
 LOSS_BCE, LOSS_BCE_LOGITS, LOSS_MSE = 0, 1, 2
